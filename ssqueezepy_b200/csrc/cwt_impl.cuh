@@ -266,35 +266,51 @@ static int launch_sblk_fwd(const SblkArgs<T>& S, cudaStream_t st) {
   SSQB_LAUNCH_CHECK();
   return 0;
 }
+// How a launch of the short-block rows shares the GPU.  Alone, it is a persistent grid of as
+// many CTAs as fit, walking the items in steps of its width.  Next to the gridded interpolation
+// (HBM-bound, SMs mostly waiting) it takes its items from a counter and one CTA per SM at the
+// highest stream priority, so that its CTAs are placed first and the interpolation's short CTAs
+// fill the rest of each SM; a TAIL launch of one CTA per SM, queued after the interpolation, then
+// draws from the same counter so that the rows do not finish at half width once the
+// interpolation has drained.
+enum SblkShare { SBLK_ALONE, SBLK_BESIDE_GRID, SBLK_TAIL };
+
 template <typename T, int NARR, bool SSQ>
-static int launch_sblk_rows_t(const SblkArgs<T>& S, cudaStream_t st) {
+static int launch_sblk_rows_t(const SblkArgs<T>& S, SblkShare share, cudaStream_t st) {
   constexpr int LP = SblkGeom<T>::LOG_P;
   using V4 = typename V4T<T>::type;
   size_t smem = ((size_t)1 << LP) * (sizeof(V4) + sizeof(cx<T>));
   auto kern = sblk_rows_kernel<T, LP, NARR, SSQ>;
   static bool attr_set = false;
-  static int ctas = 2 * 132;
+  static int sms = 132, per = 2, prio_high = 0;
   if (!attr_set) {
     SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int dev = 0, sms = 132, per = 2;
+    int dev = 0, least = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kern, (1 << LP) / 8, smem) != cudaSuccess || per < 1) per = 1;
-    ctas = sms * per;
+    SSQB_CUDA(cudaDeviceGetStreamPriorityRange(&least, &prio_high));
     attr_set = true;
   }
-  long long items = S.B * (long long)S.n_rows * S.nblk;
-  unsigned g = (unsigned)(items < ctas ? items : ctas);
+  const long long items = S.B * (long long)S.n_rows * S.nblk;
+  if (items > 0x7fffffffll) return set_error(SSQB_E_UNSUPP, "too many short-block items");
+  const long long ctas = (share == SBLK_ALONE) ? (long long)sms * per : sms;
+  const unsigned g = (unsigned)(items < ctas ? items : ctas);
   if (g < 1) return 0;
-  kern<<<g, (1 << LP) / 8, smem, st>>>(S);
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(g); cfg.blockDim = dim3((1 << LP) / 8); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributePriority; attr[0].val.priority = prio_high;
+  cfg.attrs = attr; cfg.numAttrs = (share == SBLK_BESIDE_GRID) ? 1 : 0;
+  SSQB_CUDA(cudaLaunchKernelEx(&cfg, kern, S));
   SSQB_LAUNCH_CHECK();
   return 0;
 }
 template <typename T>
-static int launch_sblk_rows(const SblkArgs<T>& S, int narr, bool ssq, cudaStream_t st) {
-  if (narr == 2 && ssq) return launch_sblk_rows_t<T, 2, true>(S, st);
-  if (narr == 2) return launch_sblk_rows_t<T, 2, false>(S, st);
-  return launch_sblk_rows_t<T, 1, false>(S, st);
+static int launch_sblk_rows(const SblkArgs<T>& S, int narr, bool ssq, SblkShare share, cudaStream_t st) {
+  if (narr == 2 && ssq) return launch_sblk_rows_t<T, 2, true>(S, share, st);
+  if (narr == 2) return launch_sblk_rows_t<T, 2, false>(S, share, st);
+  return launch_sblk_rows_t<T, 1, false>(S, share, st);
 }
 
 // ---- gridded narrow-band rows (cwt_grid.cuh) ------------------------------------------
@@ -551,6 +567,8 @@ struct CwtPlan : public CwtPlanBase {
   };
   SblkClass sblk[SBLK_NCLS];
   bool have_sblk = false, have_cut = false;
+  DevBuf<unsigned> sblk_ctr_d;                // per class: item counter of its row launches
+  cudaEvent_t ev_sblk_ready[SBLK_NCLS] = {nullptr, nullptr, nullptr};   // counter zeroed, spectra ready
   DevBuf<cx<T>> rootsP_d, twsP_d, xa_d, Gxa_d;
   DevBuf<T> ctab_d;
   DevBuf<long long> xa_lo_d, xa_len_d;
@@ -599,6 +617,7 @@ struct CwtPlan : public CwtPlanBase {
     if (copy_st) cudaStreamDestroy(copy_st);
     if (ev_done) cudaEventDestroy(ev_done);
     for (int i = 0; i < 2; ++i) if (ev_sa[i]) cudaEventDestroy(ev_sa[i]);
+    for (int i = 0; i < SBLK_NCLS; ++i) if (ev_sblk_ready[i]) cudaEventDestroy(ev_sblk_ready[i]);
   }
   // optional per-kernel timing (bench.py roofline): CUDA events on the launch stream
   bool profiling = false;
@@ -858,6 +877,9 @@ struct CwtPlan : public CwtPlanBase {
       SSQB_CUDA(K.pd_d.ensure(K.rows.size() * (size_t)Pn));
     }
     if (!have_sblk) return 0;
+    SSQB_CUDA(sblk_ctr_d.ensure(SBLK_NCLS));
+    for (int c = 0; c < SBLK_NCLS; ++c)
+      if (!ev_sblk_ready[c]) SSQB_CUDA(cudaEventCreateWithFlags(&ev_sblk_ready[c], cudaEventDisableTiming));
     SSQB_CUDA(rootsP_d.upload(make_roots<T>(Pn, 1, Pn)));
     {
       // per-stage twiddles of sblk_rows_kernel: stage Ns (radix r) at Ns - 8, [q - 1][k]
@@ -1253,7 +1275,8 @@ struct CwtPlan : public CwtPlanBase {
       graphs_ok = false;
       return exec_impl(xv, B, Wxv, dWxv, Txv, ssq, out_mul_host, rpadded, st);
     }
-    e = cudaGraphInstantiate(&gexec, g, 0);
+    // per-node priorities: the short-block launches beside the interpolation keep theirs
+    e = cudaGraphInstantiate(&gexec, g, cudaGraphInstantiateFlagUseNodePriority);
     cudaGraphDestroy(g);
     if (e != cudaSuccess) {
       cudaGetLastError(); gexec = nullptr; graphs_ok = false;
@@ -1291,9 +1314,10 @@ struct CwtPlan : public CwtPlanBase {
     long long target, smin = 1;
     if (env > 0) target = env;
     else {
-      // measured on H100 SXM at a 400 W power limit (GMW, 300 scales, N = 160 000, median of 3
-      // runs of 20 steps): B = 32: one group 16.6 ms, groups of 16 / 8 / 4: 16.9 / 16.9 / 16.7 ms;
-      // B = 8: 4.12 ms, groups of 4 / 2: 4.06 / 4.17 ms -- all within the run-to-run spread (~1 ms)
+      // measured on H100 SXM at a 700 W power limit (GMW, 300 scales, N = 160 000, windows of 5
+      // steps, tools/time_groups.py), with the short-block rows running beside the interpolation:
+      // B = 32: one group 14.13 ms, groups of 16 / 8 / 4: 13.32-13.33 / 13.25-13.32 / 13.64 ms;
+      // two windows of the same size differ by up to 0.07 ms, so 8 and 16 are equal
       target = (B >= 32) ? 8 : B / 2;
       // a group must stream enough output to amortise its own launches and tails (>= 128 MB of Tx)
       const double plane = (double)d.na * (double)d.N * (double)sizeof(cx<T>);
@@ -1435,16 +1459,30 @@ struct CwtPlan : public CwtPlanBase {
       }
       return s;
     };
-    auto least_loaded = [&](int first) -> int {
+    auto least_loaded = [&](int first, int last) -> int {
       int k = first;
-      for (int i = first + 1; i <= (lanes_on ? NLANES : 0); ++i) if (load[i] < load[k]) k = i;
+      for (int i = first + 1; i <= (lanes_on ? last : 0); ++i) if (load[i] < load[k]) k = i;
       return k;
     };
+    // With gridded rows, all block rows go to lane 1 and the short-block launches there run
+    // next to the interpolation (SblkShare); stage A of the gridded rows uses lanes 2 and 3.
+    // Batched float32 calls only.  For one signal the launches are short, and the counter resets
+    // and tail launches cost more than the overlap returns (C2, 400 W H100: 0.512 against
+    // 0.507 ms per step); float64 gains nothing side by side (C5: 20.75 against 20.71 ms).
+    const bool sblk_beside = lanes_on && have_grid_rows && sizeof(T) == 4 && B >= 2;
+    const int blk_last = sblk_beside ? 1 : NLANES;
+    std::vector<int> sblk_tails;                             // classes launched beside the grid
+    auto sblk_rows_args = [&](SblkArgs<T>& S, int c) {
+      sblk_args(S, sblk[c], B);
+      S.A.Wx = Wx; S.A.dWx = dWx; S.A.Tx = Tx; S.A.Nout = Nout; S.A.out_mul = out_mul;
+      S.write_dWx = dWx ? 1 : 0;
+      S.item_ctr = sblk_beside ? sblk_ctr_d.p + c : nullptr;   // alone: fixed stride, no counter
+    };
     struct Job { double w; FastArgs<T> P; int cls; int le; long long gb; long long rows; int sblk_cls; };
-    auto run_jobs = [&](std::vector<Job>& jobs, bool need_xh, int first) -> int {
+    auto run_jobs = [&](std::vector<Job>& jobs, bool need_xh, int first, int last) -> int {
       std::sort(jobs.begin(), jobs.end(), [](const Job& a, const Job& b) { return a.w > b.w; });
       for (const Job& J : jobs) {
-        const int k = lanes_on ? least_loaded(first) : 0;
+        const int k = lanes_on ? least_loaded(first, last) : 0;
         load[k] += J.w;
         cudaStream_t ls = acquire(k, need_xh);
         int r2 = 0;
@@ -1452,12 +1490,15 @@ struct CwtPlan : public CwtPlanBase {
           r2 = analytic(B, ls); if (r2) return r2;
           r2 = sblk_forward(sblk[J.sblk_cls], x, B, ls); if (r2) return r2;
         }
+        if (J.sblk_cls >= 0 && sblk_beside) {
+          SSQB_CUDA(cudaMemsetAsync(sblk_ctr_d.p + J.sblk_cls, 0, sizeof(unsigned), ls));
+          SSQB_CUDA(cudaEventRecord(ev_sblk_ready[J.sblk_cls], ls));
+          sblk_tails.push_back(J.sblk_cls);
+        }
         r2 = prof_begin(2, J.rows, ls); if (r2) return r2;
         if (J.sblk_cls >= 0) {
-          SblkArgs<T> S; sblk_args(S, sblk[J.sblk_cls], B);
-          S.A.Wx = Wx; S.A.dWx = dWx; S.A.Tx = Tx; S.A.Nout = Nout; S.A.out_mul = out_mul;
-          S.write_dWx = dWx ? 1 : 0;
-          r2 = launch_sblk_rows<T>(S, narr, ssq, ls);
+          SblkArgs<T> S; sblk_rows_args(S, J.sblk_cls);
+          r2 = launch_sblk_rows<T>(S, narr, ssq, sblk_beside ? SBLK_BESIDE_GRID : SBLK_ALONE, ls);
         } else {
           r2 = launch_direct<T>(J.P, J.cls, J.le, narr, J.gb, ls);
         }
@@ -1501,7 +1542,7 @@ struct CwtPlan : public CwtPlanBase {
       }
     }
     if (lanes_on && !bjobs.empty()) {
-      rc = run_jobs(bjobs, false, 1); if (rc) return rc;       // lanes only: st does the FFT
+      rc = run_jobs(bjobs, false, 1, blk_last); if (rc) return rc;   // lanes only: st does the FFT
       bjobs.clear();
     }
 
@@ -1544,7 +1585,7 @@ struct CwtPlan : public CwtPlanBase {
     if (two_pass_rows > 0) {
       cudaStream_t ts = st;
       int tk = 0;
-      if (lanes_on) { tk = least_loaded(1); load[tk] += 3.0 * (double)two_pass_rows; ts = acquire(tk, true, false); }
+      if (lanes_on) { tk = least_loaded(sblk_beside ? 2 : 1, NLANES); load[tk] += 3.0 * (double)two_pass_rows; ts = acquire(tk, true, false); }
       long long chunk = rows_per_chunk(narr, two_pass_rows);
       SSQB_CUDA(ensure_scratch(narr, chunk));
       for (long long r0 = 0; r0 < two_pass_rows; r0 += chunk) {
@@ -1599,11 +1640,22 @@ struct CwtPlan : public CwtPlanBase {
         Job J; memset(&J.P, 0, sizeof(J.P));
         J.cls = 0; J.le = 0; J.gb = 0; J.rows = B * (long long)sblk[2].rows.size();
         J.w = (double)J.rows * 0.9; J.sblk_cls = 2;
-        jobs.push_back(J);
+        if (sblk_beside) {                               // behind the plain classes on lane 1
+          std::vector<Job> cut(1, J);
+          rc = run_jobs(cut, true, 1, 1); if (rc) return rc;
+        } else {
+          jobs.push_back(J);
+        }
       }
     }
     for (const Job& J : bjobs) jobs.push_back(J);        // lanes off: blocks run here
-    rc = run_jobs(jobs, true, 0); if (rc) return rc;
+    rc = run_jobs(jobs, true, 0, NLANES); if (rc) return rc;
+    // the tails of the short-block launches, on the caller's stream behind the interpolation
+    for (int c : sblk_tails) {
+      SSQB_CUDA(cudaStreamWaitEvent(st, ev_sblk_ready[c], 0));
+      SblkArgs<T> S; sblk_rows_args(S, c);
+      rc = launch_sblk_rows<T>(S, narr, ssq, SBLK_TAIL, st); if (rc) return rc;
+    }
     if (lanes_on)
       for (int i = 0; i < NLANES; ++i)
         if (lane_used[i]) {

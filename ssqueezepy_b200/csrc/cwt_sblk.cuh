@@ -52,6 +52,8 @@ struct SblkArgs {
   int nblk, hop, h2;
   int write_dWx;
   T sigma;                     // taper width (tables)
+  unsigned* item_ctr;          // rows: next (block, row, signal) item, zeroed before the launch;
+                               // null: each CTA walks the items in steps of gridDim.x
 };
 
 template <typename T> struct SblkGeom { static constexpr int LOG_P = (sizeof(T) == 4) ? 12 : 11; };
@@ -144,8 +146,20 @@ sblk_rows_kernel(const SblkArgs<T> S) {
   // read consecutive entries (the natural table, indexed k*q*step, costs 8-16 wavefronts per
   // load).  Stage Ns (radix r) starts at Ns - 8 and holds (r - 1) * Ns entries: < P in total.
   cx<T>* tw = reinterpret_cast<cx<T>*>(s + P);         // [P]
+  // item = (block k, row r, signal b), k fastest.  Without a counter a CTA walks the items in
+  // steps of gridDim.x.  With S.item_ctr the items are taken from the counter: the CTAs of this
+  // launch and of any other launch sharing the counter split them between them, whenever each
+  // CTA happens to run.  Thread 0 then claims the next item during the current one (the
+  // atomic's latency hides behind the FFT stages) and hands it over through s_next.
+  __shared__ unsigned s_next;
   const int j = threadIdx.x;
+  const unsigned items = (unsigned)(S.B * S.n_rows * S.nblk);
+  const bool ctr = S.item_ctr != nullptr;
+  if (ctr && j == 0) s_next = atomicAdd(S.item_ctr, 1u);
   for (int m = j; m < P; m += NT) tw[m] = S.twsP[m];
+  __syncthreads();
+  unsigned it = ctr ? s_next : blockIdx.x;
+  if (it >= items) return;
 
   const int Nout = (int)A.Nout;
   T g2lo = 0, g2hi = 0; bool fast_ok = false; unsigned rowbytes = 0;
@@ -157,22 +171,13 @@ sblk_rows_kernel(const SblkArgs<T> S) {
     fast_ok = (A.grid.kind <= 1) && (A.grid.ftol < 0.25f);
     rowbytes = (unsigned)Nout * (unsigned)sizeof(cx<T>);
   }
-  // item = (block k, row r, signal b), k fastest; a CTA walks its items in steps of gridDim.x,
-  // carried in mixed radix (no division inside the loop)
-  int k, r, b;
-  {
-    const long long it0 = blockIdx.x;
-    k = (int)(it0 % S.nblk);
-    const long long rr = it0 / S.nblk;
-    r = (int)(rr % S.n_rows); b = (int)(rr / S.n_rows);
-  }
   const T xi_step = (T)(SSQB_TWO_PI / (double)P) / A.dt;
-  const int gk = (int)(gridDim.x % (unsigned)S.nblk);
-  const int gr = (int)((gridDim.x / (unsigned)S.nblk) % (unsigned)S.n_rows);
-  const int gb = (int)((gridDim.x / (unsigned)S.nblk) / (unsigned)S.n_rows);
 
 #pragma unroll 1
-  for (; b < (int)S.B; ) {
+  for (;;) {
+    const int k = (int)(it % (unsigned)S.nblk);
+    const unsigned rr = it / (unsigned)S.nblk;
+    const int r = (int)(rr % (unsigned)S.n_rows), b = (int)(rr / (unsigned)S.n_rows);
     const SblkRow ri = S.rows[r];
 
     cx<T> vw[8], vd[8];
@@ -199,7 +204,9 @@ sblk_rows_kernel(const SblkArgs<T> S) {
       }
     }
     idft<T, 8>(vw); if (NARR == 2) idft<T, 8>(vd);
-    __syncthreads();                                   // previous item is done with s (and tw is loaded)
+    __syncthreads();                                   // previous item is done with s and s_next
+    unsigned claim = 0;
+    if (ctr && j == 0) claim = atomicAdd(S.item_ctr, 1u);
 #pragma unroll
     for (int q = 0; q < 8; ++q) {
       V4 o; o.x = vw[q].x; o.y = vw[q].y; o.z = vd[q].x; o.w = vd[q].y;
@@ -208,6 +215,7 @@ sblk_rows_kernel(const SblkArgs<T> S) {
     __syncthreads();
     // ---- middle radix-8 stages (Ns = 8, 64, ..), in place ------------------------------------
     constexpr int NMID = (TAIL == 1) ? NR8 - 2 : NR8 - 1;
+    static_assert(NMID >= 1, "the next item is handed over in the last middle stage");
 #pragma unroll
     for (int st = 0; st < NMID; ++st) {
       const int Ns = 8 << (3 * st);
@@ -232,6 +240,7 @@ sblk_rows_kernel(const SblkArgs<T> S) {
         }
       }
       idft<T, 8>(vw); if (NARR == 2) idft<T, 8>(vd);
+      if (ctr && st == NMID - 1 && j == 0) s_next = claim;
       __syncthreads();
       const int j0 = (j - kk) * 8 + kk;
 #pragma unroll
@@ -241,6 +250,7 @@ sblk_rows_kernel(const SblkArgs<T> S) {
       }
       __syncthreads();
     }
+    const unsigned it_next = ctr ? s_next : it + gridDim.x;
     // ---- last stage: outputs t = j + NT m stay in registers -----------------------------------
     if constexpr (TAIL == 1) {
       // radix 8, Ns = P/8 = NT: k = j
@@ -286,10 +296,6 @@ sblk_rows_kernel(const SblkArgs<T> S) {
         vd[2 * q] = d0[q]; vd[2 * q + 1] = d1[q];
       }
     }
-    // next item (mixed-radix step of gridDim.x)
-    int kn = k + gk, rn = r + gr, bn = b + gb;
-    if (kn >= S.nblk) { kn -= S.nblk; ++rn; }
-    if (rn >= S.n_rows) { rn -= S.n_rows; ++bn; }
     // ---- epilogue: block sample t -> output k*hop + t - h2 -------------------------------------
     const int a = ri.a;
     const long long row = (long long)b * A.na + a;
@@ -318,7 +324,8 @@ sblk_rows_kernel(const SblkArgs<T> S) {
         }
       }
     }
-    k = kn; r = rn; b = bn;
+    if (it_next >= items) break;
+    it = it_next;
   }
 }
 
