@@ -196,6 +196,13 @@ int ssqb_ssq_stft_exec(const ssqb_stft_desc* d, const ssqb_reassign_desc* r,
 int ssqb_ssq_stft_exec_host(const ssqb_stft_desc* d, const ssqb_reassign_desc* r,
                             const void* x_host, int64_t B, void* Sx_host,
                             void* Tx_host, void* dSx_host, void* stream);
+/* backward of stft (_stft.py:127-146, differentiable here through torch.autograd): adjoint of
+ * the linear map x -> (Sx, dSx), same descriptor as ssqb_stft_exec.  gSx_dev, gdSx_dev
+ * [B][n_fft/2+1][n_hops] complex gradients (g = dL/dRe + i dL/dIm; either may be NULL);
+ * gx_dev [B][N] real, overwritten.  Deterministic: frames and pad copies are summed in a fixed
+ * order, with no atomics.                                                                    */
+int ssqb_stft_backward(const ssqb_stft_desc* d, const void* gSx_dev, const void* gdSx_dev,
+                       int64_t B, void* gx_dev, void* stream);
 
 /* ---- inverse transforms (column reductions / overlap-add) -------------------------- */
 /* Weighted real-part column sum, the core of
@@ -242,6 +249,12 @@ typedef struct {
 } ssqb_istft_desc;
 int ssqb_istft_exec(const ssqb_istft_desc* d, const void* Sx_dev, int64_t B, void* x_dev,
                     void* stream);
+/* backward of istft (_stft.py:184-256): adjoint of Sx -> x, same descriptor as ssqb_istft_exec.
+ * gx_dev [B][N] real gradient; gSx_dev [B][n_fft/2+1][n_hops] complex, overwritten:
+ * gSx[k][i] = (c_k / n_fft) sum_m u_i[m] e^{-2 pi i k m / n_fft}, u_i = window**win_exp times the
+ * frame of gx / window-norm (un-shifted when modulated), c_0 = c_{n_fft/2} = 1, otherwise 2.      */
+int ssqb_istft_backward(const ssqb_istft_desc* d, const void* gx_dev, int64_t B,
+                        void* gSx_dev, void* stream);
 
 #ifdef __cplusplus
 }

@@ -32,6 +32,7 @@ SYMBOLS = [
     'ssqb_indexed_sum', 'ssqb_phase_cwt', 'ssqb_phase_stft', 'ssqb_stft_exec',
     'ssqb_ssq_stft_exec', 'ssqb_ssq_stft_exec_host',
     'ssqb_colsum_real', 'ssqb_invert_components', 'ssqb_istft_exec', 'ssqb_extract_ridges', 'ssqb_cwt_backward',
+    'ssqb_stft_backward', 'ssqb_istft_backward',
 ]
 
 
@@ -107,6 +108,8 @@ def _bind(lib):
     lib.ssqb_colsum_real.argtypes = [ci, ci, vp, i64, ci, i64, C.POINTER(dbl), dbl, ci, vp, vp]
     lib.ssqb_invert_components.argtypes = [ci, vp, ci, i64, vp, vp, ci, dbl, vp, vp]
     lib.ssqb_istft_exec.argtypes = [C.POINTER(IstftDesc), vp, i64, vp, vp]
+    lib.ssqb_stft_backward.argtypes = [C.POINTER(StftDesc), vp, vp, i64, vp, vp]
+    lib.ssqb_istft_backward.argtypes = [C.POINTER(IstftDesc), vp, i64, vp, vp]
     lib.ssqb_extract_ridges.argtypes = [ci, vp, i64, ci, i64, C.POINTER(dbl), C.POINTER(dbl), dbl,
                                         dbl, ci, ci, vp, vp, vp, vp]
     for name in SYMBOLS:

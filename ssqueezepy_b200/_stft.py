@@ -187,6 +187,36 @@ def _get_call(N, window, n_fft, win_len, hop_len, fs, padtype, modulated, dtype)
     return call
 
 
+class _StftFn(torch.autograd.Function):
+    """`stft` as a differentiable torch op: forward is `ssqb_stft_exec`, backward its adjoint
+    `ssqb_stft_backward`.  A gradient that does not reach Sx or dSx arrives as None and is
+    passed to the library as NULL."""
+
+    @staticmethod
+    def forward(ctx, x2, call, derivative):
+        ctx.set_materialize_grads(False)
+        ctx.call = call
+        outs = call.outputs(x2.shape[0], 2 if derivative else 1)
+        _lib.check(Bk.require_cuda().ssqb_stft_exec(
+            C.byref(call.desc), x2.detach().data_ptr(), x2.shape[0], outs[0].data_ptr(),
+            outs[1].data_ptr() if derivative else None, Bk.stream_ptr()))
+        return tuple(outs) if derivative else outs[0]
+
+    @staticmethod
+    def backward(ctx, gS, gdS=None):
+        if gS is None and gdS is None:
+            return None, None, None
+        call = ctx.call
+        cdt = Bk.cplx_dtype(call.dtype)
+        gS = None if gS is None else gS.to(cdt).contiguous()
+        gdS = None if gdS is None else gdS.to(cdt).contiguous()
+        B = (gS if gS is not None else gdS).shape[0]
+        gx = torch.empty((B, call.N), dtype=Bk.real_dtype(call.dtype), device='cuda')
+        _lib.check(Bk.require_cuda().ssqb_stft_backward(
+            C.byref(call.desc), Bk.ptr(gS), Bk.ptr(gdS), B, gx.data_ptr(), Bk.stream_ptr()))
+        return gx, None, None
+
+
 def stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=None,
          padtype='reflect', modulated=True, derivative=False, dtype=None):
     """STFT of `x` ([N] or [B, N]): `Sx` of shape [n_fft//2 + 1, n_hops]
@@ -196,17 +226,45 @@ def stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=None,
     N = x.shape[-1]
     _, fs, _ = _process_fs_and_t(fs, t, N)
     call = _get_call(N, window, n_fft, win_len, hop_len, fs, padtype, modulated, dtype)
-    xd = Bk.to_device(x, call.dtype)
+    xd = Bk.to_device(x, call.dtype)             # differentiable cast / move / reshape
     x2 = xd if xd.ndim == 2 else xd.unsqueeze(0)
-    B = x2.shape[0]
-    outs = call.outputs(B, 2 if derivative else 1)
-    _lib.check(lib.ssqb_stft_exec(C.byref(call.desc), x2.data_ptr(), B,
-                                  outs[0].data_ptr(),
-                                  outs[1].data_ptr() if derivative else None,
-                                  Bk.stream_ptr()))
+    if torch.is_tensor(x) and x.requires_grad:
+        out = _StftFn.apply(x2, call, bool(derivative))
+        outs = list(out) if derivative else [out]
+    else:
+        B = x2.shape[0]
+        outs = call.outputs(B, 2 if derivative else 1)
+        _lib.check(lib.ssqb_stft_exec(C.byref(call.desc), x2.data_ptr(), B,
+                                      outs[0].data_ptr(),
+                                      outs[1].data_ptr() if derivative else None,
+                                      Bk.stream_ptr()))
     if x.ndim == 1:
         outs = [o[0] for o in outs]
     return (outs[0], outs[1]) if derivative else outs[0]
+
+
+class _IstftFn(torch.autograd.Function):
+    """`istft` as a differentiable torch op: forward is `ssqb_istft_exec`, backward its adjoint
+    `ssqb_istft_backward`.  `tables` keeps the host arrays the descriptor points to alive."""
+
+    @staticmethod
+    def forward(ctx, S3, d, tables, real_dtype):
+        ctx.d, ctx.tables, ctx.real_dtype = d, tables, real_dtype
+        ctx.shape, ctx.cdtype = S3.shape, S3.dtype
+        x = torch.empty((S3.shape[0], d.N), dtype=real_dtype, device=S3.device)
+        _lib.check(Bk.require_cuda().ssqb_istft_exec(C.byref(d), Bk.ptr(S3.detach()), S3.shape[0],
+                                                     Bk.ptr(x), Bk.stream_ptr()))
+        return x
+
+    @staticmethod
+    def backward(ctx, gx):
+        if gx is None:
+            return None, None, None, None
+        gx = gx.to(ctx.real_dtype).contiguous()
+        gS = torch.empty(ctx.shape, dtype=ctx.cdtype, device=gx.device)
+        _lib.check(Bk.require_cuda().ssqb_istft_backward(C.byref(ctx.d), Bk.ptr(gx), gx.shape[0],
+                                                         Bk.ptr(gS), Bk.stream_ptr()))
+        return gS, None, None, None
 
 
 def istft(Sx, window=None, n_fft=None, win_len=None, hop_len=1, N=None,
@@ -240,12 +298,15 @@ def istft(Sx, window=None, n_fft=None, win_len=None, hop_len=1, N=None,
     wpow = np.ascontiguousarray(wpow, dtype=dtype)
 
     lib = Bk.require_cuda()
-    x = torch.empty((B, N), dtype=Bk.real_dtype(dtype), device=Sd.device)
     d = _lib.IstftDesc(dtype=Bk.dtype_code(dtype), N=N, n_fft=n_fft, hop=hop_len,
                        n_hops=n_hops, modulated=int(bool(modulated)),
                        wexp_host=None if wexp is None else wexp.ctypes.data,
                        wpow_host=wpow.ctypes.data)
-    _lib.check(lib.ssqb_istft_exec(C.byref(d), Bk.ptr(S3.contiguous()), B, Bk.ptr(x),
-                                   Bk.stream_ptr()))
+    if Bk.is_tensor(Sx) and Sx.requires_grad:
+        x = _IstftFn.apply(S3.contiguous(), d, (wexp, wpow), Bk.real_dtype(dtype))
+    else:
+        x = torch.empty((B, N), dtype=Bk.real_dtype(dtype), device=Sd.device)
+        _lib.check(lib.ssqb_istft_exec(C.byref(d), Bk.ptr(S3.contiguous()), B, Bk.ptr(x),
+                                       Bk.stream_ptr()))
     x = x if Sd.ndim == 3 else x[0]
     return Bk.finish(x, not was_np)

@@ -184,6 +184,16 @@ int ssqb_istft_exec(const ssqb_istft_desc* d, const void* Sx, int64_t B, void* x
   return run_istft(d, Sx, B, x, (cudaStream_t)stream);
 }
 
+int ssqb_stft_backward(const ssqb_stft_desc* d, const void* gSx, const void* gdSx, int64_t B,
+                       void* gx, void* stream) {
+  return run_stft_backward(d, gSx, gdSx, B, gx, (cudaStream_t)stream);
+}
+
+int ssqb_istft_backward(const ssqb_istft_desc* d, const void* gx, int64_t B, void* gSx,
+                        void* stream) {
+  return run_istft_backward(d, gx, B, gSx, (cudaStream_t)stream);
+}
+
 int ssqb_extract_ridges(int dtype, const void* Tf, int64_t B, int na, int64_t N, const double* ls_host,
                         const double* scales_host, double penalty, double eps, int n_ridges, int bw,
                         int64_t* idx_dev, void* f_dev, void* e_dev, void* stream) {

@@ -216,4 +216,26 @@ istft_ola_kernel(const IstftArgs<T> A) {
   A.x[(long long)b * A.N + jo] = acc;
 }
 
+// istft backward, first step: gp[b][j] = gx[b][j] / wn[j + M/2] with the forward's float64 window
+// norm and tiny rule (samples whose norm is <= tiny pass undivided).  One thread per sample walks
+// the batch, so the norm is summed once per sample.
+template <typename T>
+__global__ void __launch_bounds__(256)
+istft_bwd_norm_kernel(const IstftArgs<T> A, const T* __restrict__ gx, T* __restrict__ gp) {
+  const long long jo = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (jo >= A.N) return;
+  const int M = A.n_fft, H = A.hop;
+  const long long n = jo + M / 2;
+  long long i0 = (n - M + 1 + H - 1) / H;
+  if (n - M + 1 <= 0) i0 = 0;
+  const long long i1 = n / H;
+  double wn = 0.0;
+  for (long long i = i0; i <= i1 && i < A.max_hops; ++i) wn += (double)A.wpow[n - i * H];
+  const bool div = wn > A.tiny;
+  for (int b = 0; b < A.B; ++b) {
+    const T v = gx[(long long)b * A.N + jo];
+    gp[(long long)b * A.N + jo] = div ? (T)((double)v / wn) : v;
+  }
+}
+
 }  // namespace ssqb

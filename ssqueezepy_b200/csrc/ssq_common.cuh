@@ -233,8 +233,9 @@ __device__ __forceinline__ int bin_fused(T A, T B, T C, T D, const ReassignGrid&
 }
 
 // reflect / zero / symmetric / replicate / wrap index map of
-// ssqueezepy/utils/common.py:131-147 (np.pad modes).  Returns -1 for "zero".
-__device__ __forceinline__ int64_t pad_src_index(int64_t t, int64_t n1, int64_t N, int padtype) {
+// ssqueezepy/utils/common.py:131-147 (np.pad modes).  Returns -1 for "zero".  Also called on
+// the host, where the stft backward groups the pad samples by the sample they copy.
+__host__ __device__ __forceinline__ int64_t pad_src_index(int64_t t, int64_t n1, int64_t N, int padtype) {
   int64_t s = t - n1;
   if (s >= 0 && s < N) return s;
   switch (padtype) {

@@ -45,18 +45,30 @@ __device__ __forceinline__ long long frame_src(int l, long long i, int hop, int 
   return (l < s20) ? start + s21 + l : start + (l - s20);
 }
 
-template <typename T>
+// What the transform of a frame feeds: Sx (+ dSx), the same plus the fused reassignment
+// (ssq_stft), or the istft adjoint, which transforms one real sequence (no dSx half) and
+// writes gSx[k] = (c_k / n_fft) C[k]  (c_0 = c_{n_fft/2} = 1, otherwise 2).
+enum { STFT_EPI_PLAIN = 0, STFT_EPI_SSQ = 1, STFT_EPI_ISTFT_BWD = 2 };
+
+template <typename T, int EPI>
 __device__ __forceinline__ void stft_emit(const StftArgs<T>& A, int b, int k, long long frame,
-                                          cx<T> Ck, cx<T> Cmk, bool ssq) {
+                                          cx<T> Ck, cx<T> Cmk) {
   // C = FFT(c);  S = (C[k] + conj(C[M-k]))/2 ; kappa*dS = (C[k] - conj(C[M-k]))/(2i)
   T h = (T)0.5;
   cx<T> S  = mkc<T>((Ck.x + Cmk.x) * h, (Ck.y - Cmk.y) * h);
-  cx<T> dS = mkc<T>((Ck.y + Cmk.y) * h * A.inv_kappa, (Cmk.x - Ck.x) * h * A.inv_kappa);
   int nrows = A.n_fft / 2 + 1;
   long long o = ((long long)b * nrows + k) * A.n_hops + frame;
+  if (EPI == STFT_EPI_ISTFT_BWD) {
+    // irfft reads only the real part of the DC and Nyquist bins
+    const bool edge = (k == 0 || 2 * k == A.n_fft);
+    const T sc = (T)((edge ? 1.0 : 2.0) / (double)A.n_fft);
+    A.Sx[o] = mkc<T>(S.x * sc, edge ? (T)0 : S.y * sc);
+    return;
+  }
+  cx<T> dS = mkc<T>((Ck.y + Cmk.y) * h * A.inv_kappa, (Cmk.x - Ck.x) * h * A.inv_kappa);
   A.Sx[o] = S;
   if (A.write_dSx) A.dSx[o] = dS;
-  if (ssq && is_active_exact(S.x, S.y, A.grid.gamma)) {
+  if (EPI == STFT_EPI_SSQ && is_active_exact(S.x, S.y, A.grid.gamma)) {
     double r = phase_ratio_exact<T>(dS.x, dS.y, S.x, S.y);
     double w = fabs((double)A.Sfs[k] - r);
     int kk = bin_from_w_exact(w, A.grid);
@@ -66,7 +78,7 @@ __device__ __forceinline__ void stft_emit(const StftArgs<T>& A, int b, int k, lo
 }
 
 // ---- power-of-two n_fft -------------------------------------------------------
-template <typename T, int LOG_M, bool SSQ>
+template <typename T, int LOG_M, int EPI>
 __global__ void __launch_bounds__(Tile<T>::NT)
 stft_pow2_kernel(const StftArgs<T> A) {
   constexpr int NT = Tile<T>::NT;
@@ -93,7 +105,8 @@ stft_pow2_kernel(const StftArgs<T> A) {
       long long t = frame_src(l, i, A.hop, M, A.modulated);
       long long src = pad_src_index(t, A.n1, A.N, A.padtype);
       T v = (src >= 0) ? A.x[(long long)b * A.N + src] : (T)0;
-      z = mkc<T>(v * A.win[l], -(v * A.dwin[l]) * A.kappa);   // conj(c)
+      z = mkc<T>(v * A.win[l],                                 // conj(c)
+                 EPI == STFT_EPI_ISTFT_BWD ? (T)0 : -(v * A.dwin[l]) * A.kappa);
     }
     s[l * STRIDE + r] = z;
   }
@@ -109,13 +122,13 @@ stft_pow2_kernel(const StftArgs<T> A) {
     long long i = fr - (long long)b * A.n_hops;
     cx<T> Ck = cconj<T>(s[k * STRIDE + r]);
     cx<T> Cmk = cconj<T>(s[((M - k) & (M - 1)) * STRIDE + r]);
-    stft_emit<T>(A, b, k, i, Ck, Cmk, SSQ);
+    stft_emit<T, EPI>(A, b, k, i, Ck, Cmk);
   }
 }
 
 // ---- any other n_fft: frames -> generic-length FFT (gfft.cuh) -> Hermitian split ------------
 // c[f][l] = x_f[l] win[l] + i kappa x_f[l] dwin[l]   (frames f0 .. f0 + nf of the flattened batch)
-template <typename T>
+template <typename T, int EPI>
 __global__ void __launch_bounds__(256)
 stft_frames_kernel(const StftArgs<T> A, cx<T>* __restrict__ c, long long f0, long long nf) {
   const int M = A.n_fft;
@@ -128,9 +141,9 @@ stft_frames_kernel(const StftArgs<T> A, cx<T>* __restrict__ c, long long f0, lon
   const long long t = frame_src(l, i, A.hop, M, A.modulated);
   const long long src = pad_src_index(t, A.n1, A.N, A.padtype);
   const T v = (src >= 0) ? A.x[(long long)b * A.N + src] : (T)0;
-  c[idx] = mkc<T>(v * A.win[l], (v * A.dwin[l]) * A.kappa);
+  c[idx] = mkc<T>(v * A.win[l], EPI == STFT_EPI_ISTFT_BWD ? (T)0 : (v * A.dwin[l]) * A.kappa);
 }
-template <typename T, bool SSQ>
+template <typename T, int EPI>
 __global__ void __launch_bounds__(256)
 stft_emit_kernel(const StftArgs<T> A, const cx<T>* __restrict__ C, long long f0, long long nf) {
   const int M = A.n_fft, nrows = M / 2 + 1;
@@ -141,7 +154,157 @@ stft_emit_kernel(const StftArgs<T> A, const cx<T>* __restrict__ C, long long f0,
   const int b = (int)(fr / A.n_hops);
   const long long i = fr - (long long)b * A.n_hops;
   const cx<T> Ck = C[fl * M + k], Cmk = C[fl * M + (k ? M - k : 0)];
-  stft_emit<T>(A, b, k, i, Ck, Cmk, SSQ);
+  stft_emit<T, EPI>(A, b, k, i, Ck, Cmk);
+}
+
+// ---- stft backward (adjoint of x -> (Sx, dSx)) ------------------------------------------
+// y_i[l] = win[l] Re sum_k gS[k,i] e^{+2 pi i k l/M} + dwin[l] Re sum_k gdS[k,i] e^{+2 pi i k l/M}
+// (k = 0 .. M/2, each bin once), then gxp[t] = sum of y_i[l] over the (i, l) that frame t, and
+// gx[j] = sum of gxp[t] over the padded samples t that copy x[j].  The two real sequences of a
+// frame share one complex inverse transform, the mirror image of the forward's packing:
+// z = IFFT(G + i D / kappa) with G, D the Hermitian extensions, y = win Re z + kappa dwin Im z.
+template <typename T>
+struct StftBwdArgs {
+  long long N, n_hops;
+  int n_fft, hop, n1, B;
+  int modulated;
+  const cx<T>* gS;          // [B][n_fft/2+1][n_hops] or nullptr
+  const cx<T>* gdS;         // same, or nullptr
+  const T* win;             // the forward's tables (ifftshifted when modulated)
+  const T* dwin;
+  T kappa, inv_kappa;
+  const cx<T>* tw;          // n_fft-th roots exp(+2 pi i m / n_fft)
+  T* ybuf;                  // [B * n_hops][n_fft]: y of each frame, at its position in the frame window
+  T* gx;                    // [B][N]
+  // padded samples outside [n1, n1 + N), grouped by the sample they copy (ascending t in a group):
+  // group q adds gxp[pad_t[pad_off[q] .. pad_off[q+1])] to gx[pad_j[q]]
+  const long long* pad_off; const long long* pad_j; const long long* pad_t;
+  long long n_pad_groups;
+};
+
+// bin k (0 .. M-1) of the packed Hermitian spectrum G + i D / kappa of frame (b, i)
+template <typename T>
+__device__ __forceinline__ cx<T> stft_bwd_bin(const StftBwdArgs<T>& A, int b, long long i, int k) {
+  const int M = A.n_fft, nrows = M / 2 + 1;
+  const int kk = (k <= M / 2) ? k : M - k;
+  const long long o = ((long long)b * nrows + kk) * A.n_hops + i;
+  cx<T> g = A.gS ? A.gS[o] : mkc<T>((T)0, (T)0);
+  cx<T> d = A.gdS ? A.gdS[o] : mkc<T>((T)0, (T)0);
+  if (kk == 0 || 2 * kk == M) {                  // Re drops the imaginary part of DC / Nyquist
+    g.y = (T)0; d.y = (T)0;
+  } else {                                       // split between bins k and M - k
+    const T h = (T)0.5;
+    g = mkc<T>(g.x * h, g.y * h); d = mkc<T>(d.x * h, d.y * h);
+    if (k > M / 2) { g.y = -g.y; d.y = -d.y; }
+  }
+  return mkc<T>(g.x - d.y * A.inv_kappa, g.y + d.x * A.inv_kappa);
+}
+
+// frame sample l of z (the inverse transform) -> y at window position p = frame_src(l, i) - i*hop
+template <typename T>
+__device__ __forceinline__ T stft_bwd_y(const StftBwdArgs<T>& A, int l, cx<T> z) {
+  T y = (T)0;
+  if (A.gS) y = A.win[l] * z.x;
+  if (A.gdS) y += (A.kappa * A.dwin[l]) * z.y;
+  return y;
+}
+
+template <typename T, int LOG_M>
+__global__ void __launch_bounds__(Tile<T>::NT)
+stft_bwd_pow2_kernel(const StftBwdArgs<T> A) {
+  constexpr int NT = Tile<T>::NT;
+  constexpr int M = 1 << LOG_M;
+  constexpr int R = Tile<T>::ELEMS / M;
+  constexpr int STRIDE = R + 1;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  cx<T>* s = reinterpret_cast<cx<T>*>(smem_raw);          // [M][STRIDE]
+  cx<T>* tw = s + (size_t)M * STRIDE;                     // [M]
+  const int tid = threadIdx.x;
+  const long long total = (long long)A.B * A.n_hops;
+  const long long f0 = (long long)blockIdx.x * R;
+  for (int m = tid; m < M; m += NT) tw[m] = A.tw[m];
+#pragma unroll 1
+  for (int lin = tid; lin < M * R; lin += NT) {
+    const int r = lin % R, k = lin / R;                    // frames fastest: coalesced rows
+    const long long fr = f0 + r;
+    cx<T> z = mkc<T>((T)0, (T)0);
+    if (fr < total) {
+      const int b = (int)(fr / A.n_hops);
+      z = stft_bwd_bin<T>(A, b, fr - (long long)b * A.n_hops, k);
+    }
+    s[k * STRIDE + r] = z;
+  }
+  __syncthreads();
+  block_ifft<T, LOG_M, R, NT, STRIDE>(s, tw);             // sum_k Z[k] e^{+2 pi i k l / M}
+#pragma unroll 1
+  for (int lin = tid; lin < M * R; lin += NT) {
+    const int p = lin % M, r = lin / M;                    // window positions fastest
+    const long long fr = f0 + r;
+    if (fr >= total) continue;
+    const int l = A.modulated ? ((p + M - M / 2) & (M - 1)) : p;   // frame_src(l) = i*hop + p
+    A.ybuf[fr * M + p] = stft_bwd_y<T>(A, l, s[l * STRIDE + r]);
+  }
+}
+
+// any other n_fft: packed spectra of frames f0 .. f0 + nf -> c, inverse Gfft, then this epilogue
+template <typename T>
+__global__ void __launch_bounds__(256)
+stft_bwd_spec_kernel(const StftBwdArgs<T> A, cx<T>* __restrict__ c, long long f0, long long nf) {
+  const int M = A.n_fft;
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= nf * M) return;
+  const long long fl = idx / M; const int k = (int)(idx - fl * M);
+  const long long fr = f0 + fl;
+  const int b = (int)(fr / A.n_hops);
+  c[idx] = stft_bwd_bin<T>(A, b, fr - (long long)b * A.n_hops, k);
+}
+template <typename T>
+__global__ void __launch_bounds__(256)
+stft_bwd_frames_kernel(const StftBwdArgs<T> A, const cx<T>* __restrict__ z, long long f0, long long nf) {
+  const int M = A.n_fft;
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= nf * M) return;
+  const long long fl = idx / M; const int p = (int)(idx - fl * M);
+  const int l = A.modulated ? (p + M - M / 2) % M : p;    // M/2 = s21 of frame_src
+  A.ybuf[(f0 + fl) * M + p] = stft_bwd_y<T>(A, l, z[fl * M + l]);
+}
+
+// padded-signal gradient at t: the frames covering t, in ascending frame order
+template <typename T>
+__device__ __forceinline__ T stft_bwd_gxp(const StftBwdArgs<T>& A, int b, long long t) {
+  const int M = A.n_fft, H = A.hop;
+  long long i0 = (t - M + 1 + H - 1) / H;                 // ceil((t - M + 1) / H)
+  if (t - M + 1 <= 0) i0 = 0;
+  const long long i1 = t / H;
+  const T* __restrict__ yb = A.ybuf + (long long)b * A.n_hops * M;
+  T acc = (T)0;
+  for (long long i = i0; i <= i1 && i < A.n_hops; ++i) acc += yb[i * M + (t - i * H)];
+  return acc;
+}
+
+// gx[j] = gxp[n1 + j]: one thread per sample
+template <typename T>
+__global__ void __launch_bounds__(256)
+stft_bwd_gather_kernel(const StftBwdArgs<T> A) {
+  const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= A.N) return;
+  for (int b = blockIdx.y; b < A.B; b += gridDim.y)
+    A.gx[(long long)b * A.N + j] = stft_bwd_gxp<T>(A, b, A.n1 + j);
+}
+
+// then the padding: gx[j] += gxp[t] for the pad samples t that copy x[j], ascending t.  One
+// thread per copied sample, so every sum has one owner and a fixed order (no atomics).
+template <typename T>
+__global__ void __launch_bounds__(256)
+stft_bwd_fold_kernel(const StftBwdArgs<T> A) {
+  const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= A.n_pad_groups) return;
+  for (int b = blockIdx.y; b < A.B; b += gridDim.y) {
+    T* g = A.gx + (long long)b * A.N + A.pad_j[q];
+    T acc = *g;
+    for (long long e = A.pad_off[q]; e < A.pad_off[q + 1]; ++e) acc += stft_bwd_gxp<T>(A, b, A.pad_t[e]);
+    *g = acc;
+  }
 }
 
 }  // namespace ssqb

@@ -1,7 +1,9 @@
 // Host dispatch of the STFT / ssq_stft kernels.
 #include "host_common.h"
 #include "stft_kernels.cuh"
+#include "inverse_kernels.cuh"   // IstftArgs, istft_bwd_norm_kernel
 #include "cwt_generic.cuh"      // Gfft<T>: generic-length FFT
+#include <algorithm>
 #include <map>
 #include <memory>
 #include <vector>
@@ -38,7 +40,7 @@ static int table_blob(const std::vector<unsigned char>& h, cudaStream_t st, unsi
   return 0;
 }
 
-template <typename T, bool SSQ>
+template <typename T, int EPI>
 static int launch_stft_pow2(const StftArgs<T>& A, int logm, cudaStream_t st) {
   long long total = (long long)A.B * A.n_hops;
   switch (logm) {
@@ -46,7 +48,7 @@ static int launch_stft_pow2(const StftArgs<T>& A, int logm, cudaStream_t st) {
     case L: {                                                                             \
       constexpr int M = 1 << L; constexpr int R = Tile<T>::ELEMS / M;                     \
       size_t smem = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);                            \
-      auto kern = stft_pow2_kernel<T, L, SSQ>;                                            \
+      auto kern = stft_pow2_kernel<T, L, EPI>;                                            \
       static bool attr_done = false;                                                      \
       if (!attr_done) {                                                                   \
         SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, \
@@ -73,7 +75,7 @@ static std::mutex g_gen_mu;
 template <typename T> static std::map<std::pair<int, int>, std::unique_ptr<StftGeneric<T>>>& gen_cache() {
   static std::map<std::pair<int, int>, std::unique_ptr<StftGeneric<T>>> m; return m;
 }
-template <typename T, bool SSQ>
+template <typename T, int EPI>
 static int launch_stft_generic(const StftArgs<T>& A, cudaStream_t st) {
   int dev = 0; SSQB_CUDA(cudaGetDevice(&dev));
   std::lock_guard<std::mutex> lk(g_gen_mu);            // one caller at a time per process
@@ -90,14 +92,43 @@ static int launch_stft_generic(const StftArgs<T>& A, cudaStream_t st) {
   SSQB_CUDA(G.c.ensure((size_t)chunk * (size_t)M)); SSQB_CUDA(G.C.ensure((size_t)chunk * (size_t)M));
   for (long long f0 = 0; f0 < total; f0 += chunk) {
     const long long nf = total - f0 < chunk ? total - f0 : chunk;
-    stft_frames_kernel<T><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(A, G.c.p, f0, nf);
+    stft_frames_kernel<T, EPI><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(A, G.c.p, f0, nf);
     SSQB_LAUNCH_CHECK();
     int rc = G.fft.exec(G.c.p, G.C.p, nf, -1, (T)1, st); if (rc) return rc;
-    stft_emit_kernel<T, SSQ><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(A, G.C.p, f0, nf);
+    stft_emit_kernel<T, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(A, G.C.p, f0, nf);
     SSQB_LAUNCH_CHECK();
   }
   SSQB_CUDA(cudaStreamSynchronize(st));                // buffers are shared by later callers
   return 0;
+}
+
+// n_fft-th roots exp(+2 pi i m / n_fft): computed once per (length, dtype), not on every call
+template <typename T>
+static const std::vector<cx<T>>& roots(int M) {
+  static std::mutex tw_mu;
+  static std::map<int, std::vector<cx<T>>> tw_cache;
+  std::lock_guard<std::mutex> lk(tw_mu);
+  auto it = tw_cache.find(M);
+  if (it == tw_cache.end()) {
+    std::vector<cx<T>> v((size_t)M);
+    for (int m = 0; m < M; ++m) {
+      double ang = 2.0 * M_PI * (double)m / (double)M;
+      v[m] = mkc<T>((T)cos(ang), (T)sin(ang));
+    }
+    it = tw_cache.emplace(M, std::move(v)).first;
+  }
+  return it->second;                         // map nodes are stable
+}
+
+// kappa = power of two that balances ||win|| and ||dwin||
+template <typename T>
+static double pack_kappa(const T* win, const T* dwin, int M) {
+  double nw = 0, nd = 0;
+  for (int l = 0; l < M; ++l) { nw += (double)win[l] * win[l]; nd += (double)dwin[l] * dwin[l]; }
+  double kap = 1.0;
+  if (nd > 0 && nw > 0) kap = exp2(rint(0.5 * log2(nw / nd)));
+  if (!(kap > 1e-30 && kap < 1e30)) kap = 1.0;
+  return kap;
 }
 
 template <typename T>
@@ -112,12 +143,7 @@ static int stft_t(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const vo
   A.x = (const T*)x; A.Sx = (cx<T>*)Sx; A.dSx = (cx<T>*)dSx; A.Tx = (cx<T>*)Tx;
   A.write_dSx = dSx ? 1 : 0;
   const T* win = (const T*)d->win_host; const T* dwin = (const T*)d->dwin_host;
-  // kappa = power of two that balances ||win|| and ||dwin||
-  double nw = 0, nd = 0;
-  for (int l = 0; l < M; ++l) { nw += (double)win[l] * win[l]; nd += (double)dwin[l] * dwin[l]; }
-  double kap = 1.0;
-  if (nd > 0 && nw > 0) kap = exp2(rint(0.5 * log2(nw / nd)));
-  if (!(kap > 1e-30 && kap < 1e30)) kap = 1.0;
+  const double kap = pack_kappa(win, dwin, M);
   A.kappa = (T)kap; A.inv_kappa = (T)(1.0 / kap);
   // device copies of the small tables: built on the host, cached on the device by content
   // (a streaming caller repeats the same window / grid thousands of times; without the
@@ -126,24 +152,7 @@ static int stft_t(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const vo
   std::vector<unsigned char> h(tb);
   size_t off = 0;
   auto put = [&](const void* src, size_t bytes) { memcpy(h.data() + off, src, bytes); size_t o = off; off += bytes; return o; };
-  // n_fft-th roots: computed once per (length, dtype), not on every call
-  static std::mutex tw_mu;
-  static std::map<int, std::vector<cx<T>>> tw_cache;
-  std::vector<cx<T>>* twp;
-  {
-    std::lock_guard<std::mutex> lk(tw_mu);
-    auto it = tw_cache.find(M);
-    if (it == tw_cache.end()) {
-      std::vector<cx<T>> v((size_t)M);
-      for (int m = 0; m < M; ++m) {
-        double ang = 2.0 * M_PI * (double)m / (double)M;
-        v[m] = mkc<T>((T)cos(ang), (T)sin(ang));
-      }
-      it = tw_cache.emplace(M, std::move(v)).first;
-    }
-    twp = &it->second;                       // map nodes are stable
-  }
-  const std::vector<cx<T>>& tw = *twp;
+  const std::vector<cx<T>>& tw = roots<T>(M);
   std::vector<double> cst((size_t)nrows, 0.0);
   if (ssq) for (int i = 0; i < nrows; ++i) cst[i] = r->cst_host[i];
   size_t o_tw = put(tw.data(), sizeof(cx<T>) * M);          // 16-byte aligned first
@@ -164,9 +173,9 @@ static int stft_t(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const vo
   int logm = ilog2_exact(M);
   int rc;
   if (logm >= 1 && logm <= 12 && (Tile<T>::ELEMS >> logm) >= 1)
-    rc = ssq ? launch_stft_pow2<T, true>(A, logm, st) : launch_stft_pow2<T, false>(A, logm, st);
+    rc = ssq ? launch_stft_pow2<T, STFT_EPI_SSQ>(A, logm, st) : launch_stft_pow2<T, STFT_EPI_PLAIN>(A, logm, st);
   else
-    rc = ssq ? launch_stft_generic<T, true>(A, st) : launch_stft_generic<T, false>(A, st);
+    rc = ssq ? launch_stft_generic<T, STFT_EPI_SSQ>(A, st) : launch_stft_generic<T, STFT_EPI_PLAIN>(A, st);
   return rc;
 }
 
@@ -178,6 +187,200 @@ int run_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const void* x
   if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
   return d->dtype == SSQB_F32 ? stft_t<float>(d, r, x, B, Sx, Tx, dSx, ssq, st)
                               : stft_t<double>(d, r, x, B, Sx, Tx, dSx, ssq, st);
+}
+
+// ---- backward passes (torch.autograd) --------------------------------------------------------
+// Table blob with every piece starting on a 16-byte boundary.
+struct BlobBuilder {
+  std::vector<unsigned char> h;
+  size_t put(const void* src, size_t bytes) {
+    size_t o = (h.size() + 15) & ~(size_t)15;
+    h.resize(o + bytes);
+    if (bytes) memcpy(h.data() + o, src, bytes);
+    return o;
+  }
+};
+
+template <typename T>
+static int launch_stft_bwd_pow2(const StftBwdArgs<T>& A, int logm, cudaStream_t st) {
+  const long long total = (long long)A.B * A.n_hops;
+  switch (logm) {
+#define SSQB_SB(L)                                                                        \
+    case L: {                                                                             \
+      constexpr int M = 1 << L; constexpr int R = Tile<T>::ELEMS / M;                     \
+      size_t smem = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);                            \
+      auto kern = stft_bwd_pow2_kernel<T, L>;                                             \
+      static bool attr_done = false;                                                      \
+      if (!attr_done) {                                                                   \
+        SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                       (int)smem));                                       \
+        attr_done = true;                                                                 \
+      }                                                                                   \
+      kern<<<(unsigned)((total + R - 1) / R), Tile<T>::NT, smem, st>>>(A);                \
+      SSQB_LAUNCH_CHECK();                                                                \
+      return 0; }
+    SSQB_SB(1) SSQB_SB(2) SSQB_SB(3) SSQB_SB(4) SSQB_SB(5) SSQB_SB(6) SSQB_SB(7) SSQB_SB(8)
+    SSQB_SB(9) SSQB_SB(10) SSQB_SB(11) SSQB_SB(12)
+#undef SSQB_SB
+    default: return -1;
+  }
+}
+
+// other n_fft: packed spectra -> inverse Gfft -> epilogue, in the forward's chunks and buffers
+template <typename T>
+static int launch_stft_bwd_generic(const StftBwdArgs<T>& A, cudaStream_t st) {
+  int dev = 0; SSQB_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lk(g_gen_mu);
+  auto& slot = gen_cache<T>()[{dev, A.n_fft}];
+  if (!slot) {
+    slot.reset(new StftGeneric<T>());
+    int rc = slot->fft.init(A.n_fft);
+    if (rc) { slot.reset(); return rc; }
+  }
+  StftGeneric<T>& G = *slot;
+  const long long total = (long long)A.B * A.n_hops, M = A.n_fft;
+  long long chunk = ((128ll << 20) / (long long)sizeof(cx<T>)) / M; if (chunk < 1) chunk = 1;
+  if (chunk > total) chunk = total;
+  SSQB_CUDA(G.c.ensure((size_t)chunk * (size_t)M)); SSQB_CUDA(G.C.ensure((size_t)chunk * (size_t)M));
+  for (long long f0 = 0; f0 < total; f0 += chunk) {
+    const long long nf = total - f0 < chunk ? total - f0 : chunk;
+    const unsigned nb = (unsigned)((nf * M + 255) / 256);
+    stft_bwd_spec_kernel<T><<<nb, 256, 0, st>>>(A, G.c.p, f0, nf);
+    SSQB_LAUNCH_CHECK();
+    int rc = G.fft.exec(G.c.p, G.C.p, nf, +1, (T)1, st); if (rc) return rc;
+    stft_bwd_frames_kernel<T><<<nb, 256, 0, st>>>(A, G.C.p, f0, nf);
+    SSQB_LAUNCH_CHECK();
+  }
+  SSQB_CUDA(cudaStreamSynchronize(st));                // buffers are shared by later callers
+  return 0;
+}
+
+template <typename T>
+static int stft_bwd_t(const ssqb_stft_desc* d, const void* gS, const void* gdS, long long B,
+                      void* gx, cudaStream_t st) {
+  const int M = d->n_fft;
+  StftBwdArgs<T> A;
+  memset(&A, 0, sizeof(A));
+  A.N = d->N; A.n_hops = (d->N - 1) / d->hop + 1;
+  A.n_fft = M; A.hop = d->hop; A.n1 = d->n1; A.B = (int)B; A.modulated = d->modulated;
+  A.gS = (const cx<T>*)gS; A.gdS = (const cx<T>*)gdS; A.gx = (T*)gx;
+  const T* win = (const T*)d->win_host; const T* dwin = (const T*)d->dwin_host;
+  const double kap = pack_kappa(win, dwin, M);
+  A.kappa = (T)kap; A.inv_kappa = (T)(1.0 / kap);
+  // pad samples t grouped by the sample j they copy, ascending t within a group
+  std::vector<std::pair<long long, long long>> jt;
+  const long long Np = d->N + M - 1;
+  for (long long t = 0; t < Np; ++t) {
+    if (t == d->n1) t = d->n1 + d->N;                  // skip the unpadded part
+    if (t >= Np) break;
+    const long long j = pad_src_index(t, d->n1, d->N, d->padtype);
+    if (j >= 0) jt.emplace_back(j, t);
+  }
+  std::sort(jt.begin(), jt.end());
+  std::vector<long long> off, js, ts;
+  for (size_t e = 0; e < jt.size(); ++e) {
+    if (e == 0 || jt[e].first != jt[e - 1].first) { off.push_back((long long)e); js.push_back(jt[e].first); }
+    ts.push_back(jt[e].second);
+  }
+  off.push_back((long long)jt.size());
+  BlobBuilder bb;
+  const std::vector<cx<T>>& tw = roots<T>(M);
+  const size_t o_tw = bb.put(tw.data(), sizeof(cx<T>) * M);
+  const size_t o_win = bb.put(win, sizeof(T) * M);
+  const size_t o_dwin = bb.put(dwin, sizeof(T) * M);
+  const size_t o_off = bb.put(off.data(), sizeof(long long) * off.size());
+  const size_t o_j = bb.put(js.data(), sizeof(long long) * js.size());
+  const size_t o_t = bb.put(ts.data(), sizeof(long long) * ts.size());
+  unsigned char* blob = nullptr;
+  int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
+  A.tw = (const cx<T>*)(blob + o_tw);
+  A.win = (const T*)(blob + o_win); A.dwin = (const T*)(blob + o_dwin);
+  A.pad_off = (const long long*)(blob + o_off);
+  A.pad_j = (const long long*)(blob + o_j); A.pad_t = (const long long*)(blob + o_t);
+  A.n_pad_groups = (long long)js.size();
+  // frame buffer: B * n_hops * n_fft reals, no larger than gSx
+  SSQB_CUDA(cudaMallocAsync((void**)&A.ybuf, sizeof(T) * (size_t)B * (size_t)A.n_hops * (size_t)M, st));
+  const int logm = ilog2_exact(M);
+  if (logm >= 1 && logm <= 12 && (Tile<T>::ELEMS >> logm) >= 1) rc = launch_stft_bwd_pow2<T>(A, logm, st);
+  else rc = launch_stft_bwd_generic<T>(A, st);
+  if (rc == 0) {
+    const unsigned gy = (unsigned)(B < 65535 ? B : 65535);
+    stft_bwd_gather_kernel<T><<<dim3((unsigned)((A.N + 255) / 256), gy), 256, 0, st>>>(A);
+    SSQB_LAUNCH_CHECK();
+    if (A.n_pad_groups > 0) {
+      stft_bwd_fold_kernel<T><<<dim3((unsigned)((A.n_pad_groups + 255) / 256), gy), 256, 0, st>>>(A);
+      SSQB_LAUNCH_CHECK();
+    }
+  }
+  cudaFreeAsync(A.ybuf, st);
+  return rc;
+}
+
+int run_stft_backward(const ssqb_stft_desc* d, const void* gSx, const void* gdSx, long long B,
+                      void* gx, cudaStream_t st) {
+  if (!d || !gx || (!gSx && !gdSx)) return set_error(SSQB_E_ARG, "null pointer");
+  if (!d->win_host || !d->dwin_host) return set_error(SSQB_E_ARG, "null table");
+  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
+  return d->dtype == SSQB_F32 ? stft_bwd_t<float>(d, gSx, gdSx, B, gx, st)
+                              : stft_bwd_t<double>(d, gSx, gdSx, B, gx, st);
+}
+
+// istft backward: gp = gx / wn (istft_bwd_norm_kernel), then the stft framing and transform of
+// gp -- zero padding by n_fft/2, window = window**win_exp, ifftshifted when modulated -- with
+// the STFT_EPI_ISTFT_BWD epilogue, which writes (c_k / n_fft) C[k] into gSx.
+template <typename T>
+static int istft_bwd_t(const ssqb_istft_desc* d, const void* gx, long long B, void* gS,
+                       cudaStream_t st) {
+  const int M = d->n_fft;
+  IstftArgs<T> I;
+  memset(&I, 0, sizeof(I));
+  I.n_fft = M; I.hop = d->hop; I.n_hops = (int)d->n_hops; I.modulated = d->modulated;
+  I.B = (int)B; I.N = d->N;
+  I.max_hops = (d->N - 1) / d->hop + 1;
+  I.tiny = d->dtype == SSQB_F32 ? 1.1754943508222875e-38 : 2.2250738585072014e-308;
+  std::vector<T> win((size_t)M, (T)1);
+  const T* wexp = (const T*)d->wexp_host;
+  for (int l = 0; l < M; ++l) {
+    const int m = d->modulated ? (l + M / 2) % M : l;      // ifftshift
+    if (wexp) win[l] = wexp[m];
+  }
+  BlobBuilder bb;
+  const std::vector<cx<T>>& tw = roots<T>(M);
+  const size_t o_tw = bb.put(tw.data(), sizeof(cx<T>) * M);
+  const size_t o_win = bb.put(win.data(), sizeof(T) * M);
+  const size_t o_wpow = bb.put(d->wpow_host, sizeof(T) * M);
+  unsigned char* blob = nullptr;
+  int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
+  I.wpow = (const T*)(blob + o_wpow);
+  T* gp = nullptr;                                           // [B][N], the size of gx
+  SSQB_CUDA(cudaMallocAsync((void**)&gp, sizeof(T) * (size_t)B * (size_t)d->N, st));
+  istft_bwd_norm_kernel<T><<<(unsigned)((d->N + 255) / 256), 256, 0, st>>>(I, (const T*)gx, gp);
+  SSQB_LAUNCH_CHECK();
+  StftArgs<T> A;
+  memset(&A, 0, sizeof(A));
+  A.N = d->N; A.n_hops = d->n_hops; A.n_fft = M; A.hop = d->hop;
+  A.n1 = M / 2; A.padtype = SSQB_PAD_ZERO; A.modulated = d->modulated; A.B = (int)B;
+  A.x = gp; A.win = (const T*)(blob + o_win); A.dwin = nullptr;
+  A.kappa = (T)1; A.inv_kappa = (T)1;
+  A.Sx = (cx<T>*)gS; A.tw = (const cx<T>*)(blob + o_tw);
+  const int logm = ilog2_exact(M);
+  if (logm >= 1 && logm <= 12 && (Tile<T>::ELEMS >> logm) >= 1)
+    rc = launch_stft_pow2<T, STFT_EPI_ISTFT_BWD>(A, logm, st);
+  else
+    rc = launch_stft_generic<T, STFT_EPI_ISTFT_BWD>(A, st);
+  cudaFreeAsync(gp, st);
+  return rc;
+}
+
+int run_istft_backward(const ssqb_istft_desc* d, const void* gx, long long B, void* gSx,
+                       cudaStream_t st) {
+  if (!d || !gx || !gSx || !d->wpow_host) return set_error(SSQB_E_ARG, "null pointer");
+  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || d->n_hops < 1 || B < 1)
+    return set_error(SSQB_E_ARG, "bad shape");
+  if ((d->n_hops - 1) * (long long)d->hop > d->N - 1)
+    return set_error(SSQB_E_ARG, "frames reach beyond N + n_fft - 1 samples");
+  return d->dtype == SSQB_F32 ? istft_bwd_t<float>(d, gx, B, gSx, st)
+                              : istft_bwd_t<double>(d, gx, B, gSx, st);
 }
 
 }  // namespace ssqb
