@@ -191,16 +191,17 @@ __device__ __forceinline__ float lg2_ftz(float a) {
   float r; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(a)); return r;
 }
 
-// Tj = &Tx[signal][0][jo]; rows are `rowbytes` apart (one 32 x 32 -> 64 bit multiply-add)
+// Tj = &Tx[signal][0][jo]; rows are `rowbytes` apart (one 32 x 32 -> 64 bit multiply-add).
+// Returns false, having done nothing, when the point needs ssq_point_exact.
 template <typename T>
-__device__ __forceinline__ void ssq_point(cx<T> W, cx<T> dW, cx<T>* __restrict__ Tj,
-                                          unsigned rowbytes, T cre, double cwide, T g2lo, T g2hi,
-                                          bool fast_ok, const ReassignGrid& g) {
+__device__ __forceinline__ bool ssq_point_fast(cx<T> W, cx<T> dW, cx<T>* __restrict__ Tj,
+                                               unsigned rowbytes, T cre, double cwide, T g2lo,
+                                               T g2hi, bool fast_ok, const ReassignGrid& g) {
   // num / den with the reference's roundings (algos.py:916-918)
   T den, num;
   ssq_num_den(W, dW, num, den);
   // inactive points (|Wx| <= gamma, ~half of a typical plane) leave first
-  if (den < g2lo) return;
+  if (den < g2lo) return true;
   float wf;
   if (sizeof(T) == 4) wf = fdiv_ftz(fabsf((float)num), (float)den * 6.2831853f);
   else                wf = (float)(fabs((double)num) / ((double)den * SSQB_TWO_PI));
@@ -217,13 +218,21 @@ __device__ __forceinline__ void ssq_point(cx<T> W, cx<T> dW, cx<T>* __restrict__
   const float vc = fminf(fmaxf(v, -0.25f), g.fvhi);
   const float r = rintf(vc);
   ok = ok && (fabsf(vc - r) < g.fhalf);
-  if (!ok) { ssq_point_exact<T>(W, dW, Tj, rowbytes, cwide, g); return; }
+  if (!ok) return false;
   int kk = (int)r;
   if (g.flipud) kk = g.omax - kk;
   T re, im;
   if (g.const_wide) { re = (T)((double)W.x * cwide); im = (T)((double)W.y * cwide); }
   else              { const cx<T> c = cscale<T>(W, cre); re = c.x; im = c.y; }
   atomic_add_cx<T>(row_ptr<T>(Tj, kk, rowbytes), re, im);
+  return true;
+}
+template <typename T>
+__device__ __forceinline__ void ssq_point(cx<T> W, cx<T> dW, cx<T>* __restrict__ Tj,
+                                          unsigned rowbytes, T cre, double cwide, T g2lo, T g2hi,
+                                          bool fast_ok, const ReassignGrid& g) {
+  if (!ssq_point_fast<T>(W, dW, Tj, rowbytes, cre, cwide, g2lo, g2hi, fast_ok, g))
+    ssq_point_exact<T>(W, dW, Tj, rowbytes, cwide, g);
 }
 
 // shared-memory geometry of a row-kernel tile (shared with the host-side launch code)

@@ -277,10 +277,10 @@ enum SblkShare { SBLK_ALONE, SBLK_BESIDE_GRID, SBLK_TAIL };
 
 template <typename T, int NARR, bool SSQ>
 static int launch_sblk_rows_t(const SblkArgs<T>& S, SblkShare share, cudaStream_t st) {
-  constexpr int LP = SblkGeom<T>::LOG_P;
+  constexpr int LP = SblkGeom<T>::LOG_P, NT = SblkGeom<T>::NT;
   using V4 = typename V4T<T>::type;
   size_t smem = ((size_t)1 << LP) * (sizeof(V4) + sizeof(cx<T>));
-  auto kern = sblk_rows_kernel<T, LP, NARR, SSQ>;
+  auto kern = sblk_rows_kernel<T, LP, SblkGeom<T>::LOG_R, NARR, SSQ>;
   static bool attr_set = false;
   static int sms = 132, per = 2, prio_high = 0;
   if (!attr_set) {
@@ -288,7 +288,7 @@ static int launch_sblk_rows_t(const SblkArgs<T>& S, SblkShare share, cudaStream_
     int dev = 0, least = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kern, (1 << LP) / 8, smem) != cudaSuccess || per < 1) per = 1;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kern, NT, smem) != cudaSuccess || per < 1) per = 1;
     SSQB_CUDA(cudaDeviceGetStreamPriorityRange(&least, &prio_high));
     attr_set = true;
   }
@@ -298,7 +298,7 @@ static int launch_sblk_rows_t(const SblkArgs<T>& S, SblkShare share, cudaStream_
   const unsigned g = (unsigned)(items < ctas ? items : ctas);
   if (g < 1) return 0;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(g); cfg.blockDim = dim3((1 << LP) / 8); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cfg.gridDim = dim3(g); cfg.blockDim = dim3(NT); cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributePriority; attr[0].val.priority = prio_high;
   cfg.attrs = attr; cfg.numAttrs = (share == SBLK_BESIDE_GRID) ? 1 : 0;
@@ -777,7 +777,7 @@ struct CwtPlan : public CwtPlanBase {
         else if (S < 0 && d.wavelet != SSQB_WAV_TABLE && lo[a] >= 0 &&
                  lo[a] + len[a] - 1 == d.n_up / 2 && (-S) + 2 * SBLK_TAPER_HALF <= 512) sc = 2;
         if (sc >= 0) {
-          SblkRow r; r.a = a; r.cut = (sc == 2) ? 1 : 0;
+          SblkRow r; r.a = a; r.cut = (sc == 2) ? 1 : 0; r.groups = 0;
           r.tab_off = (long long)sblk[sc].rows.size() << SBLK_LOGP;
           sblk[sc].rows.push_back(r);
           routed = true;
@@ -882,18 +882,19 @@ struct CwtPlan : public CwtPlanBase {
       if (!ev_sblk_ready[c]) SSQB_CUDA(cudaEventCreateWithFlags(&ev_sblk_ready[c], cudaEventDisableTiming));
     SSQB_CUDA(rootsP_d.upload(make_roots<T>(Pn, 1, Pn)));
     {
-      // per-stage twiddles of sblk_rows_kernel: stage Ns (radix r) at Ns - 8, [q - 1][k]
+      // per-stage twiddles of sblk_rows_kernel: stage Ns (radix r) at Ns - R, [q - 1][k]
+      constexpr int R = 1 << SblkGeom<T>::LOG_R;
       std::vector<cx<T>> tws((size_t)Pn, mkc<T>((T)1, (T)0));
       auto fill = [&](long long Ns, int r) {
         const long long tstep = Pn / (Ns * r);
         for (int q = 1; q < r; ++q)
           for (long long k = 0; k < Ns; ++k) {
             const double ang = 2.0 * M_PI * (double)((k * q * tstep) % Pn) / (double)Pn;
-            tws[(size_t)(Ns - 8 + (q - 1) * Ns + k)] = mkc<T>((T)cos(ang), (T)sin(ang));
+            tws[(size_t)(Ns - R + (q - 1) * Ns + k)] = mkc<T>((T)cos(ang), (T)sin(ang));
           }
       };
-      long long Ns = 8;
-      for (; Ns * 8 <= Pn; Ns *= 8) fill(Ns, 8);
+      long long Ns = R;
+      for (; Ns * R <= Pn; Ns *= R) fill(Ns, R);
       if (Ns * 4 == Pn) fill(Ns, 4);
       SSQB_CUDA(twsP_d.upload(tws));
     }
@@ -905,6 +906,8 @@ struct CwtPlan : public CwtPlanBase {
       S.rows = K.rows_d.p; S.n_rows = (int)K.rows.size(); S.sigma = (T)SBLK_SIGMA;
       sblk_tab_kernel<T, SBLK_LOGP><<<dim3((unsigned)(Pn / 256), (unsigned)K.rows.size()), 256>>>(
           S, K.p_d.p, K.pd_d.p);
+      SSQB_LAUNCH_CHECK();
+      sblk_groups_kernel<T, SBLK_LOGP><<<(unsigned)K.rows.size(), 256>>>(K.rows_d.p, K.p_d.p);
       SSQB_LAUNCH_CHECK();
     }
     if (have_cut) {

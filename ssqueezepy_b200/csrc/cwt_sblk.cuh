@@ -10,8 +10,9 @@
 // samples gives the exact result on the block's inner P - 2*h2 samples, so per (signal, row,
 // block): spectrum of the block (shared by all rows, `sblk_fwd_kernel`) x the wavelet sampled
 // on the block's frequency grid -> one P-point inverse FFT of W and dW together (16-byte
-// elements, radix-8 Stockham, first stage straight from global memory, last stage straight
-// into the epilogue registers) -> fused epilogue.  No scratch, no second kernel.
+// elements, radix-16 (float32) / radix-8 (float64) Stockham, first stage straight from global
+// memory, last stage straight into the epilogue registers) -> fused epilogue.  No scratch, no
+// second kernel.
 //
 // Rows whose spectrum is CUT at Nyquist (scale * pi inside the wavelet's support: the
 // reference samples psih on [0, pi] and nothing above) are not short filters -- the jump at
@@ -33,6 +34,8 @@ struct SblkRow {
   int a;                       // scale index
   int cut;                     // 1: cut at Nyquist (source = analytic part, tapered table)
   long long tab_off;           // row * P into tab_p / tab_pd
+  unsigned groups;             // bit q: tab_p is non-zero somewhere on bins [q NT, (q+1) NT),
+                               // written by sblk_groups_kernel (NT: threads of a row CTA)
 };
 
 template <typename T>
@@ -56,7 +59,13 @@ struct SblkArgs {
                                // null: each CTA walks the items in steps of gridDim.x
 };
 
-template <typename T> struct SblkGeom { static constexpr int LOG_P = (sizeof(T) == 4) ? 12 : 11; };
+// row transform: radix 16 in float32 (4096 = 16^3: two exchanges); radix 8 with a radix-4 tail in
+// float64 (2048 = 8^3 * 4), where 16 points of 32 bytes for W and dW would not fit the registers
+template <typename T> struct SblkGeom {
+  static constexpr int LOG_P = (sizeof(T) == 4) ? 12 : 11;
+  static constexpr int LOG_R = (sizeof(T) == 4) ? 4 : 3;
+  static constexpr int NT = (1 << LOG_P) >> LOG_R;     // threads of a row CTA
+};
 
 // psih at w = scale * xi (no Nyquist halving): wavelets.py:525-527, _gmw.py:212-219
 template <typename T>
@@ -90,6 +99,25 @@ sblk_tab_kernel(const SblkArgs<T> S, T* __restrict__ tab_p, T* __restrict__ tab_
   }
   tab_p[ri.tab_off + j] = p;
   tab_pd[ri.tab_off + j] = p * ((T)xi / A.dt);
+}
+
+// SblkRow::groups of row blockIdx.x, from its finished table: stage 0 of sblk_rows_kernel loads
+// bins j + NT q only where bit q is set (most rows are exactly zero on whole groups; a plain GMW
+// row on every bin above P/2), and a group left out contributes exact zeros either way
+template <typename T, int LOG_P>
+__global__ void __launch_bounds__(256)
+sblk_groups_kernel(SblkRow* __restrict__ rows, const T* __restrict__ tab_p) {
+  constexpr int P = 1 << LOG_P, NT = SblkGeom<T>::NT;
+  __shared__ unsigned s_or;
+  if (threadIdx.x == 0) s_or = 0;
+  __syncthreads();
+  const T* __restrict__ tp = tab_p + rows[blockIdx.x].tab_off;
+  unsigned m = 0;
+  for (int e = threadIdx.x; e < P; e += blockDim.x)
+    if (tp[e] != (T)0) m |= 1u << (e / NT);           // NaN counts as non-zero
+  atomicOr(&s_or, m);
+  __syncthreads();
+  if (threadIdx.x == 0) rows[blockIdx.x].groups = s_or;
 }
 
 // ---- block spectra ------------------------------------------------------------------------
@@ -126,25 +154,43 @@ sblk_fwd_kernel(const SblkArgs<T> S) {
 }
 
 // ---- rows -----------------------------------------------------------------------------------
-// buffer between stage 0 and stage 1: element i lives at i ^ ((i >> 3) & 7), which makes
-// both the stage-0 stores (stride 8 elements across lanes) and the stage-1 loads conflict free
-__device__ __forceinline__ int sblk_swz(int i) { return i ^ ((i >> 3) & 7); }
+// buffer between stage 0 and stage 1: element i lives at i ^ ((i >> LOG_R) & 7), which makes
+// both the stage-0 stores (stride R elements across lanes) and the stage-1 loads conflict free
+// (a warp's 16-byte accesses are served 8 lanes at a time)
+template <int LOG_R>
+__device__ __forceinline__ int sblk_swz(int i) { return i ^ ((i >> LOG_R) & 7); }
 
-template <typename T, int LOG_P, int NARR, bool SSQ>
-__global__ void __launch_bounds__((1 << LOG_P) / 8, 2)
+// twiddles w^q, q = 1 .. R-1, of one butterfly: w, w^2, w^4 (and w^8) from the stage's table
+// (tws = its [0][k] entry, rows Ns apart), the other powers by multiplication: a complex product
+// costs less than a shared-memory load (the kernel's top stall is the shared-memory queue)
+template <typename T, int R>
+__device__ __forceinline__ void sblk_twiddles(const cx<T>* __restrict__ tws, int Ns, cx<T>* w) {
+  w[1] = tws[0]; w[2] = tws[Ns]; w[4] = tws[3 * Ns];
+  w[3] = cmul<T>(w[1], w[2]); w[5] = cmul<T>(w[4], w[1]);
+  w[6] = cmul<T>(w[4], w[2]); w[7] = cmul<T>(w[4], w[3]);
+  if constexpr (R == 16) {
+    w[8] = tws[7 * Ns];
+#pragma unroll
+    for (int q = 9; q < 16; ++q) w[q] = cmul<T>(w[8], w[q - 8]);
+  }
+}
+
+template <typename T, int LOG_P, int LOG_R, int NARR, bool SSQ>
+__global__ void __launch_bounds__((1 << LOG_P) >> LOG_R, 2)
 sblk_rows_kernel(const SblkArgs<T> S) {
-  constexpr int P = 1 << LOG_P, NT = P / 8;
-  constexpr int NR8 = LOG_P / 3;                       // radix-8 stages
-  constexpr int TAIL = 1 << (LOG_P - 3 * NR8);         // 1 (none) or 4
-  static_assert(TAIL == 1 || TAIL == 4, "P = 8^k or 4 * 8^k");
-  constexpr int NOUT = 8;                              // outputs per thread: t = j + NT * m
+  constexpr int P = 1 << LOG_P, R = 1 << LOG_R, NT = P / R;
+  static_assert(R == 8 || R == 16, "radix 8 or 16");
+  constexpr int NR = LOG_P / LOG_R;                    // radix-R stages
+  constexpr int TAIL = 1 << (LOG_P - LOG_R * NR);      // 1 (none) or 4
+  static_assert(TAIL == 1 || (TAIL == 4 && R == 8), "P = R^k or 4 * 8^k");
+  constexpr int NOUT = R;                              // outputs per thread: t = j + NT * m
   using V4 = typename V4T<T>::type;
   const CwtArgs<T>& A = S.A;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   V4* s = reinterpret_cast<V4*>(smem_raw);             // [P]
   // twiddles per stage, [q - 1][k] with k = butterfly index mod Ns fastest: the lanes of a warp
   // read consecutive entries (the natural table, indexed k*q*step, costs 8-16 wavefronts per
-  // load).  Stage Ns (radix r) starts at Ns - 8 and holds (r - 1) * Ns entries: < P in total.
+  // load).  Stage Ns (radix r) starts at Ns - R and holds (r - 1) * Ns entries: < P in total.
   cx<T>* tw = reinterpret_cast<cx<T>*>(s + P);         // [P]
   // item = (block k, row r, signal b), k fastest.  Without a counter a CTA walks the items in
   // steps of gridDim.x.  With S.item_ctr the items are taken from the counter: the CTAs of this
@@ -162,15 +208,6 @@ sblk_rows_kernel(const SblkArgs<T> S) {
   if (it >= items) return;
 
   const int Nout = (int)A.Nout;
-  T g2lo = 0, g2hi = 0; bool fast_ok = false; unsigned rowbytes = 0;
-  if (SSQ) {
-    const T g2 = (T)(A.grid.gamma * A.grid.gamma);
-    const T g2tol = g2 * (T)(sizeof(T) == 4 ? 1e-5 : 1e-13);
-    g2lo = g2 - g2tol;
-    g2hi = fmax(g2 + g2tol, (T)1e-30);
-    fast_ok = (A.grid.kind <= 1) && (A.grid.ftol < 0.25f);
-    rowbytes = (unsigned)Nout * (unsigned)sizeof(cx<T>);
-  }
   const T xi_step = (T)(SSQB_TWO_PI / (double)P) / A.dt;
 
 #pragma unroll 1
@@ -180,19 +217,23 @@ sblk_rows_kernel(const SblkArgs<T> S) {
     const int r = (int)(rr % (unsigned)S.n_rows), b = (int)(rr / (unsigned)S.n_rows);
     const SblkRow ri = S.rows[r];
 
-    cx<T> vw[8], vd[8];
+    cx<T> vw[R], vd[R];
     // ---- stage 0 (Ns = 1) from global memory: inputs j + NT q ---------------------------------
     {
-      cx<T> xv[8]; T pv[8];
+      cx<T> xv[R]; T pv[R];
       const cx<T>* __restrict__ X = S.Xs + (((long long)b * S.nblk + k) << LOG_P);
       const T* __restrict__ tp = S.tab_p + ri.tab_off;
+      // groups where the table is zero are not loaded (the same for the whole CTA)
 #pragma unroll
-      for (int q = 0; q < 8; ++q) { xv[q] = __ldg(&X[j + NT * q]); pv[q] = __ldg(&tp[j + NT * q]); }
+      for (int q = 0; q < R; ++q) {
+        if ((ri.groups >> q) & 1u) { xv[q] = __ldg(&X[j + NT * q]); pv[q] = __ldg(&tp[j + NT * q]); }
+        else { xv[q] = mkc<T>((T)0, (T)0); pv[q] = (T)0; }
+      }
       // dW spectrum = W spectrum * 1j * xi / dt (_cwt.py:175): xi of bin j + NT q on the block grid,
       // signed (bins above P/2 are negative frequencies) except for the rows cut at Nyquist, whose
       // table runs over [0, 2 pi) -- the same convention as sblk_tab_kernel
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
+      for (int q = 0; q < R; ++q) {
         vw[q] = cscale<T>(xv[q], pv[q]);
         if (NARR == 2) {
           const int bin = j + NT * q;
@@ -203,48 +244,43 @@ sblk_rows_kernel(const SblkArgs<T> S) {
         }
       }
     }
-    idft<T, 8>(vw); if (NARR == 2) idft<T, 8>(vd);
+    idft<T, R>(vw); if (NARR == 2) idft<T, R>(vd);
     __syncthreads();                                   // previous item is done with s and s_next
     unsigned claim = 0;
     if (ctr && j == 0) claim = atomicAdd(S.item_ctr, 1u);
 #pragma unroll
-    for (int q = 0; q < 8; ++q) {
+    for (int q = 0; q < R; ++q) {
       V4 o; o.x = vw[q].x; o.y = vw[q].y; o.z = vd[q].x; o.w = vd[q].y;
-      s[sblk_swz(8 * j + q)] = o;
+      s[sblk_swz<LOG_R>(R * j + q)] = o;
     }
     __syncthreads();
-    // ---- middle radix-8 stages (Ns = 8, 64, ..), in place ------------------------------------
-    constexpr int NMID = (TAIL == 1) ? NR8 - 2 : NR8 - 1;
+    // ---- middle radix-R stages (Ns = R, R^2, ..), in place -------------------------------------
+    constexpr int NMID = (TAIL == 1) ? NR - 2 : NR - 1;
     static_assert(NMID >= 1, "the next item is handed over in the last middle stage");
 #pragma unroll
     for (int st = 0; st < NMID; ++st) {
-      const int Ns = 8 << (3 * st);
+      const int Ns = R << (LOG_R * st);
       const int kk = j & (Ns - 1);
-      const cx<T>* __restrict__ tws = tw + (Ns - 8) + kk;
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
+      for (int q = 0; q < R; ++q) {
         const int i = j + NT * q;
-        const V4 v = s[st == 0 ? sblk_swz(i) : i];
+        const V4 v = s[st == 0 ? sblk_swz<LOG_R>(i) : i];
         vw[q] = mkc<T>(v.x, v.y); vd[q] = mkc<T>(v.z, v.w);
       }
       {
-        // w, w^2, w^4 from the table, the other powers by multiplication: 4 complex products
-        // instead of 4 shared-memory loads (the kernel's top stall is the shared-memory queue)
-        cx<T> w[8];
-        w[1] = tws[0]; w[2] = tws[Ns]; w[4] = tws[3 * Ns];
-        w[3] = cmul<T>(w[1], w[2]); w[5] = cmul<T>(w[4], w[1]);
-        w[6] = cmul<T>(w[4], w[2]); w[7] = cmul<T>(w[4], w[3]);
+        cx<T> w[R];
+        sblk_twiddles<T, R>(tw + (Ns - R) + kk, Ns, w);
 #pragma unroll
-        for (int q = 1; q < 8; ++q) {
+        for (int q = 1; q < R; ++q) {
           vw[q] = cmul<T>(vw[q], w[q]); if (NARR == 2) vd[q] = cmul<T>(vd[q], w[q]);
         }
       }
-      idft<T, 8>(vw); if (NARR == 2) idft<T, 8>(vd);
+      idft<T, R>(vw); if (NARR == 2) idft<T, R>(vd);
       if (ctr && st == NMID - 1 && j == 0) s_next = claim;
       __syncthreads();
-      const int j0 = (j - kk) * 8 + kk;
+      const int j0 = (j - kk) * R + kk;
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
+      for (int q = 0; q < R; ++q) {
         V4 o; o.x = vw[q].x; o.y = vw[q].y; o.z = vd[q].x; o.w = vd[q].y;
         s[j0 + Ns * q] = o;
       }
@@ -253,26 +289,21 @@ sblk_rows_kernel(const SblkArgs<T> S) {
     const unsigned it_next = ctr ? s_next : it + gridDim.x;
     // ---- last stage: outputs t = j + NT m stay in registers -----------------------------------
     if constexpr (TAIL == 1) {
-      // radix 8, Ns = P/8 = NT: k = j
+      // radix R, Ns = P/R = NT: k = j
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
+      for (int q = 0; q < R; ++q) {
         const V4 v = s[j + NT * q];
         vw[q] = mkc<T>(v.x, v.y); vd[q] = mkc<T>(v.z, v.w);
       }
       {
-        const cx<T>* __restrict__ tws = tw + (NT - 8) + j;
-        // w, w^2, w^4 from the table, the other powers by multiplication: 4 complex products
-        // instead of 4 shared-memory loads (the kernel's top stall is the shared-memory queue)
-        cx<T> w[8];
-        w[1] = tws[0]; w[2] = tws[NT]; w[4] = tws[3 * NT];
-        w[3] = cmul<T>(w[1], w[2]); w[5] = cmul<T>(w[4], w[1]);
-        w[6] = cmul<T>(w[4], w[2]); w[7] = cmul<T>(w[4], w[3]);
+        cx<T> w[R];
+        sblk_twiddles<T, R>(tw + (NT - R) + j, NT, w);
 #pragma unroll
-        for (int q = 1; q < 8; ++q) {
+        for (int q = 1; q < R; ++q) {
           vw[q] = cmul<T>(vw[q], w[q]); if (NARR == 2) vd[q] = cmul<T>(vd[q], w[q]);
         }
       }
-      idft<T, 8>(vw); if (NARR == 2) idft<T, 8>(vd);
+      idft<T, R>(vw); if (NARR == 2) idft<T, R>(vd);
     } else {
       // radix 4, Ns = P/4 = 2 NT: butterflies j and j + NT; outputs jj + 2 NT q
       cx<T> a0[4], a1[4], d0[4], d1[4];
@@ -284,7 +315,7 @@ sblk_rows_kernel(const SblkArgs<T> S) {
       }
 #pragma unroll
       for (int q = 1; q < 4; ++q) {
-        const cx<T> w0 = tw[(2 * NT - 8) + (q - 1) * 2 * NT + j], w1 = tw[(2 * NT - 8) + (q - 1) * 2 * NT + j + NT];
+        const cx<T> w0 = tw[(2 * NT - R) + (q - 1) * 2 * NT + j], w1 = tw[(2 * NT - R) + (q - 1) * 2 * NT + j + NT];
         a0[q] = cmul<T>(a0[q], w0); a1[q] = cmul<T>(a1[q], w1);
         if (NARR == 2) { d0[q] = cmul<T>(d0[q], w0); d1[q] = cmul<T>(d1[q], w1); }
       }
@@ -305,8 +336,24 @@ sblk_rows_kernel(const SblkArgs<T> S) {
     cx<T>* __restrict__ Zrow = (SSQ && b < A.zero_next) ? A.Tx + row * Nout + A.zero_off : nullptr;   // zero-ahead
     const T mlt = (!SSQ && A.out_mul != nullptr) ? A.out_mul[a] : (T)1;
     double cwide = 0; T cre = 0;
-    if (SSQ) { cwide = A.cst[a]; cre = (T)cwide; }
+    // reassignment constants are formed here, not once per CTA: live through the transform they
+    // would cost registers the 16 points of W and dW need
+    T g2lo = 0, g2hi = 0; bool fast_ok = false; unsigned rowbytes = 0;
+    if (SSQ) {
+      cwide = A.cst[a]; cre = (T)cwide;
+      const T g2 = (T)(A.grid.gamma * A.grid.gamma);
+      const T g2tol = g2 * (T)(sizeof(T) == 4 ? 1e-5 : 1e-13);
+      g2lo = g2 - g2tol;
+      g2hi = fmax(g2 + g2tol, (T)1e-30);
+      fast_ok = (A.grid.kind <= 1) && (A.grid.ftol < 0.25f);
+      rowbytes = (unsigned)Nout * (unsigned)sizeof(cx<T>);
+    }
     const int jbase = k * S.hop - S.h2;
+    // outputs m that need the exact reassignment.  That path is an out-of-line call; made with the
+    // NOUT points of W and dW live it would spill them, so it runs after the loop, from W and dW
+    // parked in this thread's own slots of s (the last stage read s[j + NT m] and nothing else
+    // touches them before the next item's first barrier)
+    unsigned exact = 0;
 #pragma unroll
     for (int m = 0; m < NOUT; ++m) {
       const int t = j + NT * m;
@@ -320,9 +367,21 @@ sblk_rows_kernel(const SblkArgs<T> S) {
           Wrow[jo] = W;
           if (S.write_dWx) dWrow[jo] = dW;
           if (Zrow) Zrow[jo] = mkc<T>((T)0, (T)0);
-          ssq_point<T>(W, dW, Tb + jo, rowbytes, cre, cwide, g2lo, g2hi, fast_ok, A.grid);
+          if (!ssq_point_fast<T>(W, dW, Tb + jo, rowbytes, cre, cwide, g2lo, g2hi, fast_ok, A.grid)) {
+            V4 o; o.x = W.x; o.y = W.y; o.z = dW.x; o.w = dW.y;
+            s[t] = o;
+            exact |= 1u << m;
+          }
         }
       }
+    }
+#pragma unroll 1
+    while (SSQ && exact) {
+      const int m = __ffs(exact) - 1;
+      exact &= exact - 1;
+      const int t = j + NT * m;
+      const V4 v = s[t];
+      ssq_point_exact<T>(mkc<T>(v.x, v.y), mkc<T>(v.z, v.w), Tb + (jbase + t), rowbytes, cwide, A.grid);
     }
     if (it_next >= items) break;
     it = it_next;

@@ -18,8 +18,16 @@
 namespace ssqb {
 
 template <typename T> struct Consts;
-template <> struct Consts<float>  { static __device__ __forceinline__ float  rsqrt2() { return 0.70710678118654752440f; } };
-template <> struct Consts<double> { static __device__ __forceinline__ double rsqrt2() { return 0.70710678118654752440; } };
+template <> struct Consts<float> {
+  static __device__ __forceinline__ float rsqrt2() { return 0.70710678118654752440f; }
+  static __device__ __forceinline__ float cos_pi8() { return 0.92387953251128675613f; }
+  static __device__ __forceinline__ float sin_pi8() { return 0.38268343236508977173f; }
+};
+template <> struct Consts<double> {
+  static __device__ __forceinline__ double rsqrt2() { return 0.70710678118654752440; }
+  static __device__ __forceinline__ double cos_pi8() { return 0.92387953251128675613; }
+  static __device__ __forceinline__ double sin_pi8() { return 0.38268343236508977173; }
+};
 
 // ---- in-register inverse DFTs ----------------------------------------------
 template <typename T> __device__ __forceinline__ void idft2(cx<T>* v) {
@@ -52,8 +60,39 @@ template <typename T> __device__ __forceinline__ void idft8(cx<T>* v) {
   v[1] = caxpy<T>(u5, h, b4); v[5] = caxpy<T>(u5, -h, b4);
   v[3] = caxpy<T>(u7, h, b6); v[7] = caxpy<T>(u7, -h, b6);
 }
+// 16 = 4 x 4: q = 4 q1 + q2, m = m1 + 4 m2.  Length-4 transforms over q1 for each q2, then the
+// twiddles exp(+2 pi i q2 m1 / 16), then length-4 transforms over q2 for each m1.
+template <typename T> __device__ __forceinline__ void idft16(cx<T>* v) {
+  const T h = Consts<T>::rsqrt2(), c = Consts<T>::cos_pi8(), s = Consts<T>::sin_pi8();
+  cx<T> y[4][4];                                          // [q2][m1]
+#pragma unroll
+  for (int q2 = 0; q2 < 4; ++q2) {
+    cx<T> a[4] = {v[q2], v[4 + q2], v[8 + q2], v[12 + q2]};
+    idft4<T>(a);
+#pragma unroll
+    for (int m1 = 0; m1 < 4; ++m1) y[q2][m1] = a[m1];
+  }
+  // exponents q2 * m1 = 1, 3, 9: general products; 2, 6: h * (1 + i), h * (-1 + i); 4: i
+  y[1][1] = cmul<T>(y[1][1], mkc<T>(c, s));
+  y[1][3] = cmul<T>(y[1][3], mkc<T>(s, c));
+  y[3][1] = cmul<T>(y[3][1], mkc<T>(s, c));
+  y[3][3] = cmul<T>(y[3][3], mkc<T>(-c, -s));
+  y[1][2] = cscale<T>(cadd<T>(y[1][2], cmuli<T>(y[1][2])), h);
+  y[2][1] = cscale<T>(cadd<T>(y[2][1], cmuli<T>(y[2][1])), h);
+  y[2][3] = cscale<T>(csub<T>(cmuli<T>(y[2][3]), y[2][3]), h);
+  y[3][2] = cscale<T>(csub<T>(cmuli<T>(y[3][2]), y[3][2]), h);
+  y[2][2] = cmuli<T>(y[2][2]);
+#pragma unroll
+  for (int m1 = 0; m1 < 4; ++m1) {
+    cx<T> b[4] = {y[0][m1], y[1][m1], y[2][m1], y[3][m1]};
+    idft4<T>(b);
+#pragma unroll
+    for (int m2 = 0; m2 < 4; ++m2) v[m1 + 4 * m2] = b[m2];
+  }
+}
 template <typename T, int RADIX> __device__ __forceinline__ void idft(cx<T>* v) {
-  if (RADIX == 8) idft8<T>(v);
+  if (RADIX == 16) idft16<T>(v);
+  else if (RADIX == 8) idft8<T>(v);
   else if (RADIX == 4) idft4<T>(v);
   else idft2<T>(v);
 }
