@@ -298,10 +298,12 @@ def _pad_geometry_for(N, padtype):
 class _CwtFn(torch.autograd.Function):
     """`cwt` as a differentiable torch op (the reference's GPU mode is differentiable because
     it is composed of torch ops, `_cwt.py:19`, `examples/reconstruction.py:38-70`): forward is
-    the plan's kernels, backward the adjoint `ssqb_cwt_backward`."""
+    the plan's kernels, backward the adjoint `ssqb_cwt_backward`.  A gradient that does not
+    reach Wx or dWx arrives as None and is passed to the library as NULL."""
 
     @staticmethod
     def forward(ctx, x2d, plan, derivative, out_mul, rpadded):
+        ctx.set_materialize_grads(False)
         ctx.plan, ctx.out_mul, ctx.rpadded = plan, out_mul, rpadded
         ctx.derivative = derivative
         Wx, dWx = plan.cwt(x2d.detach(), derivative=derivative, out_mul=out_mul,
@@ -312,6 +314,8 @@ class _CwtFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gW, gdW=None):
+        if gW is None and gdW is None:
+            return None, None, None, None, None
         plan = ctx.plan
         cdt = Bk.cplx_dtype(plan.dtype)
         gW = None if gW is None else gW.to(cdt).contiguous()

@@ -212,15 +212,30 @@ adj_accum_kernel(const CwtArgs<T> A, const cx<T>* __restrict__ Zh, cx<T>* __rest
   }
   acc[i] = s;
 }
+// gx[b][j] = Re g[b][n1 + j]: one thread per sample
 template <typename T>
 __global__ void __launch_bounds__(256)
 adj_unpad_kernel(const cx<T>* __restrict__ g, T* __restrict__ gx, long long N, long long n, long long n1,
-                 int padtype, long long B) {
+                 long long B) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= B * n) return;
-  const long long b = idx / n, t = idx - b * n;
-  const long long src = pad_src_index(t, n1, N, padtype);
-  if (src >= 0) atomicAdd(&gx[b * N + src], g[idx].x);
+  if (idx >= B * N) return;
+  const long long b = idx / N, j = idx - b * N;
+  gx[idx] = g[b * n + n1 + j].x;
+}
+// then the padding: gx[b][j] += Re g[b][t] for the pad samples t that copy j, ascending t (the
+// groups of `pad_groups`, tab = off | j | t).  One thread per copied sample: no atomics.
+template <typename T>
+__global__ void __launch_bounds__(256)
+adj_fold_kernel(const cx<T>* __restrict__ g, T* __restrict__ gx, long long N, long long n,
+                const long long* __restrict__ tab, long long ng, long long B) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= B * ng) return;
+  const long long b = idx / ng, q = idx - b * ng;
+  const long long* off = tab; const long long* js = tab + ng + 1; const long long* ts = js + ng;
+  T* o = gx + b * N + js[q];
+  T s = *o;
+  for (long long e = off[q]; e < off[q + 1]; ++e) s += g[b * n + ts[e]].x;
+  *o = s;
 }
 
 template <typename T>
@@ -228,11 +243,24 @@ struct CwtAdjoint {
   Gfft<T> fft; bool ready = false;
   DevBuf<cx<T>> Z, Zh, acc, gp;
   DevBuf<T> mul_d;
+  DevBuf<long long> pad_tab; long long n_groups = 0;
   // gW / gdW [B][na][Nout] (either may be null), gx [B][N] (overwritten)
   int run(const ssqb_cwt_desc& d, CwtArgs<T> A, const cx<T>* gW, const cx<T>* gdW, long long B,
           const double* out_mul_host, bool rpadded, T* gx, cudaStream_t st) {
     const long long n = d.n_up, Nout = rpadded ? n : d.N, off = rpadded ? 0 : d.n1;
-    if (!ready) { int rc = fft.init(n); if (rc) return rc; ready = true; }
+    if (!ready) {
+      int rc = fft.init(n); if (rc) return rc;
+      const PadGroups pg = pad_groups(d.N, d.n1, n, d.padtype);
+      std::vector<long long> tab(pg.off);
+      tab.insert(tab.end(), pg.j.begin(), pg.j.end());
+      tab.insert(tab.end(), pg.t.begin(), pg.t.end());
+      SSQB_CUDA(pad_tab.ensure(tab.size()));
+      SSQB_CUDA(cudaMemcpyAsync(pad_tab.p, tab.data(), tab.size() * sizeof(long long),
+                                cudaMemcpyHostToDevice, st));
+      SSQB_CUDA(cudaStreamSynchronize(st));
+      n_groups = (long long)pg.j.size();
+      ready = true;
+    }
     const T* out_mul = nullptr;
     if (out_mul_host) {
       std::vector<T> m((size_t)d.na);
@@ -246,7 +274,6 @@ struct CwtAdjoint {
     SSQB_CUDA(Z.ensure((size_t)chunk * (size_t)n)); SSQB_CUDA(Zh.ensure((size_t)chunk * (size_t)n));
     SSQB_CUDA(acc.ensure((size_t)B * (size_t)n)); SSQB_CUDA(gp.ensure((size_t)B * (size_t)n));
     SSQB_CUDA(cudaMemsetAsync(acc.p, 0, (size_t)B * (size_t)n * sizeof(cx<T>), st));
-    SSQB_CUDA(cudaMemsetAsync(gx, 0, (size_t)B * (size_t)d.N * sizeof(T), st));
     for (long long b = 0; b < B; ++b)
       for (int pass = 0; pass < 2; ++pass) {
         const cx<T>* G = pass == 0 ? gW : gdW;
@@ -262,8 +289,13 @@ struct CwtAdjoint {
         }
       }
     int rc = fft.exec(acc.p, gp.p, B, +1, (T)(1.0 / (double)n), st); if (rc) return rc;
-    adj_unpad_kernel<T><<<(unsigned)((B * n + 255) / 256), 256, 0, st>>>(gp.p, gx, d.N, n, d.n1, d.padtype, B);
+    adj_unpad_kernel<T><<<(unsigned)((B * d.N + 255) / 256), 256, 0, st>>>(gp.p, gx, d.N, n, d.n1, B);
     SSQB_LAUNCH_CHECK();
+    if (n_groups > 0) {
+      adj_fold_kernel<T><<<(unsigned)((B * n_groups + 255) / 256), 256, 0, st>>>(gp.p, gx, d.N, n, pad_tab.p,
+                                                                                   n_groups, B);
+      SSQB_LAUNCH_CHECK();
+    }
     return 0;
   }
 };

@@ -11,6 +11,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
+#include <algorithm>
+#include <utility>
+#include <vector>
 
 namespace ssqb {
 
@@ -234,7 +237,7 @@ __device__ __forceinline__ int bin_fused(T A, T B, T C, T D, const ReassignGrid&
 
 // reflect / zero / symmetric / replicate / wrap index map of
 // ssqueezepy/utils/common.py:131-147 (np.pad modes).  Returns -1 for "zero".  Also called on
-// the host, where the stft backward groups the pad samples by the sample they copy.
+// the host, where `pad_groups` groups the pad samples by the sample they copy.
 __host__ __device__ __forceinline__ int64_t pad_src_index(int64_t t, int64_t n1, int64_t N, int padtype) {
   int64_t s = t - n1;
   if (s >= 0 && s < N) return s;
@@ -257,6 +260,29 @@ __host__ __device__ __forceinline__ int64_t pad_src_index(int64_t t, int64_t n1,
       return m;
     }
   }
+}
+
+// The pad samples t of a signal padded to [0, L) (t outside [n1, n1 + N)), grouped by the
+// sample they copy: group q is sample j[q], copied by t[off[q] .. off[q + 1]) in ascending t.
+// The backward passes of stft and cwt fold the padding with one thread per group, so every
+// sample's sum has one owner and a fixed order (no atomics).
+struct PadGroups { std::vector<long long> off, j, t; };
+inline PadGroups pad_groups(long long N, long long n1, long long L, int padtype) {
+  std::vector<std::pair<long long, long long>> jt;
+  for (long long t = 0; t < L; ++t) {
+    if (t == n1) t = n1 + N;                   // skip the unpadded part
+    if (t >= L) break;
+    const long long j = pad_src_index(t, n1, N, padtype);
+    if (j >= 0) jt.emplace_back(j, t);
+  }
+  std::sort(jt.begin(), jt.end());
+  PadGroups g;
+  for (size_t e = 0; e < jt.size(); ++e) {
+    if (e == 0 || jt[e].first != jt[e - 1].first) { g.off.push_back((long long)e); g.j.push_back(jt[e].first); }
+    g.t.push_back(jt[e].second);
+  }
+  g.off.push_back((long long)jt.size());
+  return g;
 }
 
 }  // namespace ssqb

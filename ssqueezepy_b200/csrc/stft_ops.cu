@@ -268,21 +268,9 @@ static int stft_bwd_t(const ssqb_stft_desc* d, const void* gS, const void* gdS, 
   const double kap = pack_kappa(win, dwin, M);
   A.kappa = (T)kap; A.inv_kappa = (T)(1.0 / kap);
   // pad samples t grouped by the sample j they copy, ascending t within a group
-  std::vector<std::pair<long long, long long>> jt;
-  const long long Np = d->N + M - 1;
-  for (long long t = 0; t < Np; ++t) {
-    if (t == d->n1) t = d->n1 + d->N;                  // skip the unpadded part
-    if (t >= Np) break;
-    const long long j = pad_src_index(t, d->n1, d->N, d->padtype);
-    if (j >= 0) jt.emplace_back(j, t);
-  }
-  std::sort(jt.begin(), jt.end());
-  std::vector<long long> off, js, ts;
-  for (size_t e = 0; e < jt.size(); ++e) {
-    if (e == 0 || jt[e].first != jt[e - 1].first) { off.push_back((long long)e); js.push_back(jt[e].first); }
-    ts.push_back(jt[e].second);
-  }
-  off.push_back((long long)jt.size());
+  const PadGroups pg = pad_groups(d->N, d->n1, d->N + M - 1, d->padtype);
+  const std::vector<long long>& off = pg.off; const std::vector<long long>& js = pg.j;
+  const std::vector<long long>& ts = pg.t;
   BlobBuilder bb;
   const std::vector<cx<T>>& tw = roots<T>(M);
   const size_t o_tw = bb.put(tw.data(), sizeof(cx<T>) * M);
