@@ -163,6 +163,20 @@ int ssqb_ssqueeze(int dtype, const void* Wx_dev, const void* dWx_dev, void* Tx_d
 int ssqb_indexed_sum(int dtype, const void* Wx_dev, const void* w_dev, void* Tx_dev,
                      int64_t B, int na, int64_t N, const ssqb_reassign_desc* r,
                      void* stream);
+/* backward of ssqb_ssqueeze and of the fused reassignment of ssqb_ssq_cwt_exec /
+ * ssqb_ssq_stft_exec for torch.autograd, bins held where the forward put them (same k, same
+ * gamma test; Tx is linear in Wx between bin and gamma crossings):
+ *   gWout[b][i][j] = gWx[b][i][j] + c_i * gTx[b][k(i,j)][j] if |Wx| > gamma, else gWx[b][i][j].
+ * The product is typed as the forward's accumulation.  gWx_dev may be NULL (= 0) and may equal
+ * gWout_dev.  Sfs_dev as in ssqb_ssqueeze.  One thread per point, no atomics.               */
+int ssqb_ssqueeze_backward(int dtype, const void* Wx_dev, const void* dWx_dev,
+                           const void* gTx_dev, const void* gWx_dev, void* gWout_dev,
+                           int64_t B, int na, int64_t N, const ssqb_reassign_desc* r,
+                           const void* Sfs_dev, void* stream);
+/* backward of ssqb_indexed_sum (bins from the stored w, inf skipped); otherwise as above */
+int ssqb_indexed_sum_backward(int dtype, const void* w_dev, const void* gTx_dev,
+                              const void* gWx_dev, void* gWout_dev, int64_t B, int na,
+                              int64_t N, const ssqb_reassign_desc* r, void* stream);
 /* phase_cwt_cpu / phase_cwt_gpu (algos.py:706-781); total = number of elements */
 int ssqb_phase_cwt(int dtype, const void* Wx_dev, const void* dWx_dev, void* w_dev,
                    int64_t total, double gamma, void* stream);
@@ -217,6 +231,12 @@ int ssqb_stft_backward(const ssqb_stft_desc* d, const void* gSx_dev, const void*
 int ssqb_colsum_real(int dtype, int wide, const void* M_dev, int64_t B, int na, int64_t N,
                      const double* div_host, double scale, int has_scale, void* out_dev,
                      void* stream);
+/* backward of ssqb_colsum_real: gM[b][a][j] = scale / div[a] * gout[b][j] (imaginary part 0),
+ * the factor taken in float64.  gout_dev [B][N] in the forward's output type (float64 when
+ * `wide` or float64 data); gM_dev [B][na][N] complex dtype, overwritten.                 */
+int ssqb_colsum_real_backward(int dtype, int wide, const void* gout_dev, int64_t B, int na,
+                              int64_t N, const double* div_host, double scale, int has_scale,
+                              void* gM_dev, void* stream);
 /* `_invert_components` (_ssq_cwt.py:380-403): M_dev [na][N]; cc_dev, cw_dev int32 [N][K];
  * out_dev float64 [K+1][N] (components, then the uncovered remainder), times `scale`.  */
 int ssqb_invert_components(int dtype, const void* M_dev, int na, int64_t N,

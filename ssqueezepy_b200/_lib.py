@@ -32,7 +32,8 @@ SYMBOLS = [
     'ssqb_indexed_sum', 'ssqb_phase_cwt', 'ssqb_phase_stft', 'ssqb_stft_exec',
     'ssqb_ssq_stft_exec', 'ssqb_ssq_stft_exec_host',
     'ssqb_colsum_real', 'ssqb_invert_components', 'ssqb_istft_exec', 'ssqb_extract_ridges', 'ssqb_cwt_backward',
-    'ssqb_stft_backward', 'ssqb_istft_backward',
+    'ssqb_stft_backward', 'ssqb_istft_backward', 'ssqb_ssqueeze_backward',
+    'ssqb_indexed_sum_backward', 'ssqb_colsum_real_backward',
 ]
 
 
@@ -97,6 +98,12 @@ def _bind(lib):
                                   C.POINTER(ReassignDesc), vp, vp]
     lib.ssqb_indexed_sum.argtypes = [ci, vp, vp, vp, i64, ci, i64,
                                      C.POINTER(ReassignDesc), vp]
+    lib.ssqb_ssqueeze_backward.argtypes = [ci, vp, vp, vp, vp, vp, i64, ci, i64,
+                                           C.POINTER(ReassignDesc), vp, vp]
+    lib.ssqb_indexed_sum_backward.argtypes = [ci, vp, vp, vp, vp, i64, ci, i64,
+                                              C.POINTER(ReassignDesc), vp]
+    lib.ssqb_colsum_real_backward.argtypes = [ci, ci, vp, i64, ci, i64, C.POINTER(dbl), dbl, ci,
+                                              vp, vp]
     lib.ssqb_phase_cwt.argtypes = [ci, vp, vp, vp, i64, dbl, vp]
     lib.ssqb_phase_stft.argtypes = [ci, vp, vp, vp, vp, i64, ci, i64, dbl, vp]
     lib.ssqb_stft_exec.argtypes = [C.POINTER(StftDesc), vp, i64, vp, vp, vp]

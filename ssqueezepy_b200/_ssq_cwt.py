@@ -10,10 +10,11 @@ for (`get_dWx`, `get_w`).
 import numpy as np
 import torch
 
-from . import backend as Bk
+from . import _lib, backend as Bk
 from ._cwt import (cwt, CwtPlan, _clean_input, _pad_geometry_for,
                    cached_process_scales, wavelet_key, _CACHE_LOCK)
-from .algos import phase_cwt_gpu, make_reassign_desc, colsum_real, invert_components
+from .algos import (phase_cwt_gpu, make_reassign_desc, colsum_real, invert_components,
+                    reassign_backward)
 from .ssqueezing import (ssqueeze, _check_ssqueezing_args,
                          _compute_associated_frequencies, ssq_const)
 from .utils.common import EPS32, EPS64
@@ -86,9 +87,13 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
                                   gamma, dtype)
         key = (np.asarray(ssq_freqs).tobytes(), np.asarray(const).tobytes(),
                logscale, bool(flipud), float(gamma))
-        with plan._lock:                     # grid + launch belong together
-            plan.set_reassign(desc, key)
-            Tx, Wx, dWx = plan.ssq_cwt(x, get_dWx=get_dWx)
+        if torch.is_tensor(x) and x.requires_grad:
+            Tx, Wx, dWx = _SsqCwtFn.apply(plan._x2d(x), plan, desc, key)
+            dWx = dWx if get_dWx else None
+        else:
+            with plan._lock:                 # grid + launch belong together
+                plan.set_reassign(desc, key)
+                Tx, Wx, dWx = plan.ssq_cwt(x, get_dWx=get_dWx)
         if x.ndim == 1:
             Tx, Wx = Tx[0], Wx[0]
             dWx = dWx[0] if get_dWx else None
@@ -111,6 +116,44 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
     elif get_dWx:
         return Tx, Wx, ssq_freqs, sc, dWx
     return Tx, Wx, ssq_freqs, sc
+
+
+class _SsqCwtFn(torch.autograd.Function):
+    """The fused `ssq_cwt` as a differentiable torch op with outputs (Tx, Wx, dWx).  The forward
+    is the plan's fused execution with `dWx` stored; the backward holds every bin where the
+    forward put it, recomputing the bins from the saved (Wx, dWx) with the forward's exact
+    arithmetic (`ssqb_ssqueeze_backward`), then runs the cwt adjoint (`ssqb_cwt_backward`).
+    Gradients that do not arrive are None, as in `_CwtFn`."""
+
+    @staticmethod
+    def forward(ctx, x2d, plan, desc, key):
+        ctx.set_materialize_grads(False)
+        ctx.plan, ctx.desc = plan, desc
+        with plan._lock:
+            plan.set_reassign(desc, key)
+            Tx, Wx, dWx = plan.ssq_cwt(x2d.detach(), get_dWx=True)
+        ctx.save_for_backward(Wx, dWx)
+        return Tx, Wx, dWx
+
+    @staticmethod
+    def backward(ctx, gT, gW, gdW):
+        if gT is None and gW is None and gdW is None:
+            return None, None, None, None
+        plan = ctx.plan
+        Wx, dWx = ctx.saved_tensors
+        if gT is not None:
+            gW = reassign_backward(ctx.desc, gT, plan.dtype, Wx=Wx, dWx=dWx, gWx=gW)
+        cdt = Bk.cplx_dtype(plan.dtype)
+        gW = None if gW is None else gW.to(cdt).contiguous()
+        gdW = None if gdW is None else gdW.to(cdt).contiguous()
+        if gW is None and gdW is None:
+            return None, None, None, None
+        B = Wx.shape[0]
+        gx = torch.empty((B, plan.N), dtype=Bk.real_dtype(plan.dtype), device='cuda')
+        with plan._lock:
+            _lib.check(plan.lib.ssqb_cwt_backward(plan.handle, Bk.ptr(gW), Bk.ptr(gdW), B, None,
+                                                  0, gx.data_ptr(), Bk.stream_ptr()))
+        return gx, None, None, None
 
 
 _HP_CACHE = {}
@@ -208,6 +251,8 @@ def issq_cwt(Tx, wavelet='gmw', cc=None, cw=None):
     """Inverse synchrosqueezed CWT: signal (or the components along the curves `cc`
     of half-width `cw`, plus the remainder) from `Tx`; same arguments and scaling as
     the reference (`_ssq_cwt.py:313-377`): sum over frequency rows times 2 / Css.
-    Runs on the device; returns a CUDA tensor for tensor input, numpy for numpy."""
+    Runs on the device; returns a CUDA tensor for tensor input, numpy for numpy.  The full
+    inverse is differentiable in `Tx` (torch.autograd); the component form (`cc`, `cw`) is
+    not."""
     wavelet = Wavelet._init_if_not_isinstance(wavelet)
     return _invert_plane(Tx, cc, cw, 2 / adm_ssq(wavelet))

@@ -9,12 +9,51 @@ import torch
 
 from . import _lib, backend as Bk
 from ._stft import stft, _StftCall, _get_call, get_window, _check_NOLA
-from .algos import phase_stft_gpu, make_reassign_desc
+from .algos import phase_stft_gpu, make_reassign_desc, reassign_backward
 from .ssqueezing import ssqueeze, _check_ssqueezing_args
 from .utils.common import EPS32, EPS64, WARN
 from .utils.cwt_utils import infer_scaletype, _process_fs_and_t
 
 __all__ = ['ssq_stft', 'issq_stft', 'phase_stft']
+
+
+class _SsqStftFn(torch.autograd.Function):
+    """The fused `ssq_stft` as a differentiable torch op with outputs (Tx, Sx, dSx): the
+    forward is `ssqb_ssq_stft_exec` with `dSx` stored, the backward holds every bin where the
+    forward put it (`ssqb_ssqueeze_backward` on the saved Sx, dSx and the call's `Sfs`), then
+    runs the stft adjoint (`ssqb_stft_backward`)."""
+
+    @staticmethod
+    def forward(ctx, x2, call, desc):
+        ctx.set_materialize_grads(False)
+        ctx.call, ctx.desc = call, desc
+        B = x2.shape[0]
+        Sx, Tx, dSx = call.outputs(B, 3)
+        _lib.check(Bk.require_cuda().ssqb_ssq_stft_exec(
+            C.byref(call.desc), C.byref(desc), x2.detach().data_ptr(), B, Sx.data_ptr(),
+            Tx.data_ptr(), dSx.data_ptr(), Bk.stream_ptr()))
+        ctx.save_for_backward(Sx, dSx)
+        return Tx, Sx, dSx
+
+    @staticmethod
+    def backward(ctx, gT, gS, gdS):
+        if gT is None and gS is None and gdS is None:
+            return None, None, None
+        call = ctx.call
+        Sx, dSx = ctx.saved_tensors
+        if gT is not None:
+            gS = reassign_backward(ctx.desc, gT, call.dtype, Wx=Sx, dWx=dSx, gWx=gS,
+                                   Sfs=call.Sfs_tensor())
+        cdt = Bk.cplx_dtype(call.dtype)
+        gS = None if gS is None else gS.to(cdt).contiguous()
+        gdS = None if gdS is None else gdS.to(cdt).contiguous()
+        if gS is None and gdS is None:
+            return None, None, None
+        B = Sx.shape[0]
+        gx = torch.empty((B, call.N), dtype=Bk.real_dtype(call.dtype), device='cuda')
+        _lib.check(Bk.require_cuda().ssqb_stft_backward(
+            C.byref(call.desc), Bk.ptr(gS), Bk.ptr(gdS), B, gx.data_ptr(), Bk.stream_ptr()))
+        return gx, None, None
 
 
 def ssq_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=None,
@@ -42,13 +81,17 @@ def ssq_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=Non
         xd = Bk.to_device(x, call.dtype)
         x2 = xd if xd.ndim == 2 else xd.unsqueeze(0)
         B = x2.shape[0]
-        outs = call.outputs(B, 3 if get_dWx else 2)
-        Sx, Tx = outs[0], outs[1]
-        dSx = outs[2] if get_dWx else None
-        _lib.check(lib.ssqb_ssq_stft_exec(C.byref(call.desc), C.byref(desc),
-                                          x2.data_ptr(), B, Sx.data_ptr(),
-                                          Tx.data_ptr(), Bk.ptr(dSx),
-                                          Bk.stream_ptr()))
+        if torch.is_tensor(x) and x.requires_grad:
+            Tx, Sx, dSx = _SsqStftFn.apply(x2, call, desc)
+            dSx = dSx if get_dWx else None
+        else:
+            outs = call.outputs(B, 3 if get_dWx else 2)
+            Sx, Tx = outs[0], outs[1]
+            dSx = outs[2] if get_dWx else None
+            _lib.check(lib.ssqb_ssq_stft_exec(C.byref(call.desc), C.byref(desc),
+                                              x2.data_ptr(), B, Sx.data_ptr(),
+                                              Tx.data_ptr(), Bk.ptr(dSx),
+                                              Bk.stream_ptr()))
         if x.ndim == 1:
             Sx, Tx = Sx[0], Tx[0]
             dSx = dSx[0] if get_dWx else None
@@ -97,7 +140,9 @@ def issq_stft(Tx, window=None, cc=None, cw=None, n_fft=None, win_len=None,
               hop_len=1, modulated=True):
     """Inverse synchrosqueezed STFT (reference `_ssq_stft.py:139-198`): sum of `Tx.real`
     over frequency rows (or over the component bands `cc +- cw`) times
-    2 / window[n_fft // 2].  Only `hop_len=1`, `modulated=True`, as in the reference."""
+    2 / window[n_fft // 2].  Only `hop_len=1`, `modulated=True`, as in the reference.
+    The full inverse is differentiable in `Tx` (torch.autograd); the component form (`cc`,
+    `cw`) is not."""
     from ._ssq_cwt import _invert_plane
     if not modulated:
         raise ValueError("inversion with `modulated == False` "

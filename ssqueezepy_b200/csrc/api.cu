@@ -106,6 +106,22 @@ int ssqb_indexed_sum(int dtype, const void* Wx, const void* w, void* Tx, int64_t
   return run_indexed_sum(dtype, Wx, w, Tx, B, na, N, r, (cudaStream_t)stream);
 }
 
+int ssqb_ssqueeze_backward(int dtype, const void* Wx, const void* dWx, const void* gTx,
+                           const void* gWx, void* gWout, int64_t B, int na, int64_t N,
+                           const ssqb_reassign_desc* r, const void* Sfs, void* stream) {
+  if (!Wx || !dWx) return set_error(SSQB_E_ARG, "null pointer");
+  return run_reassign_backward(dtype, Wx, dWx, nullptr, gTx, gWx, gWout, B, na, N, r, Sfs,
+                               (cudaStream_t)stream);
+}
+
+int ssqb_indexed_sum_backward(int dtype, const void* w, const void* gTx, const void* gWx,
+                              void* gWout, int64_t B, int na, int64_t N,
+                              const ssqb_reassign_desc* r, void* stream) {
+  if (!w) return set_error(SSQB_E_ARG, "null pointer");
+  return run_reassign_backward(dtype, nullptr, nullptr, w, gTx, gWx, gWout, B, na, N, r,
+                               nullptr, (cudaStream_t)stream);
+}
+
 int ssqb_phase_cwt(int dtype, const void* Wx, const void* dWx, void* w, int64_t total,
                    double gamma, void* stream) {
   return run_phase(dtype, false, Wx, dWx, nullptr, w, total, 1, 1, gamma, (cudaStream_t)stream);
@@ -173,6 +189,13 @@ int ssqb_colsum_real(int dtype, int wide, const void* M, int64_t B, int na, int6
                      void* stream) {
   return run_colsum_real(dtype, wide, M, B, na, N, div_host, scale, has_scale, out,
                          (cudaStream_t)stream);
+}
+
+int ssqb_colsum_real_backward(int dtype, int wide, const void* gout, int64_t B, int na,
+                              int64_t N, const double* div_host, double scale, int has_scale,
+                              void* gM, void* stream) {
+  return run_colsum_real_backward(dtype, wide, gout, B, na, N, div_host, scale, has_scale, gM,
+                                  (cudaStream_t)stream);
 }
 
 int ssqb_invert_components(int dtype, const void* M, int na, int64_t N, const int32_t* cc,

@@ -90,6 +90,11 @@ int run_ssqueeze(int dtype, const void* Wx, const void* dWx, void* Tx, long long
                  long long N, const ssqb_reassign_desc* r, const void* Sfs, cudaStream_t st);
 int run_indexed_sum(int dtype, const void* Wx, const void* w, void* Tx, long long B, int na,
                     long long N, const ssqb_reassign_desc* r, cudaStream_t st);
+// backward of both: bins from (Wx, dWx) when w is null, else from the stored w
+int run_reassign_backward(int dtype, const void* Wx, const void* dWx, const void* w,
+                          const void* gTx, const void* gWx, void* gWout, long long B, int na,
+                          long long N, const ssqb_reassign_desc* r, const void* Sfs,
+                          cudaStream_t st);
 int run_phase(int dtype, bool stft, const void* Wx, const void* dWx, const void* Sfs, void* out,
               long long total, long long ncols, int nrows, double gamma, cudaStream_t st);
 int run_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const void* x, long long B,
@@ -102,6 +107,9 @@ int run_istft_backward(const ssqb_istft_desc* d, const void* gx, long long B, vo
 int run_colsum_real(int dtype, int wide, const void* M, long long B, int na, long long N,
                     const double* div_host, double scale, int has_scale, void* out,
                     cudaStream_t st);
+int run_colsum_real_backward(int dtype, int wide, const void* gout, long long B, int na,
+                             long long N, const double* div_host, double scale, int has_scale,
+                             void* gM, cudaStream_t st);
 int run_invert_components(int dtype, const void* M, int na, long long N, const int* cc,
                           const int* cw, int K, double scale, double* out, cudaStream_t st);
 int run_istft(const ssqb_istft_desc* d, const void* Sx, long long B, void* x, cudaStream_t st);

@@ -39,6 +39,22 @@ colsum_real_kernel(const cx<T>* __restrict__ M, TA* __restrict__ out, int na, lo
   out[(long long)b * N + j] = acc;
 }
 
+// Backward of colsum_real_kernel: gM[b][a][j] = (T)((double)gout[b][j] * f[a]) + 0i, with
+// f[a] = scale / div[a] in float64 (host).  gout is in the forward's output type TA.  One
+// thread per column writes the column's na rows (a warp stores 32 consecutive values of a row).
+template <typename T, typename TA>
+__global__ void __launch_bounds__(256)
+colsum_bwd_kernel(const TA* __restrict__ gout, const double* __restrict__ f,
+                  cx<T>* __restrict__ gM, int na, long long N) {
+  const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= N) return;
+  const int b = blockIdx.y;
+  const double g = (double)gout[(long long)b * N + j];
+  cx<T>* __restrict__ p = gM + (long long)b * na * N + j;
+#pragma unroll 4
+  for (int a = 0; a < na; ++a) __stcs(&p[(long long)a * N], mkc<T>((T)(g * f[a]), (T)0));
+}
+
 // Component inversion (`_invert_components`, _ssq_cwt.py:380-403): for component n the
 // rows [cc-cw, cc+cw] of each column (clipped to [0, na], cc == -1 -> none); the last
 // output row is what no component covered.  float64 accumulation and output as in the

@@ -35,6 +35,36 @@ int run_colsum_real(int dtype, int wide, const void* M, long long B, int na, lon
   return colsum_t<double, double>(M, B, na, N, div_host, scale, has_scale, out, st);
 }
 
+template <typename T, typename TA>
+static int colsum_bwd_t(const void* gout, long long B, int na, long long N, const double* div_host,
+                        double scale, int has_scale, void* gM, cudaStream_t st) {
+  std::vector<double> h((size_t)na);
+  for (int a = 0; a < na; ++a) {
+    const double s = has_scale ? scale : 1.0;
+    h[a] = div_host ? s / div_host[a] : s;
+  }
+  double* f = nullptr;
+  SSQB_CUDA(cudaMallocAsync((void**)&f, sizeof(double) * na, st));
+  SSQB_CUDA(cudaMemcpyAsync(f, h.data(), sizeof(double) * na, cudaMemcpyHostToDevice, st));
+  SSQB_CUDA(cudaStreamSynchronize(st));                  // `h` is a local
+  dim3 grid((unsigned)((N + 255) / 256), (unsigned)B);
+  colsum_bwd_kernel<T, TA><<<grid, 256, 0, st>>>((const TA*)gout, f, (cx<T>*)gM, na, N);
+  SSQB_LAUNCH_CHECK();
+  SSQB_CUDA(cudaFreeAsync(f, st));
+  return 0;
+}
+
+int run_colsum_real_backward(int dtype, int wide, const void* gout, long long B, int na,
+                             long long N, const double* div_host, double scale, int has_scale,
+                             void* gM, cudaStream_t st) {
+  if (!gout || !gM) return set_error(SSQB_E_ARG, "null pointer");
+  if (B < 1 || na < 1 || N < 1) return set_error(SSQB_E_ARG, "bad shape");
+  if (dtype == SSQB_F32)
+    return wide ? colsum_bwd_t<float, double>(gout, B, na, N, div_host, scale, has_scale, gM, st)
+                : colsum_bwd_t<float, float>(gout, B, na, N, div_host, scale, has_scale, gM, st);
+  return colsum_bwd_t<double, double>(gout, B, na, N, div_host, scale, has_scale, gM, st);
+}
+
 int run_invert_components(int dtype, const void* M, int na, long long N, const int* cc,
                           const int* cw, int K, double scale, double* out, cudaStream_t st) {
   if (!M || !out || !cc || !cw) return set_error(SSQB_E_ARG, "null pointer");

@@ -8,6 +8,8 @@
 //   indexed_sum_colowner_kernel<- algos.py:172-250 `_indexed_sum_*_par`
 //   phase_cwt_kernel           <- algos.py:706-740 `_phase_cwt_par`
 //   phase_stft_kernel          <- algos.py:784-816 `_phase_stft_par`
+//   ssqueeze_bwd_kernel,
+//   indexed_sum_bwd_kernel     backward of the two reassignments for torch.autograd (bins held)
 //
 // Layout: Wx, dWx, Tx are [B][na][N] complex (row-major); thread j of a warp reads
 // 32 consecutive complex values of a row (256/512 B, coalesced).
@@ -101,6 +103,29 @@ __device__ __forceinline__ float log2f_glibc(float x) {
 __device__ __forceinline__ double log2_typed(float w)  { return (double)log2f_glibc(w); }
 __device__ __forceinline__ double log2_typed(double w) { return log2(w); }
 
+// bin of a stored real `w` (algos.py:172-250 `_indexed_sum_*_par`; grid kinds 0-2, the host
+// maps the STFT grid to 2), after the optional flip; -1 for an inf `w`, which is skipped
+// (algos.py:188)
+template <typename T>
+__device__ __forceinline__ int bin_from_stored_w(T wv, const ReassignGrid& g) {
+  if (isinf(wv)) return -1;
+  double kk;
+  if (g.kind == 0) {
+    double v = (log2_typed(wv) - g.a0) / g.d0;
+    kk = fmin(rint(fmax(v, 0.0)), (double)g.omax);
+  } else if (g.kind == 1) {
+    double wl = log2_typed(wv);
+    if (wl > g.a1) kk = fmin(rint((wl - g.a1) / g.d1) + (double)g.idx1, (double)g.omax);
+    else           kk = rint(fmax((wl - g.a0) / g.d0, 0.0));
+  } else {
+    double v = ((double)wv - g.a0) / g.d0;
+    kk = fmin(rint(fmax(v, 0.0)), (double)g.omax);
+  }
+  if (!(kk == kk)) kk = 0.0;
+  int k = (int)kk;
+  return g.flipud ? (g.omax - k) : k;
+}
+
 template <typename T>
 __global__ void __launch_bounds__(256)
 indexed_sum_colowner_kernel(const cx<T>* __restrict__ Wx, const T* __restrict__ w,
@@ -111,26 +136,74 @@ indexed_sum_colowner_kernel(const cx<T>* __restrict__ Wx, const T* __restrict__ 
   long long base = (long long)blockIdx.y * na * N;
   Wx += base; w += base; Tx += base;
   for (int i = 0; i < na; ++i) {
-    T wv = w[(long long)i * N + j];
-    if (isinf(wv)) continue;                              // algos.py:188
-    double kk;
-    if (g.kind == 0) {
-      double v = (log2_typed(wv) - g.a0) / g.d0;
-      kk = fmin(rint(fmax(v, 0.0)), (double)g.omax);
-    } else if (g.kind == 1) {
-      double wl = log2_typed(wv);
-      if (wl > g.a1) kk = fmin(rint((wl - g.a1) / g.d1) + (double)g.idx1, (double)g.omax);
-      else           kk = rint(fmax((wl - g.a0) / g.d0, 0.0));
-    } else {
-      double v = ((double)wv - g.a0) / g.d0;
-      kk = fmin(rint(fmax(v, 0.0)), (double)g.omax);
-    }
-    if (!(kk == kk)) kk = 0.0;
-    int k = (int)kk;
-    if (g.flipud) k = g.omax - k;
+    int k = bin_from_stored_w<T>(w[(long long)i * N + j], g);
+    if (k < 0) continue;
     accumulate_exact<T>(&Tx[(long long)k * N + j], Wx[(long long)i * N + j], cst[i],
                         g.const_wide);
   }
+}
+
+// ---- backward of the reassignment ----------------------------------------------------
+// Tx is linear in Wx once the bins and the gamma test are held where the forward put them,
+// so the gradient is the transpose of the scatter, a gather:
+//   gWout[b][i][j] = gWx[b][i][j] + c_i * gTx[b][k(i,j)][j]   (active points; else gWx)
+// One thread per point, no atomics (deterministic).  gWx may be null (= 0) and may alias
+// gWout: each thread reads its own element before it writes it.
+
+// gW + gT * c with accumulate_exact's typing
+template <typename T>
+__device__ __forceinline__ cx<T> gather_exact(cx<T> gW, cx<T> gT, double cc, int wide) {
+  if (sizeof(T) == 8 || wide) {
+    double re = add_rn((double)gW.x, mul_rn((double)gT.x, cc));
+    double im = add_rn((double)gW.y, mul_rn((double)gT.y, cc));
+    return mkc<T>((T)re, (T)im);
+  }
+  float c32 = (float)cc;
+  float re = add_rn((float)gW.x, mul_rn((float)gT.x, c32));
+  float im = add_rn((float)gW.y, mul_rn((float)gT.y, c32));
+  return mkc<T>((T)re, (T)im);
+}
+
+// grid (ceil(N / 256), na, B); bins as ssqueeze_colowner_kernel computes them
+template <typename T>
+__global__ void __launch_bounds__(256)
+ssqueeze_bwd_kernel(const cx<T>* __restrict__ Wx, const cx<T>* __restrict__ dWx,
+                    const cx<T>* __restrict__ gTx, const cx<T>* gWx, cx<T>* gWout,
+                    const double* __restrict__ cst, const T* __restrict__ Sfs, int na,
+                    long long N, const ReassignGrid g) {
+  const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= N) return;
+  const int i = blockIdx.y;
+  const long long base = (long long)blockIdx.z * na * N;
+  const long long idx = base + (long long)i * N + j;
+  cx<T> out = gWx ? gWx[idx] : mkc<T>((T)0, (T)0);
+  const cx<T> W = Wx[idx];
+  if (is_active_exact(W.x, W.y, g.gamma)) {
+    const cx<T> dW = dWx[idx];
+    const double r = phase_ratio_exact<T>(dW.x, dW.y, W.x, W.y);
+    const double w = (g.kind == 3) ? fabs((double)Sfs[i] - r) : fabs(r);
+    const int k = bin_from_w_exact(w, g);
+    out = gather_exact<T>(out, gTx[base + (long long)k * N + j], cst[i], g.const_wide);
+  }
+  gWout[idx] = out;
+}
+
+// grid (ceil(N / 256), na, B); bins as indexed_sum_colowner_kernel computes them
+template <typename T>
+__global__ void __launch_bounds__(256)
+indexed_sum_bwd_kernel(const T* __restrict__ w, const cx<T>* __restrict__ gTx,
+                       const cx<T>* gWx, cx<T>* gWout, const double* __restrict__ cst,
+                       int na, long long N, const ReassignGrid g) {
+  const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= N) return;
+  const int i = blockIdx.y;
+  const long long base = (long long)blockIdx.z * na * N;
+  const long long idx = base + (long long)i * N + j;
+  cx<T> out = gWx ? gWx[idx] : mkc<T>((T)0, (T)0);
+  const int k = bin_from_stored_w<T>(w[idx], g);
+  if (k >= 0)
+    out = gather_exact<T>(out, gTx[base + (long long)k * N + j], cst[i], g.const_wide);
+  gWout[idx] = out;
 }
 
 template <typename T> __device__ __forceinline__ T t_inf();

@@ -87,6 +87,49 @@ int run_indexed_sum(int dtype, const void* Wx, const void* w, void* Tx, long lon
                            : indexed_sum_t<double>(Wx, w, Tx, B, na, N, r, st);
 }
 
+// backward of both reassignments: `w` null -> bins from (Wx, dWx) as ssqueeze, else from the
+// stored w as indexed_sum
+template <typename T>
+static int reassign_bwd_t(const void* Wx, const void* dWx, const void* w, const void* gTx,
+                          const void* gWx, void* gWout, long long B, int na, long long N,
+                          const ssqb_reassign_desc* r, const void* Sfs, cudaStream_t st) {
+  ReassignGrid g;
+  int rc = fill_grid(r, na, &g); if (rc) return rc;
+  if (w) {
+    if (g.kind == 3) g.kind = 2;
+  } else if (g.kind == 3 && !Sfs) {
+    return set_error(SSQB_E_ARG, "SSQB_GRID_STFT needs Sfs_dev");
+  }
+  if (B > 65535) return set_error(SSQB_E_UNSUPP, "batch of %lld > 65535", B);
+  double* cst = nullptr;
+  SSQB_CUDA(cudaMallocAsync((void**)&cst, sizeof(double) * na, st));
+  SSQB_CUDA(cudaMemcpyAsync(cst, r->cst_host, sizeof(double) * na, cudaMemcpyHostToDevice, st));
+  dim3 grid((unsigned)((N + 255) / 256), (unsigned)na, (unsigned)B);
+  if (w)
+    indexed_sum_bwd_kernel<T><<<grid, 256, 0, st>>>((const T*)w, (const cx<T>*)gTx,
+                                                    (const cx<T>*)gWx, (cx<T>*)gWout, cst, na,
+                                                    N, g);
+  else
+    ssqueeze_bwd_kernel<T><<<grid, 256, 0, st>>>((const cx<T>*)Wx, (const cx<T>*)dWx,
+                                                 (const cx<T>*)gTx, (const cx<T>*)gWx,
+                                                 (cx<T>*)gWout, cst, (const T*)Sfs, na, N, g);
+  SSQB_LAUNCH_CHECK();
+  SSQB_CUDA(cudaFreeAsync(cst, st));
+  return 0;
+}
+
+int run_reassign_backward(int dtype, const void* Wx, const void* dWx, const void* w,
+                          const void* gTx, const void* gWx, void* gWout, long long B, int na,
+                          long long N, const ssqb_reassign_desc* r, const void* Sfs,
+                          cudaStream_t st) {
+  if ((!w && (!Wx || !dWx)) || !gTx || !gWout || !r || !r->cst_host)
+    return set_error(SSQB_E_ARG, "null pointer");
+  if (B < 1 || na < 1 || N < 1 || na > 65535) return set_error(SSQB_E_ARG, "bad shape");
+  return dtype == SSQB_F32
+      ? reassign_bwd_t<float>(Wx, dWx, w, gTx, gWx, gWout, B, na, N, r, Sfs, st)
+      : reassign_bwd_t<double>(Wx, dWx, w, gTx, gWx, gWout, B, na, N, r, Sfs, st);
+}
+
 template <typename T>
 static int phase_t(bool stft, const void* Wx, const void* dWx, const void* Sfs, void* out,
                    long long total, long long ncols, int nrows, double gamma, cudaStream_t st) {
