@@ -116,12 +116,16 @@ int ssqb_cwt_exec(ssqb_cwt_plan* plan, const void* x_dev, int64_t B,
 
 /* ssq_cwt: _ssq_cwt.py:250-289 = cwt(derivative=True) + ssqueeze_fast
  * (algos.py:126-150) fused; Tx_dev [B][na][N] is zeroed here and accumulated
- * with red.global.add; dWx_dev may be NULL (never materialised then).          */
+ * with red.global.add; dWx_dev may be NULL (never materialised then).  Wx_dev may
+ * be NULL too: the fused kernels then never store Wx (Tx only, half the output
+ * traffic); a plan of non-power-of-two length keeps Wx in an internal buffer.
+ * ssqb_cwt_exec and ssqb_cwt_exec_host still require Wx.                        */
 int ssqb_ssq_cwt_exec(ssqb_cwt_plan* plan, const void* x_dev, int64_t B,
                       void* Wx_dev, void* Tx_dev, void* dWx_dev, void* stream);
 
 /* same two calls with HOST buffers (pageable or pinned); H2D / D2H copies are
- * issued on `stream` and the call returns after the stream is synchronised.     */
+ * issued on `stream` and the call returns after the stream is synchronised.
+ * ssqb_ssq_cwt_exec_host: Wx_host may be NULL (no Wx staging, no Wx copy).       */
 int ssqb_cwt_exec_host(ssqb_cwt_plan* plan, const void* x_host, int64_t B,
                        void* Wx_host, void* dWx_host, const double* out_mul_host,
                        int rpadded, void* stream);
@@ -203,7 +207,8 @@ typedef struct {
  *   x_dev [B][N]; Sx_dev, dSx_dev [B][n_fft/2+1][n_hops]; dSx_dev may be NULL  */
 int ssqb_stft_exec(const ssqb_stft_desc* d, const void* x_dev, int64_t B,
                    void* Sx_dev, void* dSx_dev, void* stream);
-/* ssq_stft: _ssq_stft.py:88-122 = stft + `_ssq_stft_par` fused (Tx zeroed here) */
+/* ssq_stft: _ssq_stft.py:88-122 = stft + `_ssq_stft_par` fused (Tx zeroed here).
+ * Sx_dev / Sx_host may be NULL (Tx only: Sx is never stored); dSx may be NULL.  */
 int ssqb_ssq_stft_exec(const ssqb_stft_desc* d, const ssqb_reassign_desc* r,
                        const void* x_dev, int64_t B, void* Sx_dev, void* Tx_dev,
                        void* dSx_dev, void* stream);

@@ -190,16 +190,18 @@ class CwtPlan:
                                               int(bool(rpadded)), Bk.stream_ptr()))
         return Wx, dWx
 
-    def ssq_cwt(self, x, get_dWx=False):
+    def ssq_cwt(self, x, get_dWx=False, get_Wx=True):
+        """(Tx, Wx, dWx); Wx is None (never stored) with get_Wx=False, dWx without get_dWx."""
         xd = self._x2d(x)
         B = xd.shape[0]
         cdt = Bk.cplx_dtype(self.dtype)
-        Wx = torch.empty((B, self.na, self.N), dtype=cdt, device='cuda')
-        Tx = torch.empty_like(Wx)
-        dWx = torch.empty_like(Wx) if get_dWx else None
+        shape = (B, self.na, self.N)
+        Wx = torch.empty(shape, dtype=cdt, device='cuda') if get_Wx else None
+        Tx = torch.empty(shape, dtype=cdt, device='cuda')
+        dWx = torch.empty_like(Tx) if get_dWx else None
         with self._lock:
             _lib.check(self.lib.ssqb_ssq_cwt_exec(self.handle, xd.data_ptr(), B,
-                                                  Wx.data_ptr(), Tx.data_ptr(),
+                                                  Bk.ptr(Wx), Tx.data_ptr(),
                                                   Bk.ptr(dWx), Bk.stream_ptr()))
         return Tx, Wx, dWx
 

@@ -30,11 +30,21 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
             difftype='trig', difforder=None, gamma=None, vectorized=True,
             preserve_transform=None, astensor=True, order=0, nan_checks=None,
             patience=0, flipud=True, cache_wavelet=None, get_w=False,
-            get_dWx=False):
+            get_dWx=False, get_Wx=True):
     """Returns `(Tx, Wx, ssq_freqs, scales[, w][, dWx])` like the reference.
     `Tx`, `Wx` (and `w`, `dWx`) are CUDA tensors when `astensor=True`, numpy
     arrays otherwise; `ssq_freqs` is a float64 numpy array; `Wx` is never
-    modified (`preserve_transform` has nothing to preserve)."""
+    modified (`preserve_transform` has nothing to preserve).
+
+    `get_Wx=False` returns `Wx` as None, in the same position.  On the fused
+    route (`squeezing='sum'`, no `get_w`, `order=0`) the `Wx` plane is then
+    never allocated or written: a call needs one [B, na, N] plane less of
+    device memory and HBM traffic.  The two-step routes (`get_w`,
+    `squeezing='abs'` or a function, higher `order`) need `Wx` as the input of
+    `ssqueeze`; they compute it as usual and drop it before returning, so they
+    save no peak memory, nor does `padtype=None` on a length that is not a power
+    of two (its plan keeps `Wx` in a buffer of its own).  With `x.requires_grad`, `Wx` and `dWx` are still kept
+    for the backward."""
     if not hasattr(x, 'ndim'):
         raise TypeError("`x` must be a numpy array or torch Tensor "
                         "(got %s)" % type(x))
@@ -75,6 +85,8 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
                                  dWx=None if get_w else dWx, transform='cwt')
         if not get_dWx:
             dWx = None
+        if not get_Wx:
+            Wx = None
     else:
         x = _clean_input(x, nan_checks)
         n_up, n1, pad_kind = _pad_geometry_for(N, padtype)
@@ -90,12 +102,14 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
         if torch.is_tensor(x) and x.requires_grad:
             Tx, Wx, dWx = _SsqCwtFn.apply(plan._x2d(x), plan, desc, key)
             dWx = dWx if get_dWx else None
+            Wx = Wx if get_Wx else None       # the backward keeps its own reference
         else:
             with plan._lock:                 # grid + launch belong together
                 plan.set_reassign(desc, key)
-                Tx, Wx, dWx = plan.ssq_cwt(x, get_dWx=get_dWx)
+                Tx, Wx, dWx = plan.ssq_cwt(x, get_dWx=get_dWx, get_Wx=get_Wx)
         if x.ndim == 1:
-            Tx, Wx = Tx[0], Wx[0]
+            Tx = Tx[0]
+            Wx = Wx[0] if get_Wx else None
             dWx = dWx[0] if get_dWx else None
         w = None
         sc = plan.scales_tensor().clone()        # fresh arrays: callers may modify them in place

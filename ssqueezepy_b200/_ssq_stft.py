@@ -59,8 +59,14 @@ class _SsqStftFn(torch.autograd.Function):
 def ssq_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=None,
              modulated=True, ssq_freqs=None, padtype='reflect', squeezing='sum',
              gamma=None, preserve_transform=None, dtype=None, astensor=True,
-             flipud=False, get_w=False, get_dWx=False):
-    """Returns `(Tx, Sx, ssq_freqs, Sfs[, w][, dSx])` like the reference."""
+             flipud=False, get_w=False, get_dWx=False, get_Sx=True):
+    """Returns `(Tx, Sx, ssq_freqs, Sfs[, w][, dSx])` like the reference.
+
+    `get_Sx=False` returns `Sx` as None, in the same position.  On the fused
+    route (`squeezing='sum'`, no `get_w`, no `ssq_freqs`) `Sx` is then never
+    allocated or written.  The two-step routes compute `Sx` as the input of
+    `ssqueeze` and drop it before returning, so they save no peak memory.  With
+    `x.requires_grad`, `Sx` and `dSx` are still kept for the backward."""
     if x.ndim == 2 and get_w:
         raise NotImplementedError("`get_w=True` unsupported with batched input.")
     N = x.shape[-1]
@@ -84,16 +90,19 @@ def ssq_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=Non
         if torch.is_tensor(x) and x.requires_grad:
             Tx, Sx, dSx = _SsqStftFn.apply(x2, call, desc)
             dSx = dSx if get_dWx else None
+            Sx = Sx if get_Sx else None       # the backward keeps its own reference
         else:
-            outs = call.outputs(B, 3 if get_dWx else 2)
-            Sx, Tx = outs[0], outs[1]
-            dSx = outs[2] if get_dWx else None
+            outs = call.outputs(B, int(get_Sx) + 1 + int(get_dWx))
+            Sx = outs.pop(0) if get_Sx else None
+            Tx = outs.pop(0)
+            dSx = outs.pop(0) if get_dWx else None
             _lib.check(lib.ssqb_ssq_stft_exec(C.byref(call.desc), C.byref(desc),
-                                              x2.data_ptr(), B, Sx.data_ptr(),
+                                              x2.data_ptr(), B, Bk.ptr(Sx),
                                               Tx.data_ptr(), Bk.ptr(dSx),
                                               Bk.stream_ptr()))
         if x.ndim == 1:
-            Sx, Tx = Sx[0], Tx[0]
+            Tx = Tx[0]
+            Sx = Sx[0] if get_Sx else None
             dSx = dSx[0] if get_dWx else None
         w = None
         ssq_freqs = Sfs[::-1].copy() if flipud else Sfs.copy()
@@ -116,6 +125,8 @@ def ssq_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=Non
                                  transform='stft')
         if not get_dWx:
             dSx = None
+        if not get_Sx:
+            Sx = None
         Sfs_out = torch.as_tensor(Sfs, device='cuda') if astensor else Sfs
 
     if not astensor:

@@ -71,7 +71,7 @@ int ssqb_cwt_exec_host(ssqb_cwt_plan* p, const void* x, int64_t B, void* Wx, voi
 
 int ssqb_ssq_cwt_exec_host(ssqb_cwt_plan* p, const void* x, int64_t B, void* Wx, void* Tx,
                            void* dWx, void* stream) {
-  if (!p || !x || !Wx || !Tx) return set_error(SSQB_E_ARG, "null argument");
+  if (!p || !x || !Tx) return set_error(SSQB_E_ARG, "null argument");   // Wx may be NULL
   return p->impl->exec_host(x, B, Wx, dWx, Tx, true, nullptr, false, (cudaStream_t)stream);
 }
 
@@ -145,7 +145,7 @@ int ssqb_ssq_stft_exec(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, con
 
 int ssqb_ssq_stft_exec_host(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const void* x,
                             int64_t B, void* Sx, void* Tx, void* dSx, void* stream) {
-  if (!d || !x || !Sx || !Tx) return set_error(SSQB_E_ARG, "null argument");
+  if (!d || !x || !Tx) return set_error(SSQB_E_ARG, "null argument");   // Sx may be NULL
   cudaStream_t st = (cudaStream_t)stream;
   size_t es = d->dtype == SSQB_F32 ? 4 : 8;
   long long n_hops = (d->N - 1) / d->hop + 1;
@@ -167,13 +167,14 @@ int ssqb_ssq_stft_exec_host(const ssqb_stft_desc* d, const ssqb_reassign_desc* r
   };
   cudaError_t e;
   if ((e = cudaMallocAsync(&xd, nx, st)) != cudaSuccess) return fail(e, "cudaMallocAsync(x)");
-  if ((e = cudaMallocAsync(&Sd, nout, st)) != cudaSuccess) return fail(e, "cudaMallocAsync(Sx)");
+  if (Sx && (e = cudaMallocAsync(&Sd, nout, st)) != cudaSuccess) return fail(e, "cudaMallocAsync(Sx)");
   if ((e = cudaMallocAsync(&Td, nout, st)) != cudaSuccess) return fail(e, "cudaMallocAsync(Tx)");
   if (dSx && (e = cudaMallocAsync(&dSd, nout, st)) != cudaSuccess) return fail(e, "cudaMallocAsync(dSx)");
   if ((e = cudaMemcpyAsync(xd, x, nx, cudaMemcpyHostToDevice, st)) != cudaSuccess) return fail(e, "H2D copy");
   int rc = run_stft(d, r, xd, B, Sd, Td, dSd, true, st);
   if (rc == 0) {
-    if ((e = cudaMemcpyAsync(Sx, Sd, nout, cudaMemcpyDeviceToHost, st)) != cudaSuccess) return fail(e, "D2H copy");
+    if (Sx && (e = cudaMemcpyAsync(Sx, Sd, nout, cudaMemcpyDeviceToHost, st)) != cudaSuccess)
+      return fail(e, "D2H copy");
     if ((e = cudaMemcpyAsync(Tx, Td, nout, cudaMemcpyDeviceToHost, st)) != cudaSuccess) return fail(e, "D2H copy");
     if (dSx && (e = cudaMemcpyAsync(dSx, dSd, nout, cudaMemcpyDeviceToHost, st)) != cudaSuccess)
       return fail(e, "D2H copy");

@@ -243,9 +243,9 @@ struct RowsTile {
   static constexpr int SARR = ELEMS + (PAD ? F : 0);
 };
 
-template <typename T, int LOGE, int LOG_F, int NARR, int GEN, int QMAX, bool SSQ, int BPT>
-__global__ void __launch_bounds__((1 << LOGE) / (8 * BPT), (BPT == 1 && LOGE <= 12 && sizeof(T) == 4) ? 2 : 1)
-cwt_rows_kernel(const FastArgs<T> P) {
+// STORE_W = false: the fused epilogue without the Wx store (cwt_rows_tx_kernel)
+template <typename T, int LOGE, int LOG_F, int NARR, int GEN, int QMAX, bool SSQ, int BPT, bool STORE_W>
+__device__ __forceinline__ void cwt_rows_body(const FastArgs<T>& P) {
   // Length-F inverse transform over i1 (F = 8, 64 or 512 = one, two or three radix-8
   // stages; narrow-band rows use the shortest F that still holds their band), for
   // R2 = ELEMS/F output phases t2 per CTA:  t = (n/F)*t1 + t2.
@@ -437,7 +437,7 @@ cwt_rows_kernel(const FastArgs<T> P) {
     eoff = P.blk_h2; elim = P.blk_hop;
   }
   const long long row = (long long)sig * A.na + a;
-  cx<T>* __restrict__ Wrow = A.Wx + row * A.Nout;
+  cx<T>* __restrict__ Wrow = STORE_W ? A.Wx + row * A.Nout : nullptr;
   cx<T>* __restrict__ dWrow = A.dWx ? A.dWx + row * A.Nout : nullptr;
   cx<T>* __restrict__ Tb = A.Tx ? A.Tx + (long long)sig * A.na * A.Nout : nullptr;
   const int Nout = (int)A.Nout;
@@ -475,7 +475,7 @@ cwt_rows_kernel(const FastArgs<T> P) {
         const int jj = ((j[bb] + F8 * q) << logI2) + jbase;
         const int jo = jj + eshift;
         if ((unsigned)jj < (unsigned)elim && jo < Nout) {
-          Wrow[jo] = v[0][bb][q];
+          if (STORE_W) Wrow[jo] = v[0][bb][q];
           if (P.write_dWx) dWrow[jo] = v[1][bb][q];
           if (Zrow) Zrow[jo] = mkc<T>((T)0, (T)0);
           ssq_point<T>(v[0][bb][q], v[1][bb][q], Tb + jo, rowbytes, cre, cwide, g2lo, g2hi,
@@ -487,6 +487,19 @@ cwt_rows_kernel(const FastArgs<T> P) {
 }
 
 #undef SSQB_SIDX
+
+template <typename T, int LOGE, int LOG_F, int NARR, int GEN, int QMAX, bool SSQ, int BPT>
+__global__ void __launch_bounds__((1 << LOGE) / (8 * BPT), (BPT == 1 && LOGE <= 12 && sizeof(T) == 4) ? 2 : 1)
+cwt_rows_kernel(const FastArgs<T> P) {
+  cwt_rows_body<T, LOGE, LOG_F, NARR, GEN, QMAX, SSQ, BPT, true>(P);
+}
+
+// ssq call that skips Wx: Tx, dWx (when asked for) and the zero-ahead stores as above
+template <typename T, int LOGE, int LOG_F, int GEN, int QMAX, int BPT>
+__global__ void __launch_bounds__((1 << LOGE) / (8 * BPT), (BPT == 1 && LOGE <= 12 && sizeof(T) == 4) ? 2 : 1)
+cwt_rows_tx_kernel(const FastArgs<T> P) {
+  cwt_rows_body<T, LOGE, LOG_F, 2, GEN, QMAX, true, BPT, false>(P);
+}
 
 // ---- (3) pass 1 of the two-pass route for wide-band rows ---------------------------
 // One CTA = one row x R1 = ELEMS/I2 consecutive i1, BOTH arrays (W, dW):

@@ -307,7 +307,7 @@ struct GenericCwtPlan : public CwtPlanBase {
   Gfft<T> fft;
   DevBuf<T> scales_d, out_mul_d;
   DevBuf<double> cst_d;
-  DevBuf<cx<T>> xp_d, xh_d, ZW, ZD, OW, OD, dW_tmp;
+  DevBuf<cx<T>> xp_d, xh_d, ZW, ZD, OW, OD, W_tmp, dW_tmp;
   ssqb_reassign_desc rd{}; std::vector<double> rd_cst; bool have_grid = false;
   int init(const ssqb_cwt_desc* desc) {
     d = *desc;
@@ -347,12 +347,14 @@ struct GenericCwtPlan : public CwtPlanBase {
   }
   int exec(const void* xv, long long B, void* Wxv, void* dWxv, void* Txv, bool ssq,
            const double* out_mul_host, bool rpadded, cudaStream_t st) override {
-    if (B < 1 || !xv || !Wxv) return set_error(SSQB_E_ARG, "bad arguments");
+    if (B < 1 || !xv || (!Wxv && !ssq)) return set_error(SSQB_E_ARG, "bad arguments");
     if (ssq && (!Txv || !have_grid)) return set_error(SSQB_E_ARG, "ssq needs Tx and a reassignment grid");
     if (ssq && rpadded) return set_error(SSQB_E_ARG, "ssq works on the unpadded part");
     const long long n = d.n_up, Nout = rpadded ? n : d.N, off = rpadded ? 0 : d.n1;
     const long long rows = B * d.na;
     cx<T>* Wx = (cx<T>*)Wxv; cx<T>* dWx = (cx<T>*)dWxv;
+    // the column-owner ssqueeze reads Wx and dWx: planes the caller did not ask for are internal
+    if (ssq && !Wx) { SSQB_CUDA(W_tmp.ensure((size_t)rows * (size_t)Nout)); Wx = W_tmp.p; }
     if (ssq && !dWx) { SSQB_CUDA(dW_tmp.ensure((size_t)rows * (size_t)Nout)); dWx = dW_tmp.p; }
     const T* out_mul = nullptr;
     if (out_mul_host) {
@@ -397,13 +399,15 @@ struct GenericCwtPlan : public CwtPlanBase {
     const long long Nout = rpadded ? d.n_up : d.N;
     const size_t nx = (size_t)B * (size_t)d.N, nout = (size_t)B * d.na * (size_t)Nout;
     DevBuf<T> xs; DevBuf<cx<T>> Ws, dWs, Ts;
-    SSQB_CUDA(xs.ensure(nx)); SSQB_CUDA(Ws.ensure(nout));
+    SSQB_CUDA(xs.ensure(nx));
+    if (Wx) SSQB_CUDA(Ws.ensure(nout));
     if (dWx) SSQB_CUDA(dWs.ensure(nout));
     if (ssq) SSQB_CUDA(Ts.ensure(nout));
     SSQB_CUDA(cudaMemcpyAsync(xs.p, x, nx * sizeof(T), cudaMemcpyHostToDevice, st));
-    int rc = exec(xs.p, B, Ws.p, dWx ? dWs.p : nullptr, ssq ? Ts.p : nullptr, ssq, out_mul_host, rpadded, st);
+    int rc = exec(xs.p, B, Wx ? Ws.p : nullptr, dWx ? dWs.p : nullptr, ssq ? Ts.p : nullptr, ssq,
+                  out_mul_host, rpadded, st);
     if (rc == 0) {
-      SSQB_CUDA(cudaMemcpyAsync(Wx, Ws.p, nout * sizeof(cx<T>), cudaMemcpyDeviceToHost, st));
+      if (Wx) SSQB_CUDA(cudaMemcpyAsync(Wx, Ws.p, nout * sizeof(cx<T>), cudaMemcpyDeviceToHost, st));
       if (dWx) SSQB_CUDA(cudaMemcpyAsync(dWx, dWs.p, nout * sizeof(cx<T>), cudaMemcpyDeviceToHost, st));
       if (ssq) SSQB_CUDA(cudaMemcpyAsync(Tx, Ts.p, nout * sizeof(cx<T>), cudaMemcpyDeviceToHost, st));
     }

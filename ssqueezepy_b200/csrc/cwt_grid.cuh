@@ -291,9 +291,9 @@ template <typename T, int K, int PPK> struct InterpGeom {
   static constexpr int NT = 256;
 };
 
-template <typename T, int K, int PPK, int NARR, bool SSQ, bool REGWIN>
-__global__ void __launch_bounds__(256, (sizeof(T) == 4) ? 3 : 1)
-grid_interp_kernel(const GridArgs<T> G) {
+// STORE_W = false: the fused epilogue without the Wx store (grid_interp_tx_kernel)
+template <typename T, int K, int PPK, int NARR, bool SSQ, bool REGWIN, bool STORE_W>
+__device__ __forceinline__ void grid_interp_body(const GridArgs<T>& G) {
   constexpr int PP = K * PPK;
   constexpr int NT = 256;
   using V4 = typename V4T<T>::type;
@@ -357,7 +357,7 @@ grid_interp_kernel(const GridArgs<T> G) {
   const int a = ri.a;
   const long long row = (long long)b * A.na + a;
   const int Nout = (int)A.Nout;
-  cx<T>* __restrict__ Wrow = A.Wx + row * Nout;
+  cx<T>* __restrict__ Wrow = STORE_W ? A.Wx + row * Nout : nullptr;
   cx<T>* __restrict__ dWrow = A.dWx ? A.dWx + row * Nout : nullptr;
   cx<T>* __restrict__ Tb = A.Tx ? A.Tx + (long long)b * A.na * Nout : nullptr;
   cx<T>* __restrict__ Zrow = (SSQ && b < A.zero_next) ? A.Tx + row * Nout + A.zero_off : nullptr;   // zero-ahead
@@ -395,7 +395,7 @@ grid_interp_kernel(const GridArgs<T> G) {
         if (NARR == 2 && G.write_dWx) dWrow[jo] = cscale<T>(cmul<T>(ad, tw), mlt);
       } else {
         const cx<T> dW = cmul<T>(ad, tw);
-        Wrow[jo] = W;
+        if (STORE_W) Wrow[jo] = W;
         if (G.write_dWx) dWrow[jo] = dW;
         if (Zrow) Zrow[jo] = mkc<T>((T)0, (T)0);
         ssq_point<T>(W, dW, Tb + jo, rowbytes, cre, cwide, g2lo, g2hi, fast_ok, A.grid);
@@ -441,6 +441,19 @@ grid_interp_kernel(const GridArgs<T> G) {
       emit(i, aw, ad);
     }
   }
+}
+
+template <typename T, int K, int PPK, int NARR, bool SSQ, bool REGWIN>
+__global__ void __launch_bounds__(256, (sizeof(T) == 4) ? 3 : 1)
+grid_interp_kernel(const GridArgs<T> G) {
+  grid_interp_body<T, K, PPK, NARR, SSQ, REGWIN, true>(G);
+}
+
+// ssq call that skips Wx: Tx, dWx (when asked for) and the zero-ahead stores as above
+template <typename T, int K, int PPK, bool REGWIN>
+__global__ void __launch_bounds__(256, (sizeof(T) == 4) ? 3 : 1)
+grid_interp_tx_kernel(const GridArgs<T> G) {
+  grid_interp_body<T, K, PPK, 2, true, REGWIN, false>(G);
 }
 
 

@@ -89,7 +89,14 @@ static int launch_pass2(const CwtArgs<T>& A, int write_dWx, cudaStream_t st) {
 
 static int g_rows_bpt = 1;     // butterflies per thread in the row kernels (SSQB_BPT=1|2)
 
-template <typename T, int LOGE, int LOG_F, int NARR, int GEN, int QMAX, bool SSQ, int BPT>
+// STORE_W = false: the ssq call skips Wx (cwt_rows_tx_kernel)
+template <typename T, int LOGE, int LOG_F, int NARR, int GEN, int QMAX, bool SSQ, int BPT, bool STORE_W>
+static auto rows_kernel() {
+  if constexpr (STORE_W) return cwt_rows_kernel<T, LOGE, LOG_F, NARR, GEN, QMAX, SSQ, BPT>;
+  else return cwt_rows_tx_kernel<T, LOGE, LOG_F, GEN, QMAX, BPT>;
+}
+
+template <typename T, int LOGE, int LOG_F, int NARR, int GEN, int QMAX, bool SSQ, int BPT, bool STORE_W>
 static int launch_rows_b(const FastArgs<T>& P, unsigned grid_y, cudaStream_t st) {
   constexpr int ELEMS = 1 << LOGE;
   constexpr int NT = ELEMS / (8 * BPT);
@@ -98,7 +105,7 @@ static int launch_rows_b(const FastArgs<T>& P, unsigned grid_y, cudaStream_t st)
   size_t smem = (size_t)512 * sizeof(cx<T>);
   if (LOG_F > 3) smem += (size_t)NARR * RowsTile<T, LOGE, LOG_F>::SARR * sizeof(cx<T>);
   if (GEN == GEN_DIRECT) smem += (size_t)QMAX * F * 4 * sizeof(T);
-  auto kern = cwt_rows_kernel<T, LOGE, LOG_F, NARR, GEN, QMAX, SSQ, BPT>;
+  auto kern = rows_kernel<T, LOGE, LOG_F, NARR, GEN, QMAX, SSQ, BPT, STORE_W>();
   static size_t attr_smem = 0;
   if (smem > attr_smem) {
     SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -111,16 +118,25 @@ static int launch_rows_b(const FastArgs<T>& P, unsigned grid_y, cudaStream_t st)
   return 0;
 }
 
-template <typename T, int LOGE, int LOG_F, int NARR, int GEN, int QMAX, bool SSQ>
+template <typename T, int LOGE, int LOG_F, int NARR, int GEN, int QMAX, bool SSQ, bool STORE_W = true>
 static int launch_rows_s(const FastArgs<T>& P, unsigned grid_y, cudaStream_t st) {
-  // 1024-thread CTAs need <= 64 registers: float32 only
-  if (g_rows_bpt == 1 && sizeof(T) == 4)
-    return launch_rows_b<T, LOGE, LOG_F, NARR, GEN, QMAX, SSQ, 1>(P, grid_y, st);
-  return launch_rows_b<T, LOGE, LOG_F, NARR, GEN, QMAX, SSQ, 2>(P, grid_y, st);
+  // Tx only: two butterflies per thread whatever SSQB_BPT says.  At one butterfly per thread (1024
+  // threads, <= 64 registers) ptxas spills 12-32 B of the Tx-only body where the storing twin
+  // spills 0-16 B; at two it spills nothing
+  if constexpr (!STORE_W) {
+    return launch_rows_b<T, LOGE, LOG_F, NARR, GEN, QMAX, SSQ, 2, false>(P, grid_y, st);
+  } else {
+    // 1024-thread CTAs need <= 64 registers: float32 only
+    if (g_rows_bpt == 1 && sizeof(T) == 4)
+      return launch_rows_b<T, LOGE, LOG_F, NARR, GEN, QMAX, SSQ, 1, true>(P, grid_y, st);
+    return launch_rows_b<T, LOGE, LOG_F, NARR, GEN, QMAX, SSQ, 2, true>(P, grid_y, st);
+  }
 }
 
 template <typename T, int LOGE, int LOG_F, int NARR, int GEN, int QMAX>
 static int launch_rows_t(const FastArgs<T>& P, unsigned grid_y, cudaStream_t st) {
+  if (NARR == 2 && P.ssq && !P.A.Wx)
+    return launch_rows_s<T, LOGE, LOG_F, 2, GEN, QMAX, true, false>(P, grid_y, st);
   if (NARR == 2 && P.ssq)
     return launch_rows_s<T, LOGE, LOG_F, 2, GEN, QMAX, true>(P, grid_y, st);
   return launch_rows_s<T, LOGE, LOG_F, NARR, GEN, QMAX, false>(P, grid_y, st);
@@ -275,12 +291,13 @@ static int launch_sblk_fwd(const SblkArgs<T>& S, cudaStream_t st) {
 // interpolation has drained.
 enum SblkShare { SBLK_ALONE, SBLK_BESIDE_GRID, SBLK_TAIL };
 
-template <typename T, int NARR, bool SSQ>
+template <typename T, int NARR, bool SSQ, bool STORE_W = true>
 static int launch_sblk_rows_t(const SblkArgs<T>& S, SblkShare share, cudaStream_t st) {
   constexpr int LP = SblkGeom<T>::LOG_P, NT = SblkGeom<T>::NT;
   using V4 = typename V4T<T>::type;
   size_t smem = ((size_t)1 << LP) * (sizeof(V4) + sizeof(cx<T>));
   auto kern = sblk_rows_kernel<T, LP, SblkGeom<T>::LOG_R, NARR, SSQ>;
+  if constexpr (!STORE_W) kern = sblk_rows_tx_kernel<T, LP, SblkGeom<T>::LOG_R>;
   static bool attr_set = false;
   static int sms = 132, per = 2, prio_high = 0;
   if (!attr_set) {
@@ -308,6 +325,7 @@ static int launch_sblk_rows_t(const SblkArgs<T>& S, SblkShare share, cudaStream_
 }
 template <typename T>
 static int launch_sblk_rows(const SblkArgs<T>& S, int narr, bool ssq, SblkShare share, cudaStream_t st) {
+  if (narr == 2 && ssq && !S.A.Wx) return launch_sblk_rows_t<T, 2, true, false>(S, share, st);
   if (narr == 2 && ssq) return launch_sblk_rows_t<T, 2, true>(S, share, st);
   if (narr == 2) return launch_sblk_rows_t<T, 2, false>(S, share, st);
   return launch_sblk_rows_t<T, 1, false>(S, share, st);
@@ -460,13 +478,14 @@ template <typename T> static int interp_ppk(bool ssq, int narr) {
   return GridTaps<T>::PPK;
 }
 
-template <typename T, int NARR, bool SSQ, bool RW, int PPK = GridTaps<T>::PPK>
+template <typename T, int NARR, bool SSQ, bool RW, int PPK = GridTaps<T>::PPK, bool STORE_W = true>
 static int launch_grid_interp_t(const GridArgs<T>& G, unsigned max_tiles, cudaStream_t st) {
   constexpr int K = GridTaps<T>::K, PP = K * PPK;
   using V4 = typename V4T<T>::type;
   // coarse samples per CTA = (256 / min(U, 256)) * PP; U >= 16
   size_t smem = (size_t)(16 * PP + K - 1) * sizeof(V4) + (size_t)16 * PP * sizeof(cx<T>);
   auto kern = grid_interp_kernel<T, K, PPK, NARR, SSQ, RW>;
+  if constexpr (!STORE_W) kern = grid_interp_tx_kernel<T, K, PPK, RW>;
   static bool attr_set = false;
   if (!attr_set) {
     SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -484,10 +503,23 @@ static int launch_grid_interp(const GridArgs<T>& G, int narr, unsigned max_tiles
     static int regwin = -1;
     if (regwin < 0) { const char* e = getenv("SSQB_F64_REGWIN"); regwin = e ? atoi(e) : 1; }
     if (!regwin) {
+      if (narr == 2 && G.ssq && !G.A.Wx)
+        return launch_grid_interp_t<T, 2, true, false, GridTaps<T>::PPK, false>(G, max_tiles, st);
       if (narr == 2 && G.ssq) return launch_grid_interp_t<T, 2, true, false>(G, max_tiles, st);
       if (narr == 2) return launch_grid_interp_t<T, 2, false, false>(G, max_tiles, st);
       return launch_grid_interp_t<T, 1, false, false>(G, max_tiles, st);
     }
+  }
+  if (narr == 2 && G.ssq && !G.A.Wx) {              // Tx only: the same PPK choices as below
+    if constexpr (sizeof(T) == 4)
+      switch (interp_ppk<T>(true, 2)) {
+        case 8:  return launch_grid_interp_t<T, 2, true, true, 8, false>(G, max_tiles, st);
+        case 16: return launch_grid_interp_t<T, 2, true, true, 16, false>(G, max_tiles, st);
+        default: break;
+      }
+    if constexpr (sizeof(T) == 8)
+      if (interp_ppk<T>(true, 2) == 4) return launch_grid_interp_t<T, 2, true, true, 4, false>(G, max_tiles, st);
+    return launch_grid_interp_t<T, 2, true, true, GridTaps<T>::PPK, false>(G, max_tiles, st);
   }
   if (narr == 2 && G.ssq) {
     if constexpr (sizeof(T) == 4)
@@ -1356,7 +1388,7 @@ struct CwtPlan : public CwtPlanBase {
         zero_next_ = (b0 + S < B) ? (int)S : 0;
         zero_off_ = (long long)((size_t)S * plane);
         rc = exec_body((const T*)xv + (size_t)b0 * (size_t)d.N, S,
-                       (cx<T>*)Wxv + (size_t)b0 * plane,
+                       Wxv ? (cx<T>*)Wxv + (size_t)b0 * plane : nullptr,
                        dWxv ? (cx<T>*)dWxv + (size_t)b0 * plane : nullptr,
                        (cx<T>*)Txv + (size_t)b0 * plane, ssq, out_mul_host, rpadded, st);
       }
@@ -1380,7 +1412,7 @@ struct CwtPlan : public CwtPlanBase {
   int exec_body(const void* xv, long long B, void* Wxv, void* dWxv, void* Txv, bool ssq,
                 const double* out_mul_host, bool rpadded, cudaStream_t st) {
     if (B < 1) return set_error(SSQB_E_ARG, "B must be >= 1");
-    if (!xv || !Wxv) return set_error(SSQB_E_ARG, "null x / Wx");
+    if (!xv || (!Wxv && !ssq)) return set_error(SSQB_E_ARG, "null x / Wx");   // ssq: Wx may be NULL
     if (ssq && (!Txv || !have_grid))
       return set_error(SSQB_E_ARG, "ssq needs Tx and ssqb_cwt_plan_set_reassign()");
     if (ssq && rpadded) return set_error(SSQB_E_ARG, "ssq works on the unpadded part");
@@ -1612,6 +1644,7 @@ struct CwtPlan : public CwtPlanBase {
         acquire(tk, true);                                 // pass 2 writes Tx: wait for the zero fill
         rc = prof_begin(2, nr, ts); if (rc) return rc;
         if (fast)           rc = launch_rows_scratch<T>(P, narr, ts);
+        else if (ssq && !Wx) rc = launch_pass2<T, 2, EPI_SSQ_TX>(A, dWx ? 1 : 0, ts);
         else if (ssq)       rc = launch_pass2<T, 2, EPI_SSQ>(A, dWx ? 1 : 0, ts);
         else if (narr == 2) rc = launch_pass2<T, 2, EPI_CWT>(A, 1, ts);
         else                rc = launch_pass2<T, 1, EPI_CWT>(A, 0, ts);
@@ -1683,7 +1716,7 @@ struct CwtPlan : public CwtPlanBase {
     const long long Nout = rpadded ? d.n_up : d.N;
     const size_t nx = (size_t)CH * (size_t)d.N, nout = (size_t)CH * d.na * (size_t)Nout;
     SSQB_CUDA(x_stage.ensure(2 * nx));
-    SSQB_CUDA(Wx_stage.ensure(2 * nout));
+    if (Wx) SSQB_CUDA(Wx_stage.ensure(2 * nout));
     if (dWx) SSQB_CUDA(dWx_stage.ensure(2 * nout));
     if (ssq) SSQB_CUDA(Tx_stage.ensure(2 * nout));
     if (!copy_st) {
@@ -1703,7 +1736,7 @@ struct CwtPlan : public CwtPlanBase {
       const size_t cx_ = (size_t)nb * (size_t)d.N, co = (size_t)nb * d.na * (size_t)Nout;
       if (slot_busy[sl]) SSQB_CUDA(cudaStreamWaitEvent(st, ev_d2h[sl], 0));   // slot drained
       T* xs = x_stage.p + sl * nx;
-      cx<T>* Ws = Wx_stage.p + sl * nout;
+      cx<T>* Ws = Wx ? Wx_stage.p + sl * nout : nullptr;
       cx<T>* dWs = dWx ? dWx_stage.p + sl * nout : nullptr;
       cx<T>* Ts = ssq ? Tx_stage.p + sl * nout : nullptr;
       SSQB_CUDA(cudaMemcpyAsync(xs, xh_ + (size_t)b0 * (size_t)d.N, cx_ * sizeof(T),
@@ -1713,7 +1746,7 @@ struct CwtPlan : public CwtPlanBase {
       SSQB_CUDA(cudaEventRecord(ev_comp[sl], st));
       SSQB_CUDA(cudaStreamWaitEvent(copy_st, ev_comp[sl], 0));
       const size_t ho = (size_t)b0 * d.na * (size_t)Nout;
-      SSQB_CUDA(cudaMemcpyAsync(Wh + ho, Ws, co * sizeof(cx<T>), cudaMemcpyDeviceToHost, copy_st));
+      if (Wx) SSQB_CUDA(cudaMemcpyAsync(Wh + ho, Ws, co * sizeof(cx<T>), cudaMemcpyDeviceToHost, copy_st));
       if (dWx) SSQB_CUDA(cudaMemcpyAsync(dWh + ho, dWs, co * sizeof(cx<T>), cudaMemcpyDeviceToHost, copy_st));
       if (ssq) SSQB_CUDA(cudaMemcpyAsync(Th + ho, Ts, co * sizeof(cx<T>), cudaMemcpyDeviceToHost, copy_st));
       SSQB_CUDA(cudaEventRecord(ev_d2h[sl], copy_st));

@@ -26,7 +26,8 @@ template <> struct Tile<float>  { static constexpr int ELEMS = 8192; static cons
 template <> struct Tile<double> { static constexpr int ELEMS = 4096; static constexpr int NT = 256; };
 
 enum { MODE_X = 0, MODE_CWT = 1 };
-enum { EPI_FWD = 0, EPI_CWT = 1, EPI_SSQ = 2 };
+// EPI_SSQ_TX: EPI_SSQ without the Wx store (the caller asked for Tx only; zero-ahead stays)
+enum { EPI_FWD = 0, EPI_CWT = 1, EPI_SSQ = 2, EPI_SSQ_TX = 3 };
 enum { WAV_MORLET = 0, WAV_GMW = 1, WAV_TABLE = 2 };
 
 template <typename T>
@@ -64,9 +65,9 @@ struct CwtArgs {
   const cx<T>* tw_hi;          // exp(2 pi i m 2^log_lo / n),   m < n / 2^log_lo
   int log_lo;
   ReassignGrid grid;
-  // zero-ahead (batched ssq calls run in groups of signals): while a thread stores Wx[b][a][j] it
-  // also stores 0 to Tx[b + group][a][j] of the NEXT group, so that only the first group needs a
-  // separate zero fill.  zero_next = signals of the next group (0: none), zero_off = elements
+  // zero-ahead (batched ssq calls run in groups of signals): the thread that owns Wx[b][a][j] (and
+  // stores it, unless the call skips Wx) also stores 0 to Tx[b + group][a][j] of the NEXT group,
+  // so that only the first group needs a separate zero fill.  zero_next = signals of the next group (0: none), zero_off = elements
   // from this group's Tx[b][a][j] to the next group's
   int zero_next;
   long long zero_off;
@@ -338,7 +339,7 @@ cwt_pass2_kernel(const CwtArgs<T> A, const int write_dWx) {
       A.Wx[o] = W;
       if (NARR == 2) A.dWx[o] = dW;
     } else {
-      A.Wx[o] = W;
+      if (EPI == EPI_SSQ) A.Wx[o] = W;
       if (write_dWx) A.dWx[o] = dW;
       if (b < A.zero_next) A.Tx[o + A.zero_off] = mkc<T>((T)0, (T)0);
       if (is_active_fast(W.x, W.y, A.grid.gamma)) {

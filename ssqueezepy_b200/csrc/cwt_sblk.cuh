@@ -175,9 +175,9 @@ __device__ __forceinline__ void sblk_twiddles(const cx<T>* __restrict__ tws, int
   }
 }
 
-template <typename T, int LOG_P, int LOG_R, int NARR, bool SSQ>
-__global__ void __launch_bounds__((1 << LOG_P) >> LOG_R, 2)
-sblk_rows_kernel(const SblkArgs<T> S) {
+// STORE_W = false: the fused epilogue without the Wx store (sblk_rows_tx_kernel)
+template <typename T, int LOG_P, int LOG_R, int NARR, bool SSQ, bool STORE_W>
+__device__ __forceinline__ void sblk_rows_body(const SblkArgs<T>& S) {
   constexpr int P = 1 << LOG_P, R = 1 << LOG_R, NT = P / R;
   static_assert(R == 8 || R == 16, "radix 8 or 16");
   constexpr int NR = LOG_P / LOG_R;                    // radix-R stages
@@ -330,7 +330,7 @@ sblk_rows_kernel(const SblkArgs<T> S) {
     // ---- epilogue: block sample t -> output k*hop + t - h2 -------------------------------------
     const int a = ri.a;
     const long long row = (long long)b * A.na + a;
-    cx<T>* __restrict__ Wrow = A.Wx + row * Nout;
+    cx<T>* __restrict__ Wrow = STORE_W ? A.Wx + row * Nout : nullptr;
     cx<T>* __restrict__ dWrow = A.dWx ? A.dWx + row * Nout : nullptr;
     cx<T>* __restrict__ Tb = A.Tx ? A.Tx + (long long)b * A.na * Nout : nullptr;
     cx<T>* __restrict__ Zrow = (SSQ && b < A.zero_next) ? A.Tx + row * Nout + A.zero_off : nullptr;   // zero-ahead
@@ -364,7 +364,7 @@ sblk_rows_kernel(const SblkArgs<T> S) {
           Wrow[jo] = cscale<T>(W, mlt);
           if (NARR == 2 && S.write_dWx) dWrow[jo] = cscale<T>(dW, mlt);
         } else {
-          Wrow[jo] = W;
+          if (STORE_W) Wrow[jo] = W;
           if (S.write_dWx) dWrow[jo] = dW;
           if (Zrow) Zrow[jo] = mkc<T>((T)0, (T)0);
           if (!ssq_point_fast<T>(W, dW, Tb + jo, rowbytes, cre, cwide, g2lo, g2hi, fast_ok, A.grid)) {
@@ -386,6 +386,19 @@ sblk_rows_kernel(const SblkArgs<T> S) {
     if (it_next >= items) break;
     it = it_next;
   }
+}
+
+template <typename T, int LOG_P, int LOG_R, int NARR, bool SSQ>
+__global__ void __launch_bounds__((1 << LOG_P) >> LOG_R, 2)
+sblk_rows_kernel(const SblkArgs<T> S) {
+  sblk_rows_body<T, LOG_P, LOG_R, NARR, SSQ, true>(S);
+}
+
+// ssq call that skips Wx: Tx, dWx (when asked for) and the zero-ahead stores as above
+template <typename T, int LOG_P, int LOG_R>
+__global__ void __launch_bounds__((1 << LOG_P) >> LOG_R, 2)
+sblk_rows_tx_kernel(const SblkArgs<T> S) {
+  sblk_rows_body<T, LOG_P, LOG_R, 2, true, false>(S);
 }
 
 }  // namespace ssqb

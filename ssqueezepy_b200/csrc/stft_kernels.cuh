@@ -47,8 +47,9 @@ __device__ __forceinline__ long long frame_src(int l, long long i, int hop, int 
 
 // What the transform of a frame feeds: Sx (+ dSx), the same plus the fused reassignment
 // (ssq_stft), or the istft adjoint, which transforms one real sequence (no dSx half) and
-// writes gSx[k] = (c_k / n_fft) C[k]  (c_0 = c_{n_fft/2} = 1, otherwise 2).
-enum { STFT_EPI_PLAIN = 0, STFT_EPI_SSQ = 1, STFT_EPI_ISTFT_BWD = 2 };
+// writes gSx[k] = (c_k / n_fft) C[k]  (c_0 = c_{n_fft/2} = 1, otherwise 2).  STFT_EPI_SSQ_TX is
+// STFT_EPI_SSQ without the Sx store (the caller asked for Tx only).
+enum { STFT_EPI_PLAIN = 0, STFT_EPI_SSQ = 1, STFT_EPI_ISTFT_BWD = 2, STFT_EPI_SSQ_TX = 3 };
 
 template <typename T, int EPI>
 __device__ __forceinline__ void stft_emit(const StftArgs<T>& A, int b, int k, long long frame,
@@ -66,9 +67,9 @@ __device__ __forceinline__ void stft_emit(const StftArgs<T>& A, int b, int k, lo
     return;
   }
   cx<T> dS = mkc<T>((Ck.y + Cmk.y) * h * A.inv_kappa, (Cmk.x - Ck.x) * h * A.inv_kappa);
-  A.Sx[o] = S;
+  if (EPI != STFT_EPI_SSQ_TX) A.Sx[o] = S;
   if (A.write_dSx) A.dSx[o] = dS;
-  if (EPI == STFT_EPI_SSQ && is_active_exact(S.x, S.y, A.grid.gamma)) {
+  if ((EPI == STFT_EPI_SSQ || EPI == STFT_EPI_SSQ_TX) && is_active_exact(S.x, S.y, A.grid.gamma)) {
     double r = phase_ratio_exact<T>(dS.x, dS.y, S.x, S.y);
     double w = fabs((double)A.Sfs[k] - r);
     int kk = bin_from_w_exact(w, A.grid);

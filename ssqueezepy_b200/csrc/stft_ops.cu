@@ -172,7 +172,10 @@ static int stft_t(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const vo
   }
   int logm = ilog2_exact(M);
   int rc;
-  if (logm >= 1 && logm <= 12 && (Tile<T>::ELEMS >> logm) >= 1)
+  const bool pow2 = logm >= 1 && logm <= 12 && (Tile<T>::ELEMS >> logm) >= 1;
+  if (ssq && !Sx)        // Tx only
+    rc = pow2 ? launch_stft_pow2<T, STFT_EPI_SSQ_TX>(A, logm, st) : launch_stft_generic<T, STFT_EPI_SSQ_TX>(A, st);
+  else if (pow2)
     rc = ssq ? launch_stft_pow2<T, STFT_EPI_SSQ>(A, logm, st) : launch_stft_pow2<T, STFT_EPI_PLAIN>(A, logm, st);
   else
     rc = ssq ? launch_stft_generic<T, STFT_EPI_SSQ>(A, st) : launch_stft_generic<T, STFT_EPI_PLAIN>(A, st);
@@ -181,7 +184,7 @@ static int stft_t(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const vo
 
 int run_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const void* x, long long B,
              void* Sx, void* Tx, void* dSx, bool ssq, cudaStream_t st) {
-  if (!d || !x || !Sx) return set_error(SSQB_E_ARG, "null pointer");
+  if (!d || !x || (!Sx && !ssq)) return set_error(SSQB_E_ARG, "null pointer");   // ssq: Sx may be NULL
   if (!d->win_host || !d->dwin_host || !d->Sfs_host) return set_error(SSQB_E_ARG, "null table");
   if (ssq && (!r || !r->cst_host || !Tx)) return set_error(SSQB_E_ARG, "ssq needs Tx + reassign");
   if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");

@@ -39,10 +39,12 @@ def gather_batch(local, B, group=None):
     return torch.cat([p[:hi - lo] for p, (lo, hi) in zip(parts, sizes)], dim=0)
 
 
-def ssq_cwt_sharded(x, *args, gather=False, group=None, _compute=None, **kw):
+def ssq_cwt_sharded(x, *args, gather=False, group=None, _compute=None, get_Wx=True, **kw):
     """`ssq_cwt` on this rank's slice of the batch `x` ([B, N], identical on every
     rank).  Returns `(Tx, Wx, ssq_freqs, scales)` for the local slice, or for the
-    whole batch if `gather=True`.  `_compute` (tests) replaces the transform."""
+    whole batch if `gather=True`.  With `get_Wx=False`, `Wx` is None: it is neither
+    computed into memory on the fused route nor gathered, which halves the gather.
+    `_compute` (tests) replaces the transform."""
     if x.ndim != 2:
         raise ValueError("sharded execution needs a batched input [B, N]; a single "
                          "signal does not shard (one global FFT): run replicas")
@@ -52,11 +54,14 @@ def ssq_cwt_sharded(x, *args, gather=False, group=None, _compute=None, **kw):
     lo, hi = shard_bounds(B, rank, world)
     if _compute is None:
         from ._ssq_cwt import ssq_cwt as _compute
+    if not get_Wx:
+        kw['get_Wx'] = False
     if hi > lo:
         Tx, Wx, ssq_freqs, scales = _compute(x[lo:hi], *args, **kw)[:4]
     else:                                   # more ranks than signals
         Tx1, Wx1, ssq_freqs, scales = _compute(x[:1], *args, **kw)[:4]
-        Tx, Wx = Tx1[:0], Wx1[:0]
+        Tx, Wx = Tx1[:0], (None if Wx1 is None else Wx1[:0])
     if gather and world > 1:
-        Tx, Wx = gather_batch(Tx, B, group), gather_batch(Wx, B, group)
+        Tx = gather_batch(Tx, B, group)
+        Wx = None if Wx is None else gather_batch(Wx, B, group)
     return Tx, Wx, ssq_freqs, scales
