@@ -215,6 +215,23 @@ int ssqb_ssq_stft_exec(const ssqb_stft_desc* d, const ssqb_reassign_desc* r,
 int ssqb_ssq_stft_exec_host(const ssqb_stft_desc* d, const ssqb_reassign_desc* r,
                             const void* x_host, int64_t B, void* Sx_host,
                             void* Tx_host, void* dSx_host, void* stream);
+/* second-order ssq_stft (Oberlin, Meignen & Perrier, IEEE TSP 2015; not in the reference): the
+ * reassigned frequency corrects the first-order estimate by the local frequency modulation,
+ * which makes it exact for linear chirps under Gaussian windows.  Modulated frames only.  The
+ * three extra tables are [n_fft] of the data dtype, ifftshifted like win_host; with
+ * tau_l = (l - n_fft/2) / fs on the unshifted window:                                          */
+typedef struct {
+  const void* ddwin_host;  /* second spectral derivative of the window, times fs^2          */
+  const void* twin_host;   /* tau * window                                                  */
+  const void* tdwin_host;  /* tau * diff window (the dwin_host values, times fs)            */
+} ssqb_stft2_tables;
+/* Tx_dev set: like ssqb_ssq_stft_exec (Tx zeroed here; Sx_dev may be NULL = Tx only; dSx_dev
+ * may be NULL); w_dev must then be NULL.  Tx_dev NULL: w-only mode, w_dev [B][n_fft/2+1][n_hops]
+ * real receives the second-order w (inf where |Sx| < gamma, as ssqb_phase_stft), Sx_dev and
+ * dSx_dev are stored when not NULL.  r: the ssqb_ssq_stft_exec reassignment (SSQB_GRID_STFT). */
+int ssqb_ssq_stft2_exec(const ssqb_stft_desc* d, const ssqb_stft2_tables* t,
+                        const ssqb_reassign_desc* r, const void* x_dev, int64_t B,
+                        void* Sx_dev, void* Tx_dev, void* dSx_dev, void* w_dev, void* stream);
 /* backward of stft (_stft.py:127-146, differentiable here through torch.autograd): adjoint of
  * the linear map x -> (Sx, dSx), same descriptor as ssqb_stft_exec.  gSx_dev, gdSx_dev
  * [B][n_fft/2+1][n_hops] complex gradients (g = dL/dRe + i dL/dIm; either may be NULL);

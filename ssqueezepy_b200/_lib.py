@@ -30,7 +30,7 @@ SYMBOLS = [
     'ssqb_ssq_cwt_exec_host', 'ssqb_cwt_debug_xh', 'ssqb_cwt_plan_set_profiling',
     'ssqb_cwt_plan_get_profile', 'ssqb_ssqueeze',
     'ssqb_indexed_sum', 'ssqb_phase_cwt', 'ssqb_phase_stft', 'ssqb_stft_exec',
-    'ssqb_ssq_stft_exec', 'ssqb_ssq_stft_exec_host',
+    'ssqb_ssq_stft_exec', 'ssqb_ssq_stft_exec_host', 'ssqb_ssq_stft2_exec',
     'ssqb_colsum_real', 'ssqb_invert_components', 'ssqb_istft_exec', 'ssqb_extract_ridges', 'ssqb_cwt_backward',
     'ssqb_stft_backward', 'ssqb_istft_backward', 'ssqb_ssqueeze_backward',
     'ssqb_indexed_sum_backward', 'ssqb_colsum_real_backward',
@@ -64,6 +64,11 @@ class StftDesc(C.Structure):
                 ('modulated', C.c_int),
                 ('win_host', C.c_void_p), ('dwin_host', C.c_void_p),
                 ('Sfs_host', C.c_void_p)]
+
+
+class Stft2Tables(C.Structure):
+    _fields_ = [('ddwin_host', C.c_void_p), ('twin_host', C.c_void_p),
+                ('tdwin_host', C.c_void_p)]
 
 
 class IstftDesc(C.Structure):
@@ -112,6 +117,8 @@ def _bind(lib):
     lib.ssqb_ssq_stft_exec_host.argtypes = [C.POINTER(StftDesc),
                                             C.POINTER(ReassignDesc),
                                             vp, i64, vp, vp, vp, vp]
+    lib.ssqb_ssq_stft2_exec.argtypes = [C.POINTER(StftDesc), C.POINTER(Stft2Tables),
+                                        C.POINTER(ReassignDesc), vp, i64, vp, vp, vp, vp, vp]
     lib.ssqb_colsum_real.argtypes = [ci, ci, vp, i64, ci, i64, C.POINTER(dbl), dbl, ci, vp, vp]
     lib.ssqb_invert_components.argtypes = [ci, vp, ci, i64, vp, vp, ci, dbl, vp, vp]
     lib.ssqb_istft_exec.argtypes = [C.POINTER(IstftDesc), vp, i64, vp, vp]

@@ -59,14 +59,25 @@ class _SsqStftFn(torch.autograd.Function):
 def ssq_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=None,
              modulated=True, ssq_freqs=None, padtype='reflect', squeezing='sum',
              gamma=None, preserve_transform=None, dtype=None, astensor=True,
-             flipud=False, get_w=False, get_dWx=False, get_Sx=True):
+             flipud=False, get_w=False, get_dWx=False, get_Sx=True, ssq_order=1):
     """Returns `(Tx, Sx, ssq_freqs, Sfs[, w][, dSx])` like the reference.
+
+    `ssq_order=2` reassigns by the second-order frequency estimate (Oberlin, Meignen &
+    Perrier, IEEE TSP 2015), which corrects the first-order bias in proportion to the
+    frequency modulation: exact for linear chirps under a Gaussian window, and the column
+    sums of `Tx` (so `issq_stft`) are those of the first order.  Needs `modulated=True`.
+    `get_w` then returns the second-order `w`.  With `x.requires_grad` the gradient holds
+    every bin where the forward put it, as at first order.
 
     `get_Sx=False` returns `Sx` as None, in the same position.  On the fused
     route (`squeezing='sum'`, no `get_w`, no `ssq_freqs`) `Sx` is then never
     allocated or written.  The two-step routes compute `Sx` as the input of
     `ssqueeze` and drop it before returning, so they save no peak memory.  With
     `x.requires_grad`, `Sx` and `dSx` are still kept for the backward."""
+    if ssq_order not in (1, 2) or isinstance(ssq_order, bool):
+        raise ValueError("`ssq_order` must be 1 or 2 (got %s)" % (ssq_order,))
+    if ssq_order == 2 and not modulated:
+        raise ValueError("`ssq_order=2` requires `modulated=True`")
     if x.ndim == 2 and get_w:
         raise NotImplementedError("`get_w=True` unsupported with batched input.")
     N = x.shape[-1]
@@ -77,6 +88,11 @@ def ssq_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=Non
         raise ValueError("`ssq_freqs` must be linearly distributed "
                          "for `ssq_stft`")
     fused = (squeezing == 'sum') and not get_w and ssq_freqs is None
+    grad = torch.is_tensor(x) and x.requires_grad
+    if ssq_order == 2 and not (fused and not grad):
+        return _ssq_stft2_twostep(x, N, window, n_fft, win_len, hop_len, fs, modulated,
+                                  ssq_freqs, padtype, squeezing, gamma, dtype, astensor,
+                                  flipud, get_w, get_dWx, get_Sx)
     if fused:
         lib = Bk.require_cuda()
         call = _get_call(N, window, n_fft, win_len, hop_len, fs, padtype, modulated, dtype)
@@ -87,7 +103,16 @@ def ssq_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=Non
         xd = Bk.to_device(x, call.dtype)
         x2 = xd if xd.ndim == 2 else xd.unsqueeze(0)
         B = x2.shape[0]
-        if torch.is_tensor(x) and x.requires_grad:
+        if ssq_order == 2:
+            outs = call.outputs(B, int(get_Sx) + 1 + int(get_dWx))
+            Sx = outs.pop(0) if get_Sx else None
+            Tx = outs.pop(0)
+            dSx = outs.pop(0) if get_dWx else None
+            _lib.check(lib.ssqb_ssq_stft2_exec(C.byref(call.desc), C.byref(call.order2_tables()),
+                                               C.byref(desc), x2.data_ptr(), B, Bk.ptr(Sx),
+                                               Tx.data_ptr(), Bk.ptr(dSx), None,
+                                               Bk.stream_ptr()))
+        elif torch.is_tensor(x) and x.requires_grad:
             Tx, Sx, dSx = _SsqStftFn.apply(x2, call, desc)
             dSx = dSx if get_dWx else None
             Sx = Sx if get_Sx else None       # the backward keeps its own reference
@@ -129,6 +154,10 @@ def ssq_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=Non
             Sx = None
         Sfs_out = torch.as_tensor(Sfs, device='cuda') if astensor else Sfs
 
+    return _pack(Tx, Sx, ssq_freqs, Sfs_out, w, dSx, astensor, get_w, get_dWx)
+
+
+def _pack(Tx, Sx, ssq_freqs, Sfs_out, w, dSx, astensor, get_w, get_dWx):
     if not astensor:
         Tx, Sx, w, dSx = [Bk.finish(g, False) for g in (Tx, Sx, w, dSx)]
     if get_w and get_dWx:
@@ -138,6 +167,44 @@ def ssq_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=Non
     elif get_dWx:
         return Tx, Sx, ssq_freqs, Sfs_out, dSx
     return Tx, Sx, ssq_freqs, Sfs_out
+
+
+def _ssq_stft2_twostep(x, N, window, n_fft, win_len, hop_len, fs, modulated, ssq_freqs,
+                       padtype, squeezing, gamma, dtype, astensor, flipud, get_w, get_dWx,
+                       get_Sx):
+    """Second order, every route but the fused one: the second-order `w` from
+    `ssqb_ssq_stft2_exec` in w-only mode, then `ssqueeze(Sx, w, ...)`.  With `x.requires_grad`,
+    `Sx` comes from the differentiable `stft` and `w` (which only chooses bins) from a detached
+    call, so the gradient is that of `indexed_sum_onfly` with the bins held."""
+    lib = Bk.require_cuda()
+    call = _get_call(N, window, n_fft, win_len, hop_len, fs, padtype, modulated, dtype)
+    if gamma is None:
+        gamma = 10 * (EPS64 if call.dtype == 'float64' else EPS32)
+    Sfs = call.Sfs.copy()
+    desc = call.reassign_desc(flipud, gamma, make_reassign_desc)
+    xd = Bk.to_device(x, call.dtype)
+    x2 = xd if xd.ndim == 2 else xd.unsqueeze(0)
+    B = x2.shape[0]
+    w = torch.empty((B, call.n_rows, call.n_hops), dtype=Bk.real_dtype(call.dtype), device='cuda')
+    if torch.is_tensor(x) and x.requires_grad:
+        Sx, dSx = stft(x, window, n_fft=n_fft, win_len=win_len, hop_len=hop_len, fs=fs,
+                       padtype=padtype, modulated=modulated, derivative=True, dtype=dtype)
+        S_, dS_ = None, None
+    else:
+        Sx, dSx = call.outputs(B, 2)
+        S_, dS_ = Sx, (dSx if get_dWx else None)
+    _lib.check(lib.ssqb_ssq_stft2_exec(C.byref(call.desc), C.byref(call.order2_tables()),
+                                       C.byref(desc), x2.detach().data_ptr(), B, Bk.ptr(S_),
+                                       None, Bk.ptr(dS_), w.data_ptr(), Bk.stream_ptr()))
+    if x.ndim == 1:
+        w = w[0]
+        Sx, dSx = (Sx, dSx) if Sx.ndim == 2 else (Sx[0], dSx[0])
+    Tx, ssq_freqs = ssqueeze(Sx, w, squeezing=squeezing,
+                             ssq_freqs=Sfs if ssq_freqs is None else ssq_freqs, Sfs=Sfs,
+                             flipud=flipud, gamma=gamma, maprange='maximal', transform='stft')
+    Sfs_out = torch.as_tensor(Sfs, device='cuda') if astensor else Sfs
+    return _pack(Tx, Sx if get_Sx else None, ssq_freqs, Sfs_out, w if get_w else None,
+                 dSx if get_dWx else None, astensor, get_w, get_dWx)
 
 
 def phase_stft(Sx, dSx, Sfs, gamma=None, parallel=None):

@@ -137,6 +137,31 @@ class _StftCall:
         self.desc = d
         self._Sfs_dev = None
         self._rdesc = {}
+        self._window_spec, self._win_len, self.fs = window, win_len, fs
+        self._tables2 = None
+
+    def order2_tables(self):
+        """`ssqb_stft2_tables` of second-order synchrosqueezing, built on first use: g'' (the
+        second spectral derivative of the window, times fs^2), tau g and tau g' (g' times fs),
+        tau = (l - n_fft//2) / fs on the unshifted window, all ifftshifted like `_win`."""
+        if self._tables2 is None:
+            import scipy.fft as sfft
+            w = np.asarray(get_window(self._window_spec, self._win_len, self.n_fft,
+                                      dtype='float64'), dtype=np.float64)
+            n, fs = len(w), self.fs
+            xi = xi_grid(n)
+            if n % 2 == 0:
+                xi[n // 2] = 0
+            wh = sfft.fft(w)
+            d1 = sfft.ifft(wh * 1j * xi).real * fs
+            d2 = sfft.ifft(wh * (1j * xi) ** 2).real * fs ** 2
+            tau = (np.arange(n) - n // 2) / fs
+            arrs = [np.ascontiguousarray(np.fft.ifftshift(a), dtype=self.dtype)
+                    for a in (d2, tau * w, tau * d1)]
+            t = _lib.Stft2Tables(*[a.ctypes.data for a in arrs])
+            t._keep = arrs          # the host arrays live as long as the struct
+            self._tables2 = t
+        return self._tables2
 
     def Sfs_tensor(self):
         """`Sfs` on the device (uploaded once per call object; callers get a copy)."""

@@ -143,6 +143,12 @@ int ssqb_ssq_stft_exec(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, con
   return run_stft(d, r, x, B, Sx, Tx, dSx, true, (cudaStream_t)stream);
 }
 
+int ssqb_ssq_stft2_exec(const ssqb_stft_desc* d, const ssqb_stft2_tables* t,
+                        const ssqb_reassign_desc* r, const void* x, int64_t B, void* Sx, void* Tx,
+                        void* dSx, void* w, void* stream) {
+  return run_stft2(d, t, r, x, B, Sx, Tx, dSx, w, (cudaStream_t)stream);
+}
+
 int ssqb_ssq_stft_exec_host(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const void* x,
                             int64_t B, void* Sx, void* Tx, void* dSx, void* stream) {
   if (!d || !x || !Tx) return set_error(SSQB_E_ARG, "null argument");   // Sx may be NULL

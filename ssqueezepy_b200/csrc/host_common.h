@@ -99,6 +99,8 @@ int run_phase(int dtype, bool stft, const void* Wx, const void* dWx, const void*
               long long total, long long ncols, int nrows, double gamma, cudaStream_t st);
 int run_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const void* x, long long B,
              void* Sx, void* Tx, void* dSx, bool ssq, cudaStream_t st);
+int run_stft2(const ssqb_stft_desc* d, const ssqb_stft2_tables* t2, const ssqb_reassign_desc* r,
+              const void* x, long long B, void* Sx, void* Tx, void* dSx, void* w, cudaStream_t st);
 int run_stft_backward(const ssqb_stft_desc* d, const void* gSx, const void* gdSx, long long B,
                       void* gx, cudaStream_t st);
 int run_istft_backward(const ssqb_istft_desc* d, const void* gx, long long B, void* gSx,

@@ -308,4 +308,186 @@ stft_bwd_fold_kernel(const StftBwdArgs<T> A) {
   }
 }
 
+// ---- second-order synchrosqueezing: ssq_stft(ssq_order=2) ------------------------------------
+// Each frame needs five windowed spectra: V^g, V^g' (the first-order pair), V^g'', V^{tau g} and
+// V^{tau g'}, tau = (frame position - n_fft//2) / fs.  They travel as three complex transforms:
+//   c1 = f g + i kappa  f g'       (the first-order packing)
+//   c2 = f tau g + i kappa2 f tau g'
+//   c3 = f g''                     (real; the spectrum is C3[k] itself)
+// The first-order kernels above are untouched; Stft2Args carries their arguments unchanged.
+template <typename T>
+struct Stft2Args {
+  StftArgs<T> A;            // framing, g / g' tables, kappa, Sx / dSx / Tx, Sfs, cst, grid
+  const T* ddwin;           // [n_fft] g'' * fs^2, ifftshifted like win
+  const T* twin;            // [n_fft] tau * g
+  const T* tdwin;           // [n_fft] tau * g' (g' already times fs)
+  T kappa2, inv_kappa2;     // power of two balancing ||tau g|| and ||tau g'||
+  T* w;                     // [B][n_fft/2+1][n_hops] (STFT2_EPI_W) or nullptr
+  T gamma_t;                // gamma in the data type: w = inf where |Sx| < gamma (phase_stft)
+};
+
+// SSQ2 stores Sx and scatters into Tx; SSQ2_TX does not store Sx; W writes the real w plane
+// (and Sx when A.Sx is set).  All three store dSx when A.write_dSx.
+enum { STFT2_EPI_SSQ = 0, STFT2_EPI_SSQ_TX = 1, STFT2_EPI_W = 2 };
+
+// |D| must exceed this fraction of |V^g|^2 for the second-order estimate to be used: where
+// the time derivative of the reassigned time nearly vanishes, q is an unstable ratio
+#define SSQB_SSQ2_EPS 1e-3
+
+// Second-order reassigned frequency w2 (float64), Oberlin, Meignen & Perrier (IEEE TSP 2015):
+//   om1 = eta - V^g' / (2 pi i V^g)
+//   D   = V^{tau g} V^g' - V^{tau g'} V^g
+//   q   = (V^g'' V^g - (V^g')^2) / (2 pi i D)
+//   om2 = om1 - q V^{tau g} / V^g
+// w2 = |Re om2| where |D| > eps |V^g|^2 and Re om2 is finite, else w1 (the first-order w).
+template <typename T>
+__device__ __forceinline__ double ssq2_w(double eta, cx<T> S, cx<T> dS, cx<T> S2, cx<T> St,
+                                         cx<T> Std, double w1) {
+  const double sx = S.x, sy = S.y, dx = dS.x, dy = dS.y;
+  const double ss = sx * sx + sy * sy;
+  // r = dS / S;  Re om1 = eta - Im(r) / (2 pi)
+  const double ry = (dy * sx - dx * sy) / ss;
+  const double re1 = eta - ry / SSQB_TWO_PI;
+  // D = St dS - Std S
+  const double Dx = ((double)St.x * dx - (double)St.y * dy) - ((double)Std.x * sx - (double)Std.y * sy);
+  const double Dy = ((double)St.x * dy + (double)St.y * dx) - ((double)Std.x * sy + (double)Std.y * sx);
+  const double DD = Dx * Dx + Dy * Dy;
+  if (!(DD > SSQB_SSQ2_EPS * SSQB_SSQ2_EPS * ss * ss)) return w1;
+  // num = S2 S - dS^2;  u = num / D;  q = -i u / (2 pi)
+  const double nx = ((double)S2.x * sx - (double)S2.y * sy) - (dx * dx - dy * dy);
+  const double ny = ((double)S2.x * sy + (double)S2.y * sx) - 2.0 * dx * dy;
+  const double ux = (nx * Dx + ny * Dy) / DD, uy = (ny * Dx - nx * Dy) / DD;
+  const double qx = uy / SSQB_TWO_PI, qy = -ux / SSQB_TWO_PI;
+  // v = St / S;  Re om2 = Re om1 - Re(q v)
+  const double vx = ((double)St.x * sx + (double)St.y * sy) / ss;
+  const double vy = ((double)St.y * sx - (double)St.x * sy) / ss;
+  const double re2 = re1 - (qx * vx - qy * vy);
+  return isfinite(re2) ? fabs(re2) : w1;
+}
+
+// spectra of frame `frame` at bin k from the three packed transforms -> outputs
+template <typename T, int EPI>
+__device__ __forceinline__ void stft2_emit(const Stft2Args<T>& P, int b, int k, long long frame,
+                                           cx<T> C1k, cx<T> C1mk, cx<T> C2k, cx<T> C2mk, cx<T> S2) {
+  const StftArgs<T>& A = P.A;
+  const T h = (T)0.5;
+  const cx<T> S   = mkc<T>((C1k.x + C1mk.x) * h, (C1k.y - C1mk.y) * h);
+  const cx<T> dS  = mkc<T>((C1k.y + C1mk.y) * h * A.inv_kappa, (C1mk.x - C1k.x) * h * A.inv_kappa);
+  const cx<T> St  = mkc<T>((C2k.x + C2mk.x) * h, (C2k.y - C2mk.y) * h);
+  const cx<T> Std = mkc<T>((C2k.y + C2mk.y) * h * P.inv_kappa2, (C2mk.x - C2k.x) * h * P.inv_kappa2);
+  const int nrows = A.n_fft / 2 + 1;
+  const long long o = ((long long)b * nrows + k) * A.n_hops + frame;
+  if (EPI == STFT2_EPI_SSQ || (EPI == STFT2_EPI_W && A.Sx)) A.Sx[o] = S;
+  if (A.write_dSx) A.dSx[o] = dS;
+  if (EPI == STFT2_EPI_W) {
+    double w = __longlong_as_double(0x7ff0000000000000ll);          // inf: below gamma
+    if (!is_below_exact(S.x, S.y, P.gamma_t)) {
+      const double w1 = fabs((double)A.Sfs[k] - phase_ratio_exact<T>(dS.x, dS.y, S.x, S.y));
+      w = ssq2_w<T>((double)A.Sfs[k], S, dS, S2, St, Std, w1);
+    }
+    P.w[o] = (T)w;
+    return;
+  }
+  if (is_active_exact(S.x, S.y, A.grid.gamma)) {
+    const double w1 = fabs((double)A.Sfs[k] - phase_ratio_exact<T>(dS.x, dS.y, S.x, S.y));
+    const double w = ssq2_w<T>((double)A.Sfs[k], S, dS, S2, St, Std, w1);
+    const int kk = bin_from_w_exact(w, A.grid);
+    const T cc = (T)A.cst[k];
+    atomic_add_cx<T>(&A.Tx[((long long)b * nrows + kk) * A.n_hops + frame], S.x * cc, S.y * cc);
+  }
+}
+
+// frames per CTA of the power-of-two kernel: three transforms per frame, and at least 8 NT
+// elements per transform batch so every Stockham stage divides over the threads
+template <typename T, int LOG_M> struct Stft2Tile {
+  static constexpr int M = 1 << LOG_M;
+  static constexpr int F = (Tile<T>::ELEMS / 2) / M > 0 ? (Tile<T>::ELEMS / 2) / M : 1;
+  static constexpr int R = 3 * F;
+  static constexpr size_t SMEM = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);
+};
+
+template <typename T, int LOG_M, int EPI>
+__global__ void __launch_bounds__(Tile<T>::NT)
+stft2_pow2_kernel(const Stft2Args<T> P) {
+  constexpr int NT = Tile<T>::NT;
+  constexpr int M = 1 << LOG_M;
+  constexpr int F = Stft2Tile<T, LOG_M>::F;
+  constexpr int R = Stft2Tile<T, LOG_M>::R;
+  constexpr int STRIDE = R + 1;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  cx<T>* s = reinterpret_cast<cx<T>*>(smem_raw);          // [M][STRIDE]: c1 of F frames, c2, c3
+  cx<T>* tw = s + (size_t)M * STRIDE;                     // [M]
+  const StftArgs<T>& A = P.A;
+  const int tid = threadIdx.x;
+  const long long total_frames = (long long)A.B * A.n_hops;
+  const long long f0 = (long long)blockIdx.x * F;
+
+  for (int m = tid; m < M; m += NT) tw[m] = A.tw[m];
+#pragma unroll 1
+  for (int lin = tid; lin < M * F; lin += NT) {
+    const int r = lin % F, l = lin / F;
+    const long long fr = f0 + r;
+    T v = (T)0;
+    if (fr < total_frames) {
+      const int b = (int)(fr / A.n_hops);
+      const long long i = fr - (long long)b * A.n_hops;
+      const long long src = pad_src_index(frame_src(l, i, A.hop, M, A.modulated), A.n1, A.N, A.padtype);
+      v = (src >= 0) ? A.x[(long long)b * A.N + src] : (T)0;
+    }
+    // conjugated inputs: the forward DFT from the inverse engine
+    s[l * STRIDE + r]         = mkc<T>(v * A.win[l], -(v * A.dwin[l]) * A.kappa);
+    s[l * STRIDE + F + r]     = mkc<T>(v * P.twin[l], -(v * P.tdwin[l]) * P.kappa2);
+    s[l * STRIDE + 2 * F + r] = mkc<T>(v * P.ddwin[l], (T)0);
+  }
+  __syncthreads();
+  block_ifft<T, LOG_M, R, NT, STRIDE>(s, tw);
+#pragma unroll 1
+  for (int lin = tid; lin < (M / 2 + 1) * F; lin += NT) {
+    const int r = lin % F, k = lin / F;
+    const long long fr = f0 + r;
+    if (fr >= total_frames) continue;
+    const int b = (int)(fr / A.n_hops);
+    const long long i = fr - (long long)b * A.n_hops;
+    const int mk = (M - k) & (M - 1);
+    stft2_emit<T, EPI>(P, b, k, i,
+                       cconj<T>(s[k * STRIDE + r]), cconj<T>(s[mk * STRIDE + r]),
+                       cconj<T>(s[k * STRIDE + F + r]), cconj<T>(s[mk * STRIDE + F + r]),
+                       cconj<T>(s[k * STRIDE + 2 * F + r]));
+  }
+}
+
+// any other n_fft (and float64 at 4096): c[3 fl + j][l] = packed sequence j of frame f0 + fl
+template <typename T>
+__global__ void __launch_bounds__(256)
+stft2_frames_kernel(const Stft2Args<T> P, cx<T>* __restrict__ c, long long f0, long long nf) {
+  const StftArgs<T>& A = P.A;
+  const int M = A.n_fft;
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= nf * M) return;
+  const long long fl = idx / M; const int l = (int)(idx - fl * M);
+  const long long fr = f0 + fl;
+  const int b = (int)(fr / A.n_hops);
+  const long long i = fr - (long long)b * A.n_hops;
+  const long long src = pad_src_index(frame_src(l, i, A.hop, M, A.modulated), A.n1, A.N, A.padtype);
+  const T v = (src >= 0) ? A.x[(long long)b * A.N + src] : (T)0;
+  cx<T>* cf = c + 3 * fl * M;
+  cf[l]         = mkc<T>(v * A.win[l], (v * A.dwin[l]) * A.kappa);
+  cf[M + l]     = mkc<T>(v * P.twin[l], (v * P.tdwin[l]) * P.kappa2);
+  cf[2 * M + l] = mkc<T>(v * P.ddwin[l], (T)0);
+}
+template <typename T, int EPI>
+__global__ void __launch_bounds__(256)
+stft2_emit_kernel(const Stft2Args<T> P, const cx<T>* __restrict__ C, long long f0, long long nf) {
+  const int M = P.A.n_fft, nrows = M / 2 + 1;
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= nf * nrows) return;
+  const int k = (int)(idx / nf); const long long fl = idx - (long long)k * nf;   // frames fastest
+  const long long fr = f0 + fl;
+  const int b = (int)(fr / P.A.n_hops);
+  const long long i = fr - (long long)b * P.A.n_hops;
+  const cx<T>* Cf = C + 3 * fl * M;
+  const int mk = k ? M - k : 0;
+  stft2_emit<T, EPI>(P, b, k, i, Cf[k], Cf[mk], Cf[M + k], Cf[M + mk], Cf[2 * M + k]);
+}
+
 }  // namespace ssqb

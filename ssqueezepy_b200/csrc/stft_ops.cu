@@ -374,4 +374,132 @@ int run_istft_backward(const ssqb_istft_desc* d, const void* gx, long long B, vo
                               : istft_bwd_t<double>(d, gx, B, gSx, st);
 }
 
+// ---- second-order ssq_stft -------------------------------------------------------------------
+// Power-of-two n_fft whose three transforms per frame fit one CTA's shared memory: one launch of
+// stft2_pow2_kernel (float32 up to 4096, float64 up to 2048).  Every other n_fft: frames -> one
+// batched Gfft of 3 transforms per frame -> emit, in chunks that keep each buffer at ~128 MB.
+static constexpr size_t kMaxBlockSmem = 227u << 10;    // sm_90 opt-in limit per block
+
+template <typename T, int L, int EPI>
+static int launch_stft2_tile(const Stft2Args<T>& P, cudaStream_t st) {
+  using TL = Stft2Tile<T, L>;
+  if constexpr (TL::SMEM > kMaxBlockSmem) {
+    return set_error(SSQB_E_UNSUPP, "n_fft = 2^%d does not fit one CTA", L);
+  } else {
+    const long long total = (long long)P.A.B * P.A.n_hops;
+    auto kern = stft2_pow2_kernel<T, L, EPI>;
+    static bool attr_done = false;
+    if (!attr_done) {
+      SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TL::SMEM));
+      attr_done = true;
+    }
+    kern<<<(unsigned)((total + TL::F - 1) / TL::F), Tile<T>::NT, TL::SMEM, st>>>(P);
+    SSQB_LAUNCH_CHECK();
+    return 0;
+  }
+}
+
+template <typename T, int L = 1>
+static bool stft2_pow2_fits(int logm) {
+  if constexpr (L > 12) return false;
+  else return logm == L ? Stft2Tile<T, L>::SMEM <= kMaxBlockSmem : stft2_pow2_fits<T, L + 1>(logm);
+}
+
+template <typename T, int EPI, int L = 1>
+static int launch_stft2_pow2(const Stft2Args<T>& P, int logm, cudaStream_t st) {
+  if constexpr (L > 12) return set_error(SSQB_E_ARG, "n_fft is not a power of two <= 4096");
+  else return logm == L ? launch_stft2_tile<T, L, EPI>(P, st) : launch_stft2_pow2<T, EPI, L + 1>(P, logm, st);
+}
+
+template <typename T, int EPI>
+static int launch_stft2_generic(const Stft2Args<T>& P, cudaStream_t st) {
+  int dev = 0; SSQB_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lk(g_gen_mu);            // buffers shared with the first order
+  auto& slot = gen_cache<T>()[{dev, P.A.n_fft}];
+  if (!slot) {
+    slot.reset(new StftGeneric<T>());
+    int rc = slot->fft.init(P.A.n_fft);
+    if (rc) { slot.reset(); return rc; }
+  }
+  StftGeneric<T>& G = *slot;
+  const long long total = (long long)P.A.B * P.A.n_hops, M = P.A.n_fft, nrows = M / 2 + 1;
+  long long chunk = ((128ll << 20) / (long long)sizeof(cx<T>)) / (3 * M); if (chunk < 1) chunk = 1;
+  if (chunk > total) chunk = total;
+  SSQB_CUDA(G.c.ensure((size_t)chunk * 3 * (size_t)M)); SSQB_CUDA(G.C.ensure((size_t)chunk * 3 * (size_t)M));
+  for (long long f0 = 0; f0 < total; f0 += chunk) {
+    const long long nf = total - f0 < chunk ? total - f0 : chunk;
+    stft2_frames_kernel<T><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(P, G.c.p, f0, nf);
+    SSQB_LAUNCH_CHECK();
+    int rc = G.fft.exec(G.c.p, G.C.p, 3 * nf, -1, (T)1, st); if (rc) return rc;
+    stft2_emit_kernel<T, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(P, G.C.p, f0, nf);
+    SSQB_LAUNCH_CHECK();
+  }
+  SSQB_CUDA(cudaStreamSynchronize(st));                // buffers are shared by later callers
+  return 0;
+}
+
+template <typename T, int EPI>
+static int launch_stft2(const Stft2Args<T>& P, cudaStream_t st) {
+  const int logm = ilog2_exact(P.A.n_fft);
+  return stft2_pow2_fits<T>(logm) ? launch_stft2_pow2<T, EPI>(P, logm, st)
+                                  : launch_stft2_generic<T, EPI>(P, st);
+}
+
+template <typename T>
+static int stft2_t(const ssqb_stft_desc* d, const ssqb_stft2_tables* t2, const ssqb_reassign_desc* r,
+                   const void* x, long long B, void* Sx, void* Tx, void* dSx, void* w,
+                   cudaStream_t st) {
+  const int M = d->n_fft, nrows = M / 2 + 1;
+  Stft2Args<T> P;
+  memset(&P, 0, sizeof(P));
+  StftArgs<T>& A = P.A;
+  A.N = d->N; A.n_fft = M; A.hop = d->hop; A.n1 = d->n1; A.padtype = d->padtype;
+  A.modulated = d->modulated; A.B = (int)B;
+  A.n_hops = (d->N - 1) / d->hop + 1;
+  A.x = (const T*)x; A.Sx = (cx<T>*)Sx; A.dSx = (cx<T>*)dSx; A.Tx = (cx<T>*)Tx;
+  A.write_dSx = dSx ? 1 : 0;
+  P.w = (T*)w;
+  P.gamma_t = (T)r->gamma;
+  const T* win = (const T*)d->win_host; const T* dwin = (const T*)d->dwin_host;
+  const T* twin = (const T*)t2->twin_host; const T* tdwin = (const T*)t2->tdwin_host;
+  const double kap = pack_kappa(win, dwin, M), kap2 = pack_kappa(twin, tdwin, M);
+  A.kappa = (T)kap; A.inv_kappa = (T)(1.0 / kap);
+  P.kappa2 = (T)kap2; P.inv_kappa2 = (T)(1.0 / kap2);
+  BlobBuilder bb;
+  const std::vector<cx<T>>& tw = roots<T>(M);
+  const size_t o_tw = bb.put(tw.data(), sizeof(cx<T>) * M);
+  const size_t o_cst = bb.put(r->cst_host, sizeof(double) * nrows);
+  const size_t o_win = bb.put(win, sizeof(T) * M);
+  const size_t o_dwin = bb.put(dwin, sizeof(T) * M);
+  const size_t o_sfs = bb.put(d->Sfs_host, sizeof(T) * nrows);
+  const size_t o_ddwin = bb.put(t2->ddwin_host, sizeof(T) * M);
+  const size_t o_twin = bb.put(twin, sizeof(T) * M);
+  const size_t o_tdwin = bb.put(tdwin, sizeof(T) * M);
+  unsigned char* blob = nullptr;
+  int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
+  A.tw = (const cx<T>*)(blob + o_tw); A.cst = (const double*)(blob + o_cst);
+  A.win = (const T*)(blob + o_win); A.dwin = (const T*)(blob + o_dwin);
+  A.Sfs = (const T*)(blob + o_sfs);
+  P.ddwin = (const T*)(blob + o_ddwin);
+  P.twin = (const T*)(blob + o_twin); P.tdwin = (const T*)(blob + o_tdwin);
+  if (!Tx) return launch_stft2<T, STFT2_EPI_W>(P, st);
+  rc = fill_grid(r, nrows, &A.grid); if (rc) return rc;
+  A.grid.kind = 3;
+  SSQB_CUDA(cudaMemsetAsync(Tx, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(cx<T>), st));
+  return Sx ? launch_stft2<T, STFT2_EPI_SSQ>(P, st) : launch_stft2<T, STFT2_EPI_SSQ_TX>(P, st);
+}
+
+int run_stft2(const ssqb_stft_desc* d, const ssqb_stft2_tables* t2, const ssqb_reassign_desc* r,
+              const void* x, long long B, void* Sx, void* Tx, void* dSx, void* w, cudaStream_t st) {
+  if (!d || !t2 || !r || !x) return set_error(SSQB_E_ARG, "null pointer");
+  if (!d->win_host || !d->dwin_host || !d->Sfs_host || !r->cst_host || !t2->ddwin_host ||
+      !t2->twin_host || !t2->tdwin_host)
+    return set_error(SSQB_E_ARG, "null table");
+  if (!Tx == !w) return set_error(SSQB_E_ARG, "exactly one of Tx and w must be given");
+  if (!d->modulated) return set_error(SSQB_E_UNSUPP, "second-order ssq_stft needs modulated frames");
+  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
+  return d->dtype == SSQB_F32 ? stft2_t<float>(d, t2, r, x, B, Sx, Tx, dSx, w, st)
+                              : stft2_t<double>(d, t2, r, x, B, Sx, Tx, dSx, w, st);
+}
+
 }  // namespace ssqb
