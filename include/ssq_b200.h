@@ -271,7 +271,10 @@ int ssqb_invert_components(int dtype, const void* M_dev, int na, int64_t N,
  * data's real dtype); scales_host float64[na] = the values returned as ridge_f; eps = the dtype's
  * machine epsilon (:119).  Outputs on the device: idx_dev int64 [B][N][n_ridges];
  * f_dev, e_dev real dtype [B][N][n_ridges] or NULL.  The backward sweep is the reference's
- * serial kernel (:211-219; its prange variant races when two bins tie).                  */
+ * serial kernel (:211-219; its prange variant races when two bins tie).  na <= 2048 (float32)
+ * or 1505 (float64); more rows return SSQB_E_UNSUPP.  Non-finite values follow NumPy: a NaN in
+ * a column makes the column's max, hence all of its -log energy, NaN; the forward argmin of a
+ * column holding a NaN is its first NaN; the NaN then reaches every later column.           */
 int ssqb_extract_ridges(int dtype, const void* Tf_dev, int64_t B, int na, int64_t N,
                         const double* ls_host, const double* scales_host, double penalty,
                         double eps, int n_ridges, int bw, int64_t* idx_dev, void* f_dev,

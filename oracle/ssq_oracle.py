@@ -809,34 +809,48 @@ def issq_stft(Tx, window=None, cc=None, cw=None, n_fft=None, win_len=None):
 # ridge extraction                         ssqueezepy/ridge_extraction.py
 # ---------------------------------------------------------------------------
 def extract_ridges(Tf, scales, penalty=2., n_ridges=1, bw=15, transform='cwt',
-                   get_params=False):
+                   get_params=False, absq=None, log=None):
     """ridge_extraction.py:11-146 with the SERIAL backward kernel (:211-219); every
     array in the data's real dtype like the reference (:117-121).  O(N na^2): small
-    inputs only."""
+    inputs only.
+
+    `absq(Tf)` and `log(x)` replace the two primitives whose last bit depends on the
+    implementation, `np.abs(Tf) ** 2` and `np.log` in `-log(energy / max + eps)`.  Everything
+    else is a fixed sequence of separately rounded operations, so with another implementation's
+    `|z|` and `log` the restatement must agree with it bit for bit.  `log(scales)` stays
+    NumPy's in every case (callers take it on the host with NumPy)."""
     Tf = np.asarray(Tf)
     eps = EPS64 if Tf.dtype == np.complex128 else EPS32
     dtype = np.float64 if Tf.dtype == np.complex128 else np.float32
     scales, eps, penalty = [np.asarray(v, dtype=dtype) for v in (scales, eps, penalty)]
     scales_orig = scales.copy().reshape(-1)
-    ls = (np.log(scales) if transform == 'cwt' else scales).squeeze()
-    energy = np.abs(Tf) ** 2
+    with np.errstate(divide='ignore', invalid='ignore'):
+        ls = (np.log(scales) if transform == 'cwt' else scales).reshape(-1)
+        P = penalty * np.subtract.outer(ls, ls) ** 2                # :91
+    with np.errstate(over='ignore'):
+        energy = np.abs(Tf) ** 2 if absq is None else np.asarray(absq(Tf), dtype=dtype)
+    log = np.log if log is None else log
     na, N = Tf.shape
-    P = (penalty * np.subtract.outer(ls, ls) ** 2).squeeze()       # :91
     idxs = np.zeros((N, n_ridges), dtype=int)
     rf = np.zeros((N, n_ridges), dtype=dtype)
     re = np.zeros((N, n_ridges), dtype=dtype)
+    tmp = np.empty((na, na), dtype=dtype)
     for i in range(n_ridges):
         with np.errstate(divide='ignore', invalid='ignore'):
-            e = -np.log(energy / energy.max(axis=0) + eps)          # :135-136
-        pen = e.copy()
-        for t in range(1, N):                                       # :178-182
-            pen[:, t] += (pen[:, t - 1][None, :] + P).min(axis=1)
-        r = np.argmin(pen, axis=0)                                  # :160-162
-        for t in range(N - 2, -1, -1):                              # :211-219
-            val = pen[r[t + 1], t + 1] - e[r[t + 1], t + 1]
-            hit = np.flatnonzero(np.abs(val - (pen[:, t] + P[r[t + 1], :])) < eps)
-            if hit.size:
-                r[t] = hit[-1]
+            e = -np.asarray(log(energy / energy.max(axis=0) + eps), dtype=dtype)   # :135-136
+        # time-major copies: the same operations as on [na, N], on contiguous rows
+        eT = np.ascontiguousarray(e.T)
+        pen = eT.copy()
+        with np.errstate(invalid='ignore'):
+            for t in range(1, N):                                   # :178-182
+                np.add(pen[t - 1][None, :], P, out=tmp)
+                pen[t] += tmp.min(axis=1)
+            r = np.argmin(pen, axis=1)                              # :160-162
+            for t in range(N - 2, -1, -1):                          # :211-219
+                val = pen[t + 1, r[t + 1]] - eT[t + 1, r[t + 1]]
+                hit = np.flatnonzero(np.abs(val - (pen[t] + P[r[t + 1], :])) < eps)
+                if hit.size:
+                    r[t] = hit[-1]
         idxs[:, i] = r
         rf[:, i] = scales_orig[r]
         re[:, i] = energy[r, np.arange(N)]

@@ -47,14 +47,15 @@ ridge_energy_kernel(const cx<T>* __restrict__ Tf, T* __restrict__ energy, long l
   const T a = t_absc<T>(v.x, v.y);
   energy[i] = mul_rn(a, a);
 }
-// eT[t][f] = -log(energy[f][t] / max_f energy[., t] + eps); one thread per column
+// eT[t][f] = -log(energy[f][t] / max_f energy[., t] + eps); one thread per column.  The max
+// propagates NaN like np.max, so a NaN anywhere in a column makes its whole `e` NaN.
 template <typename T>
 __global__ void __launch_bounds__(128)
 ridge_neglog_kernel(const T* __restrict__ energy, T* __restrict__ eT, int na, long long N, T eps) {
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= N) return;
   T mx = energy[t];
-  for (int f = 1; f < na; ++f) { const T v = energy[(long long)f * N + t]; mx = v > mx ? v : mx; }
+  for (int f = 1; f < na; ++f) { const T v = energy[(long long)f * N + t]; mx = (v > mx || v != v) ? v : mx; }
   for (int f = 0; f < na; ++f) {
     const T q = energy[(long long)f * N + t] / mx;                       // IEEE division
     eT[t * na + f] = -t_logr<T>(add_rn(q, eps));
@@ -151,7 +152,13 @@ ridge_forward_kernel(const T* __restrict__ eT, T* __restrict__ penT, long long* 
 }
 
 // ridge_fw[t] = first argmin_f penT[t][f] (ridge_extraction.py:160-162): a pure function of the
-// penalised plane, so it runs after the sweep, one warp per time step
+// penalised plane, so it runs after the sweep, one warp per time step.  As np.argmin, a NaN
+// ranks below every number, so a column holding a NaN gives its first NaN.
+template <typename T>
+__device__ __forceinline__ bool argmin_before(T v, int f, T bv, int bi) {
+  if (bv != bv) return v != v && f < bi;
+  return v != v || v < bv || (v == bv && f < bi);
+}
 template <typename T>
 __global__ void __launch_bounds__(256)
 ridge_argmin_kernel(const T* __restrict__ penT, long long* __restrict__ ridge, int na, long long total) {
@@ -159,13 +166,13 @@ ridge_argmin_kernel(const T* __restrict__ penT, long long* __restrict__ ridge, i
   const int lane = threadIdx.x & 31;
   if (t >= total) return;
   const T* row = penT + t * na;
-  T bv = t_inf_<T>(); int bi = 0x7fffffff;
-  for (int f = lane; f < na; f += 32) { const T v = row[f]; if (v < bv || (v == bv && f < bi)) { bv = v; bi = f; } }
+  T bv = t_inf_<T>(); int bi = 0x7fffffff;                   // na >= 1: lane 0 always takes f = 0
+  for (int f = lane; f < na; f += 32) { const T v = row[f]; if (argmin_before(v, f, bv, bi)) { bv = v; bi = f; } }
   for (int o = 16; o; o >>= 1) {
     const T ov = __shfl_down_sync(0xffffffffu, bv, o); const int oi = __shfl_down_sync(0xffffffffu, bi, o);
-    if (ov < bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+    if (argmin_before(ov, oi, bv, bi)) { bv = ov; bi = oi; }
   }
-  if (lane == 0) ridge[t] = (bi == 0x7fffffff) ? 0 : bi;       // all-NaN column: numpy's argmin gives 0
+  if (lane == 0) ridge[t] = bi;
 }
 
 // backward sweep, one CTA per plane; rows of penT and eT prefetched RING_DEPTH steps ahead

@@ -26,10 +26,18 @@ def extract_ridges(Tf, scales, penalty=2., n_ridges=1, bw=15, transform='cwt',
     `get_params=True` also `ridge_f` (the `scales` along the ridges) and `ridge_e` (the
     energies along them).  NumPy in -> NumPy out, CUDA tensor in -> CUDA tensors out.
 
+    At most 2048 rows in float32 and 1505 in float64 (the sweeps keep rows in shared
+    memory); more raise `RuntimeError`.  NaN and inf follow NumPy: a NaN in a column makes
+    the column's max, hence all of its normalised log energy, NaN (so does an energy that
+    overflows to inf, in its own row: inf / inf); the forward argmin of a column holding a NaN
+    is its first NaN, and the NaN reaches every later column through the penalised minimum.
+
     `parallel` is accepted for signature compatibility; the backward sweep always follows
     the reference's serial kernel (its `prange` variant races when two bins tie)."""
     if transform not in ('cwt', 'stft'):
         raise ValueError("`transform` must be one of: cwt, stft (got %s)" % transform)
+    if int(n_ridges) < 1 or int(bw) < 0:
+        raise ValueError("need n_ridges >= 1 and bw >= 0 (got %s, %s)" % (n_ridges, bw))
     lib = Bk.require_cuda()
     was_np = not Bk.is_tensor(Tf)
     dtype = Bk.dtype_of_complex(Tf)

@@ -24,9 +24,12 @@ def test_oracle_ridges_equal_reference(tag, fix, plane, sc, kw):
 @pytest.mark.gpu
 @pytest.mark.parametrize('tag,fix,plane,sc,kw', CASES)
 def test_device_ridges_vs_reference(tag, fix, plane, sc, kw):
-    """The two sweeps are integer work on float planes: indices must equal the reference's
-    wherever `-log(energy / max + eps)` (NumPy's SIMD log on the host, CUDA's logf on the
-    device: last-bit differences) does not decide a tie; in float64 they are identical."""
+    """Indices must equal the reference's wherever a last-bit difference of `energy` or of
+    `-log(energy / max + eps)` does not decide a near-tie.  Two primitives round differently
+    in float32: NumPy's SIMD `log` against CUDA's `logf`, and NumPy's complex64 `abs` (not
+    correctly rounded) against the device's correctly rounded hypot.  In float64 the indices
+    are identical.  With the device's own `|z|` and `log` the oracle agrees with the device
+    bit for bit (tests/test_gpu_ridges.py, these planes included)."""
     import torch
     if not torch.cuda.is_available():
         pytest.skip("needs a CUDA device")
