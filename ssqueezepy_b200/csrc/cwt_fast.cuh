@@ -507,10 +507,11 @@ cwt_rows_tx_kernel(const FastArgs<T> P) {
 // Z from the band tables (no transcendental work here), zero outside the band.
 // Stored pass-2-tile-major [arr][t2/R2][i1][t2%R2] through a padded shared-memory
 // transpose so that both the xh reads and the scratch writes are 128-byte runs.
-template <typename T, int LOG_M, int NARR, int LOGE1, int NT>
-__global__ void __launch_bounds__(NT, (NT * 2 <= 1024 && LOGE1 <= 12 && sizeof(T) == 4) ? 2 : 1)
+template <typename T, int LOG_M, int NARR>
+__global__ void __launch_bounds__(Tile<T>::NT, 1)
 cwt_pass1f_kernel(const FastArgs<T> P) {
-  constexpr int ELEMS = 1 << LOGE1;
+  constexpr int ELEMS = Tile<T>::ELEMS;
+  constexpr int NT = Tile<T>::NT;
   constexpr int M = 1 << LOG_M;                      // I2
   constexpr int R1 = ELEMS / M;
   constexpr int STRIDE = R1 + 1;
@@ -591,7 +592,7 @@ cwt_pass1f_kernel(const FastArgs<T> P) {
 }
 
 // ---- (3b) pass 1, 512-point transforms, both arrays as one 16-byte element -----------------
-// Same result as cwt_pass1f_kernel<T, 9, 2, ..> (n = 512 * 512 .. the C2 / C4 geometry), laid
+// Same result as cwt_pass1f_kernel<T, 9, 2> (n = 512 * 512 .. the C2 / C4 geometry), laid
 // out for the machine: a CTA = one row x R1 = 8 consecutive i1; W and dW travel together as one
 // V4 element (shared twiddles and addresses, 16-byte shared-memory exchanges, a quarter-warp =
 // one 128-byte row -> conflict free for any index stride), the first and the last of the three

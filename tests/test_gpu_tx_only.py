@@ -202,39 +202,6 @@ def test_route_tx_only_f64(S, route):
             _check_routes(rows, env, B * plan.na)
 
 
-_KNOB_SCRIPT = r"""
-import sys, numpy as np, torch
-sys.path.insert(0, sys.argv[1])
-import ssqueezepy_b200 as S
-from oracle import ssq_oracle as O
-dtype = sys.argv[2]
-N, B = 160_000, 2
-wav = S.Wavelet(('gmw', {'beta': 12, 'gamma': 3, 'dtype': dtype}))
-scales = O.bench_scales(O.OracleWavelet('gmw', dtype, beta=12, gamma=3), N, 150)
-x = torch.as_tensor(np.stack([O.chirp(N, b, dtype) for b in range(B)]), device='cuda')
-T0, W0, *_ = S.ssq_cwt(x, wav, scales=scales)
-T1, W1, *_ = S.ssq_cwt(x, wav, scales=scales, get_Wx=False)
-assert W1 is None and torch.equal(T1 != 0, T0 != 0)
-err = float(torch.linalg.vector_norm(T1 - T0) / torch.linalg.vector_norm(T0))
-assert err < (2e-6 if dtype == 'float32' else 1e-14), err
-print('OK', err)
-"""
-
-
-@pytest.mark.parametrize('knob,dtype', [('SSQB_INTERP_PPK=4', 'float32'), ('SSQB_INTERP_PPK=8', 'float32'),
-                                        ('SSQB_INTERP_PPK64=2', 'float64'), ('SSQB_F64_REGWIN=0', 'float64')])
-def test_interp_variants_tx_only(S, knob, dtype):
-    """the interpolation settings are read once per process: each runs in a process of its own"""
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    k, v = knob.split('=')
-    env = dict(os.environ, **{k: v})
-    r = subprocess.run([sys.executable, '-c', _KNOB_SCRIPT, root, dtype], env=env, cwd=root,
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and 'OK' in r.stdout, r.stdout + r.stderr
-
-
 def test_public_api_contract(S):
     """the returned tuple keeps its shape; Wx is None; with get_dWx, dWx is the stored one"""
     import torch
