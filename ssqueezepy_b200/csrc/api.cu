@@ -5,6 +5,53 @@
 namespace ssqb {
 thread_local std::string g_last_error;
 std::atomic<long long> g_launch_count{0};
+
+static std::mutex g_dev_mu;         // guards the three per-device records below
+
+cudaError_t opt_in_smem_raw(const void* kern, size_t bytes) {
+  static std::map<std::pair<const void*, int>, size_t> set;
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  std::lock_guard<std::mutex> lk(g_dev_mu);
+  size_t& have = set[{kern, dev}];
+  if (bytes <= have) return cudaSuccess;
+  e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  if (e == cudaSuccess) have = bytes;
+  return e;
+}
+
+cudaError_t device_facts(DeviceFacts* f) {
+  static std::map<int, DeviceFacts> facts;
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  std::lock_guard<std::mutex> lk(g_dev_mu);
+  auto it = facts.find(dev);
+  if (it == facts.end()) {
+    DeviceFacts g;
+    if ((e = cudaDeviceGetAttribute(&g.sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return e;
+    if ((e = cudaDeviceGetStreamPriorityRange(&g.prio_least, &g.prio_high)) != cudaSuccess) return e;
+    it = facts.emplace(dev, g).first;
+  }
+  *f = it->second;
+  return cudaSuccess;
+}
+
+int blocks_per_sm_raw(const void* kern, int threads, size_t smem) {
+  static std::map<std::pair<const void*, int>, int> per_sm;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  std::lock_guard<std::mutex> lk(g_dev_mu);
+  auto it = per_sm.find({kern, dev});
+  if (it == per_sm.end()) {
+    int per = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kern, threads, smem) != cudaSuccess || per < 1)
+      per = 1;
+    it = per_sm.emplace(std::make_pair(kern, dev), per).first;
+  }
+  return it->second;
+}
 }
 using namespace ssqb;
 

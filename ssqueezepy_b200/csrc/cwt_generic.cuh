@@ -69,11 +69,7 @@ struct Gfft {
     A.R = R;
     size_t smem = ((size_t)2 * S.n * R + S.n) * sizeof(cx<T>);
     auto kern = gfft_smem_kernel<T>;
-    static size_t attr = 0;
-    if (smem > attr) {
-      SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      attr = smem;
-    }
+    SSQB_CUDA(opt_in_smem(kern, smem));
     kern<<<(unsigned)((count + R - 1) / R), 256, smem, st>>>(A);
     SSQB_LAUNCH_CHECK();
     return 0;
@@ -164,6 +160,115 @@ gen_unpad_kernel(const cx<T>* __restrict__ src, cx<T>* __restrict__ dst, long lo
   const T m = out_mul ? out_mul[(r0 + rl) % na] : (T)1;
   dst[(r0 + rl) * Nout + j] = cscale<T>(src[rl * n + off + j], m);
 }
+
+// ---- pieces shared by the power-of-two plan (cwt_impl.cuh) and the generic-length plan ---------
+// descriptor checks that hold at every transform length
+inline int check_cwt_desc(const ssqb_cwt_desc& d) {
+  if (d.N < 1 || d.n1 < 0 || d.n1 + d.N > d.n_up)
+    return set_error(SSQB_E_ARG, "bad padding geometry N=%lld n1=%lld n_up=%lld",
+                     (long long)d.N, (long long)d.n1, (long long)d.n_up);
+  if (d.na < 1) return set_error(SSQB_E_ARG, "na must be >= 1");
+  if (d.wavelet < 0 || d.wavelet > 2) return set_error(SSQB_E_ARG, "bad wavelet kind");
+  if (d.wavelet == SSQB_WAV_TABLE && !d.psih_table_dev)
+    return set_error(SSQB_E_ARG, "SSQB_WAV_TABLE needs psih_table_dev");
+  return 0;
+}
+
+// the fields of CwtArgs every plan fills alike: geometry, scales and the wavelet's constants
+template <typename T>
+void cwt_common_args(const ssqb_cwt_desc& d, const T* scales, CwtArgs<T>& A) {
+  memset(&A, 0, sizeof(A));
+  A.N = d.N; A.n_up = d.n_up; A.n1 = d.n1; A.padtype = d.padtype; A.na = d.na;
+  A.scales = scales; A.psih_table = (const T*)d.psih_table_dev; A.wavelet = d.wavelet;
+  if (d.wavelet == SSQB_WAV_MORLET) {
+    // constants cast to dtype exactly as wavelets.py:510-516
+    double mu = d.wparams[0];
+    double cs = pow(1 + exp(-mu * mu) - 2 * exp(-0.75 * mu * mu), -0.5);
+    A.wp[0] = (T)mu; A.wp[1] = (T)exp(-0.5 * mu * mu); A.wp[2] = (T)-0.5;
+    A.wp[3] = (T)(sqrt(2.0) * cs * pow(M_PI, 0.25));
+  } else if (d.wavelet == SSQB_WAV_GMW_L1) {
+    // _gmw.py:191-198: gamma, beta, wc, wcl cast to dtype; k0 = -beta*wcl + wc**gamma
+    double gam = d.wparams[0], bet = d.wparams[1];
+    double wc = exp((1.0 / gam) * (log(bet) - log(gam)));
+    T gT = (T)gam, bT = (T)bet, wcT = (T)wc, wclT = (T)log(wc);
+    T wcg = (T)pow((double)wcT, (double)gT);         // wc**gamma rounded to dtype
+    A.wp[0] = gT; A.wp[1] = bT; A.wp[2] = (T)(-(bT * wclT)) + wcg;
+  }
+  A.dt = (T)d.dt;
+}
+
+// per-scale output factors in dtype on the device, nullptr when there are none.  The copy is
+// ordered on the caller's stream and waited for before the host vector dies.
+template <typename T>
+int upload_out_mul(const double* host, int na, DevBuf<T>& buf, const T** out, cudaStream_t st) {
+  *out = nullptr;
+  if (!host) return 0;
+  std::vector<T> m((size_t)na);
+  for (int a = 0; a < na; ++a) m[a] = (T)host[a];
+  SSQB_CUDA(buf.ensure((size_t)na));
+  SSQB_CUDA(cudaMemcpyAsync(buf.p, m.data(), m.size() * sizeof(T), cudaMemcpyHostToDevice, st));
+  SSQB_CUDA(cudaStreamSynchronize(st));
+  *out = buf.p;
+  return 0;
+}
+
+// Host buffers in, host buffers out (pinned memory recommended), for either plan.  The batch is
+// cut into chunks of two signals that ping-pong between two device staging slots: chunk c is
+// transformed on the caller's stream while the copy stream still drains the outputs of chunk
+// c-1 over PCIe, so the device holds two chunks of outputs, not the batch.
+template <typename T>
+struct HostStaging {
+  DevBuf<T> x_stage;
+  DevBuf<cx<T>> Wx_stage, dWx_stage, Tx_stage;
+  Stream copy_st;
+  Event ev_comp[2], ev_d2h[2];
+  int run(CwtPlanBase& plan, const ssqb_cwt_desc& d, const void* x, long long B, void* Wx,
+          void* dWx, void* Tx, bool ssq, const double* out_mul_host, bool rpadded, cudaStream_t st) {
+    if (B < 1) return set_error(SSQB_E_ARG, "B must be >= 1");
+    const long long CH = B < 2 ? B : 2;
+    const long long Nout = rpadded ? d.n_up : d.N;
+    const size_t nx = (size_t)CH * (size_t)d.N, nout = (size_t)CH * d.na * (size_t)Nout;
+    SSQB_CUDA(x_stage.ensure(2 * nx));
+    if (Wx) SSQB_CUDA(Wx_stage.ensure(2 * nout));
+    if (dWx) SSQB_CUDA(dWx_stage.ensure(2 * nout));
+    if (ssq) SSQB_CUDA(Tx_stage.ensure(2 * nout));
+    if (!copy_st) {
+      SSQB_CUDA(copy_st.create());
+      for (int i = 0; i < 2; ++i) { SSQB_CUDA(ev_comp[i].create()); SSQB_CUDA(ev_d2h[i].create()); }
+    }
+    const T* xh_ = (const T*)x;
+    cx<T>* Wh = (cx<T>*)Wx; cx<T>* dWh = (cx<T>*)dWx; cx<T>* Th = (cx<T>*)Tx;
+    int rc = 0, c = 0;
+    bool slot_busy[2] = {false, false};
+    for (long long b0 = 0; b0 < B; b0 += CH, ++c) {
+      const int sl = c & 1;
+      const long long nb = (B - b0 < CH) ? (B - b0) : CH;
+      const size_t cx_ = (size_t)nb * (size_t)d.N, co = (size_t)nb * d.na * (size_t)Nout;
+      if (slot_busy[sl]) SSQB_CUDA(cudaStreamWaitEvent(st, ev_d2h[sl], 0));   // slot drained
+      T* xs = x_stage.p + sl * nx;
+      cx<T>* Ws = Wx ? Wx_stage.p + sl * nout : nullptr;
+      cx<T>* dWs = dWx ? dWx_stage.p + sl * nout : nullptr;
+      cx<T>* Ts = ssq ? Tx_stage.p + sl * nout : nullptr;
+      SSQB_CUDA(cudaMemcpyAsync(xs, xh_ + (size_t)b0 * (size_t)d.N, cx_ * sizeof(T),
+                                cudaMemcpyHostToDevice, st));
+      rc = plan.exec(xs, nb, Ws, dWs, Ts, ssq, out_mul_host, rpadded, st);
+      if (rc) break;
+      SSQB_CUDA(cudaEventRecord(ev_comp[sl], st));
+      SSQB_CUDA(cudaStreamWaitEvent(copy_st, ev_comp[sl], 0));
+      const size_t ho = (size_t)b0 * d.na * (size_t)Nout;
+      if (Wx) SSQB_CUDA(cudaMemcpyAsync(Wh + ho, Ws, co * sizeof(cx<T>), cudaMemcpyDeviceToHost, copy_st));
+      if (dWx) SSQB_CUDA(cudaMemcpyAsync(dWh + ho, dWs, co * sizeof(cx<T>), cudaMemcpyDeviceToHost, copy_st));
+      if (ssq) SSQB_CUDA(cudaMemcpyAsync(Th + ho, Ts, co * sizeof(cx<T>), cudaMemcpyDeviceToHost, copy_st));
+      SSQB_CUDA(cudaEventRecord(ev_d2h[sl], copy_st));
+      slot_busy[sl] = true;
+    }
+    // the call returns with the results in the host buffers
+    cudaError_t e1 = cudaStreamSynchronize(copy_st), e2 = cudaStreamSynchronize(st);
+    if (rc) return rc;
+    SSQB_CUDA(e1); SSQB_CUDA(e2);
+    return 0;
+  }
+};
 
 // =============================================================================================
 // Adjoint of the CWT (backward pass of `cwt` for torch.autograd; the reference's GPU mode is
@@ -262,13 +367,7 @@ struct CwtAdjoint {
       ready = true;
     }
     const T* out_mul = nullptr;
-    if (out_mul_host) {
-      std::vector<T> m((size_t)d.na);
-      for (int a = 0; a < d.na; ++a) m[a] = (T)out_mul_host[a];
-      SSQB_CUDA(cudaStreamSynchronize(st));
-      SSQB_CUDA(mul_d.upload(m));
-      out_mul = mul_d.p;
-    }
+    int rc = upload_out_mul(out_mul_host, d.na, mul_d, &out_mul, st); if (rc) return rc;
     long long chunk = ((64ll << 20) / (long long)sizeof(cx<T>)) / n; if (chunk < 1) chunk = 1;
     if (chunk > d.na) chunk = d.na;
     SSQB_CUDA(Z.ensure((size_t)chunk * (size_t)n)); SSQB_CUDA(Zh.ensure((size_t)chunk * (size_t)n));
@@ -283,12 +382,12 @@ struct CwtAdjoint {
           const long long r0 = b * d.na + a0;
           adj_pad_kernel<T><<<(unsigned)(((long long)nr * n + 255) / 256), 256, 0, st>>>(G, Z.p, n, off, Nout, r0, nr, out_mul, d.na);
           SSQB_LAUNCH_CHECK();
-          int rc = fft.exec(Z.p, Zh.p, nr, -1, (T)1, st); if (rc) return rc;
+          rc = fft.exec(Z.p, Zh.p, nr, -1, (T)1, st); if (rc) return rc;
           adj_accum_kernel<T><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(A, Zh.p, acc.p + b * n, a0, nr, pass);
           SSQB_LAUNCH_CHECK();
         }
       }
-    int rc = fft.exec(acc.p, gp.p, B, +1, (T)(1.0 / (double)n), st); if (rc) return rc;
+    rc = fft.exec(acc.p, gp.p, B, +1, (T)(1.0 / (double)n), st); if (rc) return rc;
     adj_unpad_kernel<T><<<(unsigned)((B * d.N + 255) / 256), 256, 0, st>>>(gp.p, gx, d.N, n, d.n1, B);
     SSQB_LAUNCH_CHECK();
     if (n_groups > 0) {
@@ -309,34 +408,14 @@ struct GenericCwtPlan : public CwtPlanBase {
   DevBuf<double> cst_d;
   DevBuf<cx<T>> xp_d, xh_d, ZW, ZD, OW, OD, W_tmp, dW_tmp;
   ssqb_reassign_desc rd{}; std::vector<double> rd_cst; bool have_grid = false;
+  HostStaging<T> staging;
   int init(const ssqb_cwt_desc* desc) {
     d = *desc;
-    if (d.N < 1 || d.n1 < 0 || d.n1 + d.N > d.n_up) return set_error(SSQB_E_ARG, "bad padding geometry");
-    if (d.na < 1) return set_error(SSQB_E_ARG, "na must be >= 1");
-    if (d.wavelet == SSQB_WAV_TABLE && !d.psih_table_dev)
-      return set_error(SSQB_E_ARG, "SSQB_WAV_TABLE needs psih_table_dev");
+    int rc = check_cwt_desc(d); if (rc) return rc;
     std::vector<T> sc((size_t)d.na);
     for (int a = 0; a < d.na; ++a) sc[a] = (T)d.scales_host[a];
     SSQB_CUDA(scales_d.upload(sc));
     return fft.init(d.n_up);
-  }
-  void args(CwtArgs<T>& A) {
-    memset(&A, 0, sizeof(A));
-    A.N = d.N; A.n_up = d.n_up; A.n1 = d.n1; A.padtype = d.padtype; A.na = d.na;
-    A.scales = scales_d.p; A.psih_table = (const T*)d.psih_table_dev; A.wavelet = d.wavelet;
-    if (d.wavelet == SSQB_WAV_MORLET) {
-      double mu = d.wparams[0];
-      double cs = pow(1 + exp(-mu * mu) - 2 * exp(-0.75 * mu * mu), -0.5);
-      A.wp[0] = (T)mu; A.wp[1] = (T)exp(-0.5 * mu * mu); A.wp[2] = (T)-0.5;
-      A.wp[3] = (T)(sqrt(2.0) * cs * pow(M_PI, 0.25));
-    } else if (d.wavelet == SSQB_WAV_GMW_L1) {
-      double gam = d.wparams[0], bet = d.wparams[1];
-      double wc = exp((1.0 / gam) * (log(bet) - log(gam)));
-      T gT = (T)gam, bT = (T)bet, wcT = (T)wc, wclT = (T)log(wc);
-      T wcg = (T)pow((double)wcT, (double)gT);
-      A.wp[0] = gT; A.wp[1] = bT; A.wp[2] = (T)(-(bT * wclT)) + wcg;
-    }
-    A.dt = (T)d.dt;
   }
   int set_reassign(const ssqb_reassign_desc* r) override {
     rd = *r;
@@ -357,20 +436,14 @@ struct GenericCwtPlan : public CwtPlanBase {
     if (ssq && !Wx) { SSQB_CUDA(W_tmp.ensure((size_t)rows * (size_t)Nout)); Wx = W_tmp.p; }
     if (ssq && !dWx) { SSQB_CUDA(dW_tmp.ensure((size_t)rows * (size_t)Nout)); dWx = dW_tmp.p; }
     const T* out_mul = nullptr;
-    if (out_mul_host) {
-      std::vector<T> m((size_t)d.na);
-      for (int a = 0; a < d.na; ++a) m[a] = (T)out_mul_host[a];
-      SSQB_CUDA(cudaStreamSynchronize(st));
-      SSQB_CUDA(out_mul_d.upload(m));
-      out_mul = out_mul_d.p;
-    }
+    int rc = upload_out_mul(out_mul_host, d.na, out_mul_d, &out_mul, st); if (rc) return rc;
     // forward transform of the (padded) signal, scaled by 1/n (the 1/n of ifft)
     SSQB_CUDA(xp_d.ensure((size_t)B * (size_t)n)); SSQB_CUDA(xh_d.ensure((size_t)B * (size_t)n));
     gen_pad_kernel<T><<<(unsigned)((B * n + 255) / 256), 256, 0, st>>>((const T*)xv, xp_d.p, d.N, n,
                                                                        d.n1, d.padtype, B);
     SSQB_LAUNCH_CHECK();
-    int rc = fft.exec(xp_d.p, xh_d.p, B, -1, (T)(1.0 / (double)n), st); if (rc) return rc;
-    CwtArgs<T> A; args(A); A.xh = xh_d.p;
+    rc = fft.exec(xp_d.p, xh_d.p, B, -1, (T)(1.0 / (double)n), st); if (rc) return rc;
+    CwtArgs<T> A; cwt_common_args(d, scales_d.p, A); A.xh = xh_d.p;
     // rows in chunks of <= 64 MB per buffer
     long long chunk = ((64ll << 20) / (long long)sizeof(cx<T>)) / n; if (chunk < 1) chunk = 1;
     if (chunk > rows) chunk = rows;
@@ -396,25 +469,7 @@ struct GenericCwtPlan : public CwtPlanBase {
   }
   int exec_host(const void* x, long long B, void* Wx, void* dWx, void* Tx, bool ssq,
                 const double* out_mul_host, bool rpadded, cudaStream_t st) override {
-    const long long Nout = rpadded ? d.n_up : d.N;
-    const size_t nx = (size_t)B * (size_t)d.N, nout = (size_t)B * d.na * (size_t)Nout;
-    DevBuf<T> xs; DevBuf<cx<T>> Ws, dWs, Ts;
-    SSQB_CUDA(xs.ensure(nx));
-    if (Wx) SSQB_CUDA(Ws.ensure(nout));
-    if (dWx) SSQB_CUDA(dWs.ensure(nout));
-    if (ssq) SSQB_CUDA(Ts.ensure(nout));
-    SSQB_CUDA(cudaMemcpyAsync(xs.p, x, nx * sizeof(T), cudaMemcpyHostToDevice, st));
-    int rc = exec(xs.p, B, Wx ? Ws.p : nullptr, dWx ? dWs.p : nullptr, ssq ? Ts.p : nullptr, ssq,
-                  out_mul_host, rpadded, st);
-    if (rc == 0) {
-      if (Wx) SSQB_CUDA(cudaMemcpyAsync(Wx, Ws.p, nout * sizeof(cx<T>), cudaMemcpyDeviceToHost, st));
-      if (dWx) SSQB_CUDA(cudaMemcpyAsync(dWx, dWs.p, nout * sizeof(cx<T>), cudaMemcpyDeviceToHost, st));
-      if (ssq) SSQB_CUDA(cudaMemcpyAsync(Tx, Ts.p, nout * sizeof(cx<T>), cudaMemcpyDeviceToHost, st));
-    }
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (rc) return rc;
-    SSQB_CUDA(e);
-    return 0;
+    return staging.run(*this, d, x, B, Wx, dWx, Tx, ssq, out_mul_host, rpadded, st);
   }
   int debug_xh(const void* x, long long B, void* xh, cudaStream_t st) override {
     const long long n = d.n_up;
@@ -427,7 +482,7 @@ struct GenericCwtPlan : public CwtPlanBase {
   CwtAdjoint<T> adj;
   int backward(const void* gWx, const void* gdWx, long long B, const double* out_mul_host,
                bool rpadded, void* gx, cudaStream_t st) override {
-    CwtArgs<T> A; args(A);
+    CwtArgs<T> A; cwt_common_args(d, scales_d.p, A);
     return adj.run(d, A, (const cx<T>*)gWx, (const cx<T>*)gdWx, B, out_mul_host, rpadded, (T*)gx, st);
   }
   int set_profiling(int) override { return 0; }

@@ -14,31 +14,13 @@
 
 namespace ssqb {
 
-template <typename T>
-static std::vector<cx<T>> make_roots(long long count, long long step, long long n) {
-  // exp(+2 pi i (m*step) / n), m < count, evaluated in float64
-  std::vector<cx<T>> v((size_t)count);
-  for (long long m = 0; m < count; ++m) {
-    long long k = (m * step) % n;
-    // octant-exact angles keep cos/sin symmetric
-    double ang = 2.0 * M_PI * (double)k / (double)n;
-    v[(size_t)m] = mkc<T>((T)cos(ang), (T)sin(ang));
-  }
-  return v;
-}
-
-
 template <typename T, int LOG_M, int MODE>
 static int launch_pass1_t(const CwtArgs<T>& A, int narr, cudaStream_t st) {
   constexpr int M = 1 << LOG_M;
   constexpr int R1 = Tile<T>::ELEMS / M;
   size_t smem = ((size_t)M * (R1 + 1) + M) * sizeof(cx<T>);
   auto kern = cwt_pass1_kernel<T, LOG_M, MODE>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  SSQB_CUDA(opt_in_smem(kern, smem));
   long long ncol1 = (long long)A.nrows << A.logF;
   dim3 grid((unsigned)((ncol1 + R1 - 1) / R1), (unsigned)narr);
   kern<<<grid, Tile<T>::NT, smem, st>>>(A);
@@ -48,14 +30,7 @@ static int launch_pass1_t(const CwtArgs<T>& A, int narr, cudaStream_t st) {
 
 template <typename T, int MODE>
 static int launch_pass1(const CwtArgs<T>& A, int narr, cudaStream_t st) {
-  switch (A.logI2) {
-#define SSQB_P1(L) case L: return launch_pass1_t<T, L, MODE>(A, narr, st);
-    SSQB_P1(1) SSQB_P1(2) SSQB_P1(3) SSQB_P1(4) SSQB_P1(5) SSQB_P1(6)
-    SSQB_P1(7) SSQB_P1(8) SSQB_P1(9) SSQB_P1(10) SSQB_P1(11) SSQB_P1(12)
-#undef SSQB_P1
-    default: break;
-  }
-  return set_error(SSQB_E_UNSUPP, "unsupported pass-1 length 2^%d", A.logI2);
+  return dispatch_log2<1, 12>(A.logI2, [&](auto L) { return launch_pass1_t<T, L, MODE>(A, narr, st); });
 }
 
 template <typename T, int LOG_F, int NARR, int EPI>
@@ -64,11 +39,7 @@ static int launch_pass2_t(const CwtArgs<T>& A, int write_dWx, cudaStream_t st) {
   constexpr int R2 = Tile<T>::ELEMS / F;
   size_t smem = ((size_t)NARR * Tile<T>::ELEMS + F) * sizeof(cx<T>);
   auto kern = cwt_pass2_kernel<T, LOG_F, NARR, EPI>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  SSQB_CUDA(opt_in_smem(kern, smem));
   long long ncols = (long long)A.nrows << A.logI2;
   dim3 grid((unsigned)((ncols + R2 - 1) / R2));
   kern<<<grid, Tile<T>::NT, smem, st>>>(A, write_dWx);
@@ -78,13 +49,7 @@ static int launch_pass2_t(const CwtArgs<T>& A, int write_dWx, cudaStream_t st) {
 
 template <typename T, int NARR, int EPI>
 static int launch_pass2(const CwtArgs<T>& A, int write_dWx, cudaStream_t st) {
-  switch (A.logF) {
-#define SSQB_P2(L) case L: return launch_pass2_t<T, L, NARR, EPI>(A, write_dWx, st);
-    SSQB_P2(1) SSQB_P2(2) SSQB_P2(3) SSQB_P2(4) SSQB_P2(5) SSQB_P2(6)
-    SSQB_P2(7) SSQB_P2(8) SSQB_P2(9)
-#undef SSQB_P2
-    default: return set_error(SSQB_E_UNSUPP, "unsupported pass-2 length 2^%d", A.logF);
-  }
+  return dispatch_log2<1, 9>(A.logF, [&](auto L) { return launch_pass2_t<T, L, NARR, EPI>(A, write_dWx, st); });
 }
 
 // Every row kernel (direct, block and the second pass of the two-pass route) works on tiles of
@@ -113,11 +78,7 @@ static int launch_rows_b(const FastArgs<T>& P, unsigned grid_y, cudaStream_t st)
   if (LOG_F > 3) smem += (size_t)NARR * RowsTile<T, LOGE, LOG_F>::SARR * sizeof(cx<T>);
   if (GEN == GEN_DIRECT) smem += (size_t)QMAX * F * 4 * sizeof(T);
   auto kern = rows_kernel<T, LOGE, LOG_F, NARR, GEN, QMAX, SSQ, BPT, STORE_W>();
-  static size_t attr_smem = 0;
-  if (smem > attr_smem) {
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_smem = smem;
-  }
+  SSQB_CUDA(opt_in_smem(kern, smem));
   long long nF = (long long)A.n_up >> LOG_F;         // output phases per row
   dim3 grid((unsigned)(nF / (ELEMS / F)), grid_y);
   kern<<<grid, NT, smem, st>>>(P);
@@ -170,11 +131,7 @@ static int launch_pass1f_t(const FastArgs<T>& P, cudaStream_t st, int nz = 1) {
   static_assert(R1 >= 1, "tile smaller than the transform");
   size_t smem = ((size_t)NARR * M * (R1 + 1) + M) * sizeof(cx<T>);
   auto kern = cwt_pass1f_kernel<T, LOG_M, NARR>;
-  static size_t attr_smem = 0;
-  if (smem > attr_smem) {
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_smem = smem;
-  }
+  SSQB_CUDA(opt_in_smem(kern, smem));
   dim3 grid((unsigned)(512 / R1), (unsigned)P.A.nrows, (unsigned)nz);
   kern<<<grid, Tile<T>::NT, smem, st>>>(P);
   SSQB_LAUNCH_CHECK();
@@ -199,30 +156,20 @@ static int launch_pass1v(const FastArgs<T>& P, cudaStream_t st) {
   using V4 = typename V4T<T>::type;
   size_t smem = (size_t)512 * R1 * sizeof(V4) + 512 * sizeof(cx<T>);
   auto kern = cwt_pass1v_kernel<T, R1>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  SSQB_CUDA(opt_in_smem(kern, smem));
   kern<<<dim3(512 / R1, (unsigned)P.A.nrows), 64 * R1, smem, st>>>(P);
   SSQB_LAUNCH_CHECK();
   return 0;
 }
 
-// returns -100 when this geometry has no fast pass 1 (caller uses the generic kernel)
+// pass 1 of the fast path, whose geometry has 2^4 <= I2 <= 2^12
 template <typename T>
 static int launch_pass1f(const FastArgs<T>& P, int narr, cudaStream_t st) {
-  switch (P.A.logI2) {
-#define SSQB_P1F(L) case L: return narr == 2 ? launch_pass1f_t<T, L, 2>(P, st) \
-                                             : launch_pass1f_t<T, L, 1>(P, st);
-    SSQB_P1F(4) SSQB_P1F(5) SSQB_P1F(6) SSQB_P1F(7) SSQB_P1F(8)
-#undef SSQB_P1F
-    case 9: return narr == 2 ? launch_pass1v<T>(P, st) : launch_pass1f_t<T, 9, 1>(P, st);
-    case 10: return launch_pass1f_long<T, 10>(P, narr, st);
-    case 11: return launch_pass1f_long<T, 11>(P, narr, st);
-    case 12: return launch_pass1f_long<T, 12>(P, narr, st);
-    default: return -100;
-  }
+  return dispatch_log2<4, 12>(P.A.logI2, [&](auto L) {
+    if constexpr (L >= 10) return launch_pass1f_long<T, L>(P, narr, st);
+    else if constexpr (L == 9) return narr == 2 ? launch_pass1v<T>(P, st) : launch_pass1f_t<T, 9, 1>(P, st);
+    else return narr == 2 ? launch_pass1f_t<T, L, 2>(P, st) : launch_pass1f_t<T, L, 1>(P, st);
+  });
 }
 
 
@@ -232,11 +179,7 @@ static int launch_sblk_fwd(const SblkArgs<T>& S, cudaStream_t st) {
   constexpr int LP = SblkGeom<T>::LOG_P;
   size_t smem = ((size_t)1 << LP) * sizeof(cx<T>);
   auto kern = sblk_fwd_kernel<T, LP>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  SSQB_CUDA(opt_in_smem(kern, smem));
   kern<<<dim3((unsigned)S.nblk, (unsigned)S.B), (1 << LP) / 8, smem, st>>>(S);
   SSQB_LAUNCH_CHECK();
   return 0;
@@ -257,17 +200,10 @@ static int launch_sblk_rows_t(const SblkArgs<T>& S, SblkShare share, cudaStream_
   size_t smem = ((size_t)1 << LP) * (sizeof(V4) + sizeof(cx<T>));
   auto kern = sblk_rows_kernel<T, LP, SblkGeom<T>::LOG_R, NARR, SSQ>;
   if constexpr (!STORE_W) kern = sblk_rows_tx_kernel<T, LP, SblkGeom<T>::LOG_R>;
-  static bool attr_set = false;
-  static int sms = 132, per = 2, prio_high = 0;
-  if (!attr_set) {
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int dev = 0, least = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kern, NT, smem) != cudaSuccess || per < 1) per = 1;
-    SSQB_CUDA(cudaDeviceGetStreamPriorityRange(&least, &prio_high));
-    attr_set = true;
-  }
+  SSQB_CUDA(opt_in_smem(kern, smem));
+  DeviceFacts dev;
+  SSQB_CUDA(device_facts(&dev));
+  const int sms = dev.sms, per = blocks_per_sm(kern, NT, smem);
   const long long items = S.B * (long long)S.n_rows * S.nblk;
   if (items > 0x7fffffffll) return set_error(SSQB_E_UNSUPP, "too many short-block items");
   const long long ctas = (share == SBLK_ALONE) ? (long long)sms * per : sms;
@@ -276,7 +212,7 @@ static int launch_sblk_rows_t(const SblkArgs<T>& S, SblkShare share, cudaStream_
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(g); cfg.blockDim = dim3(NT); cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributePriority; attr[0].val.priority = prio_high;
+  attr[0].id = cudaLaunchAttributePriority; attr[0].val.priority = dev.prio_high;
   cfg.attrs = attr; cfg.numAttrs = (share == SBLK_BESIDE_GRID) ? 1 : 0;
   SSQB_CUDA(cudaLaunchKernelEx(&cfg, kern, S));
   SSQB_LAUNCH_CHECK();
@@ -328,11 +264,7 @@ static int launch_grid_dec_t(const GridArgs<T>& G, const GridRow* rows, int n_cl
   size_t smem = ((size_t)2 * Geo::M * Geo::R + Geo::M) * sizeof(cx<T>);
   if (smem > (size_t)227 * 1024) return set_error(SSQB_E_UNSUPP, "coarse grid 2^%d too long", LOG_M);
   auto kern = grid_dec_ifft_kernel<T, LOG_M>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  SSQB_CUDA(opt_in_smem(kern, smem));
   long long pairs = (long long)n_cls * G.B;
   dim3 grid((unsigned)((pairs + Geo::R - 1) / Geo::R));
   kern<<<grid, Geo::NT, smem, st>>>(G, rows, n_cls);
@@ -343,11 +275,7 @@ template <typename T, int LOG_M>
 static int launch_grid_dec_single(const GridArgs<T>& G, const GridRow* rows, int n_cls, cudaStream_t st) {
   size_t smem = ((size_t)1 << LOG_M) * sizeof(cx<T>);
   auto kern = grid_dec_single_kernel<T, LOG_M>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  SSQB_CUDA(opt_in_smem(kern, smem));
   kern<<<dim3((unsigned)(n_cls * G.B), 2), 1024, smem, st>>>(G, rows, n_cls);
   SSQB_LAUNCH_CHECK();
   return 0;
@@ -358,11 +286,7 @@ static int launch_grid_dec_split(const GridArgs<T>& G, int logR, const GridRow* 
                                  cudaStream_t st) {
   size_t smem = ((size_t)1 << LOG_MB) * sizeof(cx<T>);
   auto kern = grid_dec_split_kernel<T, LOG_MB>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  SSQB_CUDA(opt_in_smem(kern, smem));
   kern<<<dim3((unsigned)(((long long)n_cls * G.B) << logR), 2), 1024, smem, st>>>(G, rows, n_cls, logR);
   SSQB_LAUNCH_CHECK();
   return 0;
@@ -375,27 +299,14 @@ static int launch_grid_dec(const GridArgs<T>& G, int logM, const GridRow* rows, 
   if (logM > BASE) return launch_grid_dec_split<T, BASE>(G, logM - BASE, rows, n_cls, st);
   // one CTA per transform of 2^BASE points: it fills an SM's shared memory (1 CTA / SM)
   if (logM == BASE) return launch_grid_dec_single<T, BASE>(G, rows, n_cls, st);
-  switch (logM) {
-#define SSQB_GD(L) case L: return launch_grid_dec_t<T, L>(G, rows, n_cls, st);
-    SSQB_GD(6) SSQB_GD(7) SSQB_GD(8) SSQB_GD(9) SSQB_GD(10) SSQB_GD(11) SSQB_GD(12)
-#undef SSQB_GD
-    case 13:
-      if constexpr (sizeof(T) == 4) return launch_grid_dec_t<T, 13>(G, rows, n_cls, st);
-      break;
-    default: break;
-  }
-  return set_error(SSQB_E_UNSUPP, "no coarse-grid transform of 2^%d points", logM);
+  return dispatch_log2<6, BASE - 1>(logM, [&](auto L) { return launch_grid_dec_t<T, L>(G, rows, n_cls, st); });
 }
 
 template <typename T>
 static int launch_grid_dec_small(const GridArgs<T>& G, const DecSmallPlan& P, cudaStream_t st) {
   size_t smem = ((size_t)2 * 2048 + 2048) * sizeof(cx<T>);
   auto kern = grid_dec_ifft_small_kernel<T>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  SSQB_CUDA(opt_in_smem(kern, smem));
   if (P.cta_start[6] <= 0) return 0;
   kern<<<dim3((unsigned)P.cta_start[6]), 256, smem, st>>>(G, P);
   SSQB_LAUNCH_CHECK();
@@ -416,11 +327,7 @@ static int launch_grid_interp_t(const GridArgs<T>& G, unsigned max_tiles, cudaSt
   size_t smem = (size_t)(16 * PP + K - 1) * sizeof(V4) + (size_t)16 * PP * sizeof(cx<T>);
   auto kern = grid_interp_kernel<T, K, PPK, NARR, SSQ>;
   if constexpr (!STORE_W) kern = grid_interp_tx_kernel<T, K, PPK>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  SSQB_CUDA(opt_in_smem(kern, smem));
   dim3 grid(max_tiles, (unsigned)(G.B * G.n_rows));
   kern<<<grid, 256, smem, st>>>(G);
   SSQB_LAUNCH_CHECK();
@@ -497,7 +404,7 @@ struct CwtPlan : public CwtPlanBase {
   SblkClass sblk[SBLK_NCLS];
   bool have_sblk = false, have_cut = false;
   DevBuf<unsigned> sblk_ctr_d;                // per class: item counter of its row launches
-  cudaEvent_t ev_sblk_ready[SBLK_NCLS] = {nullptr, nullptr, nullptr};   // counter zeroed, spectra ready
+  Event ev_sblk_ready[SBLK_NCLS];               // counter zeroed, spectra ready
   DevBuf<cx<T>> rootsP_d, twsP_d, xa_d, Gxa_d;
   DevBuf<T> ctab_d;
   DevBuf<long long> xa_lo_d, xa_len_d;
@@ -520,32 +427,14 @@ struct CwtPlan : public CwtPlanBase {
   DevBuf<cx<T>> Gb_d;                         // scratch of the block forward FFTs (side stream)
   // side stream: the memset of Tx (pure HBM writes) overlaps the forward FFT and
   // pass 1 (which never touch Tx); joined before the first reassigning kernel
-  cudaStream_t side = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+  Stream side;
+  Event ev_fork, ev_join;
   // worker lanes: the row kernels of one call are independent of each other (disjoint
   // rows, commutative atomics); spreading them over a few streams lets the partial last
   // wave of one launch be filled by the next (12 launches, ~9 % of a step in tails)
   static constexpr int NLANES = 3;
-  cudaStream_t lanes[NLANES] = {nullptr, nullptr, nullptr};
-  cudaEvent_t ev_lane_fork = nullptr, ev_lane_done[NLANES] = {nullptr, nullptr, nullptr};
-  ~CwtPlan() {
-    for (int i = 0; i < NLANES; ++i) {
-      if (ev_lane_done[i]) cudaEventDestroy(ev_lane_done[i]);
-      if (lanes[i]) cudaStreamDestroy(lanes[i]);
-    }
-    if (ev_lane_fork) cudaEventDestroy(ev_lane_fork);
-    if (ev_fork) cudaEventDestroy(ev_fork);
-    if (ev_join) cudaEventDestroy(ev_join);
-    if (side) cudaStreamDestroy(side);
-    for (int i = 0; i < 2; ++i) {
-      if (ev_comp[i]) cudaEventDestroy(ev_comp[i]);
-      if (ev_d2h[i]) cudaEventDestroy(ev_d2h[i]);
-    }
-    if (copy_st) cudaStreamDestroy(copy_st);
-    if (ev_done) cudaEventDestroy(ev_done);
-    for (int i = 0; i < 2; ++i) if (ev_sa[i]) cudaEventDestroy(ev_sa[i]);
-    for (int i = 0; i < SBLK_NCLS; ++i) if (ev_sblk_ready[i]) cudaEventDestroy(ev_sblk_ready[i]);
-  }
+  Stream lanes[NLANES];
+  Event ev_lane_fork, ev_lane_done[NLANES];
   // optional per-kernel timing (bench.py roofline): CUDA events on the launch stream
   bool profiling = false;
   std::vector<cudaEvent_t> ev;          // pairs (start, stop)
@@ -588,13 +477,7 @@ struct CwtPlan : public CwtPlanBase {
     if (logn < 2 || logn > 21)
       return set_error(SSQB_E_UNSUPP, "n_up=%lld must be a power of two in [4, 2^21]",
                        (long long)d.n_up);
-    if (d.N < 1 || d.n1 < 0 || d.n1 + d.N > d.n_up)
-      return set_error(SSQB_E_ARG, "bad padding geometry N=%lld n1=%lld n_up=%lld",
-                       (long long)d.N, (long long)d.n1, (long long)d.n_up);
-    if (d.na < 1) return set_error(SSQB_E_ARG, "na must be >= 1");
-    if (d.wavelet < 0 || d.wavelet > 2) return set_error(SSQB_E_ARG, "bad wavelet kind");
-    if (d.wavelet == SSQB_WAV_TABLE && !d.psih_table_dev)
-      return set_error(SSQB_E_ARG, "SSQB_WAV_TABLE needs psih_table_dev");
+    { int rc = check_cwt_desc(d); if (rc) return rc; }
     if (logn >= 13) {
       logF = 9;                      // fast path geometry: F = 512, I2 = n/512 >= 16
     } else {
@@ -619,13 +502,13 @@ struct CwtPlan : public CwtPlanBase {
     SSQB_CUDA(tw2_d.upload(make_roots<T>(F, 1, F)));
     SSQB_CUDA(tw_lo_d.upload(make_roots<T>(1ll << log_lo, 1, n)));
     SSQB_CUDA(tw_hi_d.upload(make_roots<T>(n >> log_lo, 1ll << log_lo, n)));
-    SSQB_CUDA(cudaStreamCreateWithFlags(&side, cudaStreamNonBlocking));
-    SSQB_CUDA(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
-    SSQB_CUDA(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
-    SSQB_CUDA(cudaEventCreateWithFlags(&ev_lane_fork, cudaEventDisableTiming));
+    SSQB_CUDA(side.create());
+    SSQB_CUDA(ev_fork.create());
+    SSQB_CUDA(ev_join.create());
+    SSQB_CUDA(ev_lane_fork.create());
     for (int i = 0; i < NLANES; ++i) {
-      SSQB_CUDA(cudaStreamCreateWithFlags(&lanes[i], cudaStreamNonBlocking));
-      SSQB_CUDA(cudaEventCreateWithFlags(&ev_lane_done[i], cudaEventDisableTiming));
+      SSQB_CUDA(lanes[i].create());
+      SSQB_CUDA(ev_lane_done[i].create());
     }
     return init_fast(lo, len);
   }
@@ -777,7 +660,7 @@ struct CwtPlan : public CwtPlanBase {
     if (!have_sblk) return 0;
     SSQB_CUDA(sblk_ctr_d.ensure(SBLK_NCLS));
     for (int c = 0; c < SBLK_NCLS; ++c)
-      if (!ev_sblk_ready[c]) SSQB_CUDA(cudaEventCreateWithFlags(&ev_sblk_ready[c], cudaEventDisableTiming));
+      if (!ev_sblk_ready[c]) SSQB_CUDA(ev_sblk_ready[c].create());
     SSQB_CUDA(rootsP_d.upload(make_roots<T>(Pn, 1, Pn)));
     {
       // per-stage twiddles of sblk_rows_kernel: stage Ns (radix r) at Ns - R, [q - 1][k]
@@ -977,7 +860,7 @@ struct CwtPlan : public CwtPlanBase {
   }
   // coarse-grid inverse FFTs: the two long classes (2^13, 2^12 points: a few CTAs each) and the
   // merged launch of all shorter ones go to three streams so that their latencies overlap
-  cudaEvent_t ev_sa[2] = {nullptr, nullptr};
+  Event ev_sa[2];
   int grid_stage_a(const GridArgs<T>& G, long long B, cudaStream_t st, cudaStream_t s1,
                    cudaStream_t s2) {
     int rc = prof_begin(3, B * (long long)grid_rows.size(), st); if (rc) return rc;
@@ -1003,7 +886,7 @@ struct CwtPlan : public CwtPlanBase {
     }
     for (int i = 1; i < 3; ++i)
       if (used[i] && order[i] != st) {
-        if (!ev_sa[i - 1]) SSQB_CUDA(cudaEventCreateWithFlags(&ev_sa[i - 1], cudaEventDisableTiming));
+        if (!ev_sa[i - 1]) SSQB_CUDA(ev_sa[i - 1].create());
         SSQB_CUDA(cudaEventRecord(ev_sa[i - 1], order[i]));
         SSQB_CUDA(cudaStreamWaitEvent(st, ev_sa[i - 1], 0));
       }
@@ -1036,29 +919,9 @@ struct CwtPlan : public CwtPlanBase {
   }
 
   void base_args(CwtArgs<T>& A) {
-    memset(&A, 0, sizeof(A));
-    A.N = d.N; A.n_up = d.n_up; A.n1 = d.n1;
+    cwt_common_args(d, scales_d.p, A);
     A.logn = logn; A.logF = logF; A.logI2 = logI2;
-    A.padtype = d.padtype; A.na = d.na;
-    A.scales = scales_d.p; A.band_lo = band_lo_d.p; A.band_len = band_len_d.p;
-    A.psih_table = (const T*)d.psih_table_dev;
-    A.wavelet = d.wavelet;
-    if (d.wavelet == SSQB_WAV_MORLET) {
-      // constants cast to dtype exactly as wavelets.py:510-516
-      double mu = d.wparams[0];
-      double cs = pow(1 + exp(-mu * mu) - 2 * exp(-0.75 * mu * mu), -0.5);
-      double ks = exp(-0.5 * mu * mu);
-      A.wp[0] = (T)mu; A.wp[1] = (T)ks; A.wp[2] = (T)-0.5;
-      A.wp[3] = (T)(sqrt(2.0) * cs * pow(M_PI, 0.25));
-    } else if (d.wavelet == SSQB_WAV_GMW_L1) {
-      // _gmw.py:191-198: gamma, beta, wc, wcl cast to dtype; k0 = -beta*wcl + wc**gamma
-      double gam = d.wparams[0], bet = d.wparams[1];
-      double wc = exp((1.0 / gam) * (log(bet) - log(gam)));
-      T gT = (T)gam, bT = (T)bet, wcT = (T)wc, wclT = (T)log(wc);
-      T wcg = (T)pow((double)wcT, (double)gT);         // wc**gamma rounded to dtype
-      A.wp[0] = gT; A.wp[1] = bT; A.wp[2] = (T)(-(bT * wclT)) + wcg;
-    }
-    A.dt = (T)d.dt;
+    A.band_lo = band_lo_d.p; A.band_len = band_len_d.p;
     A.tw1 = tw1_d.p; A.tw2 = tw2_d.p; A.tw_lo = tw_lo_d.p; A.tw_hi = tw_hi_d.p;
     A.log_lo = log_lo;
     A.cst = cst_d.p;
@@ -1117,7 +980,7 @@ struct CwtPlan : public CwtPlanBase {
   // ordered on the device whatever streams they arrive on: each call first waits for the
   // completion event of the previous one (a no-op when both use the same stream).  If a call
   // fails half-way, the side / lane streams are still joined into the caller's stream.
-  cudaEvent_t ev_done = nullptr;
+  Event ev_done;
   bool ev_done_valid = false;
   long long maps_B = -1;                   // batch size the per-batch row maps were built for
   // zero-ahead state of the group being launched (see CwtArgs::zero_next)
@@ -1157,7 +1020,7 @@ struct CwtPlan : public CwtPlanBase {
 
   int exec(const void* xv, long long B, void* Wxv, void* dWxv, void* Txv, bool ssq,
            const double* out_mul_host, bool rpadded, cudaStream_t st) override {
-    if (!ev_done) SSQB_CUDA(cudaEventCreateWithFlags(&ev_done, cudaEventDisableTiming));
+    if (!ev_done) SSQB_CUDA(ev_done.create());
     if (ev_done_valid) SSQB_CUDA(cudaStreamWaitEvent(st, ev_done, 0));
     const long long S = (B >= 1) ? group_size(B, ssq, rpadded) : B;
     if (maps_B != S) {
@@ -1222,9 +1085,9 @@ struct CwtPlan : public CwtPlanBase {
         const size_t bytes = (size_t)total_rows * (size_t)Nout * sizeof(cx<T>);   // multiple of 8
         const size_t n16 = bytes / 16;
         constexpr int zctas = 16;              // CTAs per SM of the zero fill
-        static int sms = 0;
-        if (sms < 1) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms < 1) sms = 132; }
-        size_t nb = (n16 + 255) / 256; if (nb > (size_t)sms * zctas) nb = (size_t)sms * zctas; if (nb < 1) nb = 1;
+        DeviceFacts dev;
+        SSQB_CUDA(device_facts(&dev));
+        size_t nb = (n16 + 255) / 256; if (nb > (size_t)dev.sms * zctas) nb = (size_t)dev.sms * zctas; if (nb < 1) nb = 1;
         zero_fill_kernel<<<(unsigned)nb, 256, 0, side>>>(reinterpret_cast<uint4*>(Tx), n16,
                                                         reinterpret_cast<unsigned char*>(Tx) + n16 * 16,
                                                         (int)(bytes - n16 * 16));
@@ -1250,15 +1113,7 @@ struct CwtPlan : public CwtPlanBase {
     SSQB_CUDA(xh_d.ensure((size_t)B * (size_t)d.n_up));
 
     const T* out_mul = nullptr;
-    if (out_mul_host) {
-      std::vector<T> m((size_t)d.na);
-      for (int a = 0; a < d.na; ++a) m[a] = (T)out_mul_host[a];
-      SSQB_CUDA(out_mul_d.ensure((size_t)d.na));
-      SSQB_CUDA(cudaMemcpyAsync(out_mul_d.p, m.data(), m.size() * sizeof(T),
-                                cudaMemcpyHostToDevice, st));
-      SSQB_CUDA(cudaStreamSynchronize(st));   // `m` is a local
-      out_mul = out_mul_d.p;
-    }
+    rc = upload_out_mul(out_mul_host, d.na, out_mul_d, &out_mul, st); if (rc) return rc;
     int narr = (ssq || dWx) ? 2 : 1;
 
     // ---- streams of this call: 0 = the caller's stream, 1.. = worker lanes ---------------
@@ -1425,8 +1280,7 @@ struct CwtPlan : public CwtPlanBase {
         P.write_dWx = dWx ? 1 : 0; P.ssq = ssq ? 1 : 0;
         P.scratch_logR2 = ROWS_LOGE - 9;
         rc = prof_begin(1, nr, ts); if (rc) return rc;
-        rc = fast ? launch_pass1f<T>(P, narr, ts) : -100;
-        if (rc == -100) rc = launch_pass1<T, MODE_CWT>(A, narr, ts);
+        rc = fast ? launch_pass1f<T>(P, narr, ts) : launch_pass1<T, MODE_CWT>(A, narr, ts);
         if (rc) return rc;
         rc = prof_end(ts); if (rc) return rc;
         acquire(tk, true);                                 // pass 2 writes Tx: wait for the zero fill
@@ -1489,60 +1343,10 @@ struct CwtPlan : public CwtPlanBase {
     return 0;
   }
 
-  // Host buffers in, host buffers out (pinned memory recommended).  The batch is cut into
-  // chunks of two signals that ping-pong between two device staging slots:
-  // chunk c is transformed on the caller's stream while the copy stream still drains the
-  // outputs of chunk c-1 over PCIe, so the device holds two chunks of outputs, not the batch.
-  cudaStream_t copy_st = nullptr;
-  cudaEvent_t ev_comp[2] = {nullptr, nullptr}, ev_d2h[2] = {nullptr, nullptr};
+  HostStaging<T> staging;
   int exec_host(const void* x, long long B, void* Wx, void* dWx, void* Tx, bool ssq,
                 const double* out_mul_host, bool rpadded, cudaStream_t st) override {
-    if (B < 1) return set_error(SSQB_E_ARG, "B must be >= 1");
-    const long long CH = B < 2 ? B : 2;
-    const long long Nout = rpadded ? d.n_up : d.N;
-    const size_t nx = (size_t)CH * (size_t)d.N, nout = (size_t)CH * d.na * (size_t)Nout;
-    SSQB_CUDA(x_stage.ensure(2 * nx));
-    if (Wx) SSQB_CUDA(Wx_stage.ensure(2 * nout));
-    if (dWx) SSQB_CUDA(dWx_stage.ensure(2 * nout));
-    if (ssq) SSQB_CUDA(Tx_stage.ensure(2 * nout));
-    if (!copy_st) {
-      SSQB_CUDA(cudaStreamCreateWithFlags(&copy_st, cudaStreamNonBlocking));
-      for (int i = 0; i < 2; ++i) {
-        SSQB_CUDA(cudaEventCreateWithFlags(&ev_comp[i], cudaEventDisableTiming));
-        SSQB_CUDA(cudaEventCreateWithFlags(&ev_d2h[i], cudaEventDisableTiming));
-      }
-    }
-    const T* xh_ = (const T*)x;
-    cx<T>* Wh = (cx<T>*)Wx; cx<T>* dWh = (cx<T>*)dWx; cx<T>* Th = (cx<T>*)Tx;
-    int rc = 0, c = 0;
-    bool slot_busy[2] = {false, false};
-    for (long long b0 = 0; b0 < B; b0 += CH, ++c) {
-      const int sl = c & 1;
-      const long long nb = (B - b0 < CH) ? (B - b0) : CH;
-      const size_t cx_ = (size_t)nb * (size_t)d.N, co = (size_t)nb * d.na * (size_t)Nout;
-      if (slot_busy[sl]) SSQB_CUDA(cudaStreamWaitEvent(st, ev_d2h[sl], 0));   // slot drained
-      T* xs = x_stage.p + sl * nx;
-      cx<T>* Ws = Wx ? Wx_stage.p + sl * nout : nullptr;
-      cx<T>* dWs = dWx ? dWx_stage.p + sl * nout : nullptr;
-      cx<T>* Ts = ssq ? Tx_stage.p + sl * nout : nullptr;
-      SSQB_CUDA(cudaMemcpyAsync(xs, xh_ + (size_t)b0 * (size_t)d.N, cx_ * sizeof(T),
-                                cudaMemcpyHostToDevice, st));
-      rc = exec(xs, nb, Ws, dWs, Ts, ssq, out_mul_host, rpadded, st);
-      if (rc) break;
-      SSQB_CUDA(cudaEventRecord(ev_comp[sl], st));
-      SSQB_CUDA(cudaStreamWaitEvent(copy_st, ev_comp[sl], 0));
-      const size_t ho = (size_t)b0 * d.na * (size_t)Nout;
-      if (Wx) SSQB_CUDA(cudaMemcpyAsync(Wh + ho, Ws, co * sizeof(cx<T>), cudaMemcpyDeviceToHost, copy_st));
-      if (dWx) SSQB_CUDA(cudaMemcpyAsync(dWh + ho, dWs, co * sizeof(cx<T>), cudaMemcpyDeviceToHost, copy_st));
-      if (ssq) SSQB_CUDA(cudaMemcpyAsync(Th + ho, Ts, co * sizeof(cx<T>), cudaMemcpyDeviceToHost, copy_st));
-      SSQB_CUDA(cudaEventRecord(ev_d2h[sl], copy_st));
-      slot_busy[sl] = true;
-    }
-    // the call returns with the results in the host buffers
-    cudaError_t e1 = cudaStreamSynchronize(copy_st), e2 = cudaStreamSynchronize(st);
-    if (rc) return rc;
-    SSQB_CUDA(e1); SSQB_CUDA(e2);
-    return 0;
+    return staging.run(*this, d, x, B, Wx, dWx, Tx, ssq, out_mul_host, rpadded, st);
   }
 
   int debug_xh(const void* x, long long B, void* xh, cudaStream_t st) override {

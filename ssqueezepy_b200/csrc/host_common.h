@@ -7,7 +7,12 @@
 #include <string>
 #include <vector>
 #include <cmath>
+#include <cstring>
+#include <map>
+#include <mutex>
+#include <type_traits>
 #include "../../include/ssq_b200.h"
+#include "ssq_common.cuh"        // cx<T>, mkc<T>
 
 namespace ssqb {
 
@@ -42,6 +47,96 @@ inline int ilog2_exact(long long v) {     // -1 if not a power of two
   if (v <= 0 || (v & (v - 1))) return -1;
   int l = 0; while ((1ll << l) < v) ++l; return l;
 }
+
+// Calls f(std::integral_constant<int, L>{}) for the L in [LO, HI] equal to the runtime log2
+// length l and returns its result: the one place where a length picks a template instance.
+template <int LO, int HI, typename F>
+inline int dispatch_log2(int l, F&& f) {
+  if constexpr (LO > HI) {
+    return set_error(SSQB_E_UNSUPP, "no kernel for a transform of 2^%d points", l);
+  } else {
+    if (l == LO) return f(std::integral_constant<int, LO>{});
+    return dispatch_log2<LO + 1, HI>(l, f);
+  }
+}
+
+// n_fft whose frames the one-CTA power-of-two kernels of stft / istft transform (2 .. 4096)
+inline bool stft_pow2_tile(long long n_fft) {
+  const int l = ilog2_exact(n_fft);
+  return l >= 1 && l <= 12;
+}
+
+// Raises the dynamic shared-memory limit of `kern` on the current device to at least `bytes`.
+// The limit only grows, under a lock, so no caller lowers it below what another caller on the
+// same device has set for a launch in flight.
+cudaError_t opt_in_smem_raw(const void* kern, size_t bytes);
+template <typename K>
+inline cudaError_t opt_in_smem(K* kern, size_t bytes) { return opt_in_smem_raw((const void*)kern, bytes); }
+
+// Facts of the current device, queried once per device.
+struct DeviceFacts { int sms = 0, prio_least = 0, prio_high = 0; };
+cudaError_t device_facts(DeviceFacts* f);
+// CTAs of `kern` resident per SM (at least 1), queried once per (kernel, device)
+int blocks_per_sm_raw(const void* kern, int threads, size_t smem);
+template <typename K>
+inline int blocks_per_sm(K* kern, int threads, size_t smem) {
+  return blocks_per_sm_raw((const void*)kern, threads, smem);
+}
+
+// exp(+2 pi i (m * step) / n) for m < count, evaluated in float64 and rounded once
+template <typename T>
+std::vector<cx<T>> make_roots(long long count, long long step, long long n) {
+  std::vector<cx<T>> v((size_t)count);
+  for (long long m = 0; m < count; ++m) {
+    const long long k = (m * step) % n;
+    const double ang = 2.0 * M_PI * (double)k / (double)n;
+    v[(size_t)m] = mkc<T>((T)cos(ang), (T)sin(ang));
+  }
+  return v;
+}
+// the n-th roots of the STFT-family tables: built once per (length, dtype), not on every call
+template <typename T>
+const std::vector<cx<T>>& stft_roots(int n) {
+  static std::mutex mu;
+  static std::map<int, std::vector<cx<T>>> cache;
+  std::lock_guard<std::mutex> lk(mu);
+  auto it = cache.find(n);
+  if (it == cache.end()) it = cache.emplace(n, make_roots<T>(n, 1, n)).first;
+  return it->second;                         // map nodes are stable
+}
+
+// Host image of a table blob, every piece starting on a 16-byte boundary.
+struct BlobBuilder {
+  std::vector<unsigned char> h;
+  size_t put(const void* src, size_t bytes) {
+    size_t o = (h.size() + 15) & ~(size_t)15;
+    h.resize(o + bytes);
+    if (bytes) memcpy(h.data() + o, src, bytes);
+    return o;
+  }
+};
+// device copy of a blob, cached by content and device (stft_ops.cu)
+int table_blob(const std::vector<unsigned char>& h, cudaStream_t st, unsigned char** out);
+
+// owning stream / event handles, created on demand by their users
+struct Stream {
+  cudaStream_t s = nullptr;
+  Stream() = default;
+  Stream(const Stream&) = delete;
+  Stream& operator=(const Stream&) = delete;
+  ~Stream() { if (s) cudaStreamDestroy(s); }
+  cudaError_t create() { return cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking); }
+  operator cudaStream_t() const { return s; }
+};
+struct Event {
+  cudaEvent_t e = nullptr;
+  Event() = default;
+  Event(const Event&) = delete;
+  Event& operator=(const Event&) = delete;
+  ~Event() { if (e) cudaEventDestroy(e); }
+  cudaError_t create() { return cudaEventCreateWithFlags(&e, cudaEventDisableTiming); }
+  operator cudaEvent_t() const { return e; }
+};
 
 // owning device buffer that only ever grows
 template <typename T>

@@ -75,37 +75,44 @@ int run_invert_components(int dtype, const void* M, int na, long long N, const i
   if (smem > (size_t)(96 << 10)) return set_error(SSQB_E_UNSUPP, "too many components (%d)", K);
   dim3 grid((unsigned)((N + nt - 1) / nt));
   if (dtype == SSQB_F32) {
-    auto kern = invert_components_kernel<float>;
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<grid, nt, smem, st>>>((const float2*)M, out, na, N, cc, cw, K, scale);
+    SSQB_CUDA(opt_in_smem(invert_components_kernel<float>, smem));
+    invert_components_kernel<float><<<grid, nt, smem, st>>>((const float2*)M, out, na, N, cc, cw, K, scale);
   } else {
-    auto kern = invert_components_kernel<double>;
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<grid, nt, smem, st>>>((const double2*)M, out, na, N, cc, cw, K, scale);
+    SSQB_CUDA(opt_in_smem(invert_components_kernel<double>, smem));
+    invert_components_kernel<double><<<grid, nt, smem, st>>>((const double2*)M, out, na, N, cc, cw, K, scale);
   }
   SSQB_LAUNCH_CHECK();
   return 0;
 }
 
 template <typename T>
-static int launch_istft_pow2(const IstftArgs<T>& A, int logm, cudaStream_t st) {
+static int launch_istft_pow2(const IstftArgs<T>& A, cudaStream_t st) {
   const long long total = (long long)A.B * A.n_hops;
-  switch (logm) {
-#define SSQB_I(L)                                                                         \
-    case L: {                                                                             \
-      constexpr int M = 1 << L; constexpr int R = Tile<T>::ELEMS / M;                     \
-      size_t smem = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);                            \
-      auto kern = istft_frames_pow2_kernel<T, L>;                                         \
-      SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,   \
-                                     (int)smem));                                         \
-      kern<<<(unsigned)((total + R - 1) / R), Tile<T>::NT, smem, st>>>(A);                \
-      SSQB_LAUNCH_CHECK();                                                                \
-      return 0; }
-    SSQB_I(1) SSQB_I(2) SSQB_I(3) SSQB_I(4) SSQB_I(5) SSQB_I(6) SSQB_I(7) SSQB_I(8)
-    SSQB_I(9) SSQB_I(10) SSQB_I(11) SSQB_I(12)
-#undef SSQB_I
-    default: return -1;
-  }
+  return dispatch_log2<1, 12>(ilog2_exact(A.n_fft), [&](auto L) {
+    constexpr int M = 1 << L; constexpr int R = Tile<T>::ELEMS / M;
+    const size_t smem = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);
+    auto kern = istft_frames_pow2_kernel<T, L>;
+    SSQB_CUDA(opt_in_smem(kern, smem));
+    kern<<<(unsigned)((total + R - 1) / R), Tile<T>::NT, smem, st>>>(A);
+    SSQB_LAUNCH_CHECK();
+    return 0;
+  });
+}
+
+// n_fft that is not a power of two <= 4096: a direct DFT of R frames per CTA
+template <typename T>
+static int launch_istft_direct(const IstftArgs<T>& A, cudaStream_t st) {
+  const int M = A.n_fft, nrows = M / 2 + 1;
+  int R = (int)((size_t)(64 << 10) / ((size_t)nrows * sizeof(cx<T>)));
+  if (R < 1) R = 1; if (R > 32) R = 32;
+  const size_t smem = ((size_t)nrows * R + M) * sizeof(cx<T>);
+  if (smem > (size_t)(200 << 10))
+    return set_error(SSQB_E_UNSUPP, "n_fft=%d too large for the direct-DFT path", M);
+  SSQB_CUDA(opt_in_smem(istft_frames_direct_kernel<T>, smem));
+  const long long total = (long long)A.B * A.n_hops;
+  istft_frames_direct_kernel<T><<<(unsigned)((total + R - 1) / R), 256, smem, st>>>(A, R);
+  SSQB_LAUNCH_CHECK();
+  return 0;
 }
 
 template <typename T>
@@ -118,51 +125,24 @@ static int istft_t(const ssqb_istft_desc* d, const void* Sx, long long B, void* 
   A.max_hops = (d->N - 1) / d->hop + 1;             // (len(wn) - n_fft) // hop + 1
   A.Sx = (const cx<T>*)Sx; A.x = (T*)x;
   A.tiny = d->dtype == SSQB_F32 ? 1.1754943508222875e-38 : 2.2250738585072014e-308;
-  // small tables + the frame buffer, stream ordered
-  const size_t tb = sizeof(cx<T>) * (size_t)M + sizeof(T) * (size_t)(2 * M);
-  const size_t fb = sizeof(T) * (size_t)B * (size_t)d->n_hops * (size_t)M;
+  BlobBuilder bb;
+  const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
+  const size_t o_wexp = d->wexp_host ? bb.put(d->wexp_host, sizeof(T) * M) : 0;
+  const size_t o_wpow = bb.put(d->wpow_host, sizeof(T) * M);
   unsigned char* blob = nullptr;
-  SSQB_CUDA(cudaMallocAsync((void**)&blob, tb + fb + 256, st));
-  std::vector<unsigned char> h(tb);
-  std::vector<cx<T>> tw((size_t)M);
-  for (int m = 0; m < M; ++m) {
-    double ang = 2.0 * M_PI * (double)m / (double)M;
-    tw[m] = mkc<T>((T)cos(ang), (T)sin(ang));
-  }
-  memcpy(h.data(), tw.data(), sizeof(cx<T>) * M);
-  if (d->wexp_host) memcpy(h.data() + sizeof(cx<T>) * M, d->wexp_host, sizeof(T) * M);
-  memcpy(h.data() + sizeof(cx<T>) * M + sizeof(T) * M, d->wpow_host, sizeof(T) * M);
-  SSQB_CUDA(cudaMemcpyAsync(blob, h.data(), tb, cudaMemcpyHostToDevice, st));
-  SSQB_CUDA(cudaStreamSynchronize(st));                      // `h` is a local
-  A.tw = (const cx<T>*)blob;
-  A.wexp = d->wexp_host ? (const T*)(blob + sizeof(cx<T>) * M) : nullptr;
-  A.wpow = (const T*)(blob + sizeof(cx<T>) * M + sizeof(T) * M);
-  A.xbuf = (T*)(blob + ((tb + 255) / 256) * 256);
-  const int logm = ilog2_exact(M);
-  int rc = -1;
-  if (logm >= 1 && logm <= 12 && (Tile<T>::ELEMS >> logm) >= 1) rc = launch_istft_pow2<T>(A, logm, st);
-  if (rc == -1) {
-    const int nrows = M / 2 + 1;
-    int R = (int)((size_t)(64 << 10) / ((size_t)nrows * sizeof(cx<T>)));
-    if (R < 1) R = 1; if (R > 32) R = 32;
-    size_t smem = ((size_t)nrows * R + M) * sizeof(cx<T>);
-    if (smem > (size_t)(200 << 10)) {
-      cudaFreeAsync(blob, st);
-      return set_error(SSQB_E_UNSUPP, "n_fft=%d too large for the direct-DFT path", M);
-    }
-    auto kern = istft_frames_direct_kernel<T>;
-    SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const long long total = B * d->n_hops;
-    kern<<<(unsigned)((total + R - 1) / R), 256, smem, st>>>(A, R);
-    SSQB_LAUNCH_CHECK();
-    rc = 0;
-  }
+  int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
+  A.tw = (const cx<T>*)(blob + o_tw);
+  A.wexp = d->wexp_host ? (const T*)(blob + o_wexp) : nullptr;
+  A.wpow = (const T*)(blob + o_wpow);
+  // frame buffer, stream ordered
+  SSQB_CUDA(cudaMallocAsync((void**)&A.xbuf, sizeof(T) * (size_t)B * (size_t)d->n_hops * (size_t)M, st));
+  rc = stft_pow2_tile(M) ? launch_istft_pow2<T>(A, st) : launch_istft_direct<T>(A, st);
   if (rc == 0) {
     dim3 grid((unsigned)((d->N + 255) / 256), (unsigned)B);
     istft_ola_kernel<T><<<grid, 256, 0, st>>>(A);
     SSQB_LAUNCH_CHECK();
   }
-  cudaFreeAsync(blob, st);
+  cudaFreeAsync(A.xbuf, st);
   return rc;
 }
 

@@ -283,8 +283,8 @@ static int extract_ridges_t(const void* Tf, long long B, int na, long long N, co
   const size_t smem_b = ((size_t)(1 + 2 * RING_DEPTH) * na) * sizeof(T) + 16;
   if (smem > (size_t)200 * 1024 || smem_b > (size_t)200 * 1024)
     return set_error(SSQB_E_UNSUPP, "too many rows (%d) for ridge tracking", na);
-  SSQB_CUDA(cudaFuncSetAttribute(ridge_forward_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  SSQB_CUDA(cudaFuncSetAttribute(ridge_backward_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_b));
+  SSQB_CUDA(opt_in_smem(ridge_forward_kernel<T>, smem));
+  SSQB_CUDA(opt_in_smem(ridge_backward_kernel<T>, smem_b));
   for (int i = 0; i < n_ridges; ++i) {
     for (long long b = 0; b < B; ++b) {
       ridge_neglog_kernel<T><<<(unsigned)((N + 127) / 128), 128, 0, st>>>(energy.p + b * plane, eT.p + b * plane, na, N, (T)eps);

@@ -19,7 +19,7 @@ static std::mutex g_blob_mu;
 static std::vector<TableBlob> g_blobs;
 static unsigned long long g_blob_tick = 0;
 
-static int table_blob(const std::vector<unsigned char>& h, cudaStream_t st, unsigned char** out) {
+int table_blob(const std::vector<unsigned char>& h, cudaStream_t st, unsigned char** out) {
   int dev = 0;
   SSQB_CUDA(cudaGetDevice(&dev));
   std::lock_guard<std::mutex> lk(g_blob_mu);
@@ -41,33 +41,21 @@ static int table_blob(const std::vector<unsigned char>& h, cudaStream_t st, unsi
 }
 
 template <typename T, int EPI>
-static int launch_stft_pow2(const StftArgs<T>& A, int logm, cudaStream_t st) {
-  long long total = (long long)A.B * A.n_hops;
-  switch (logm) {
-#define SSQB_S(L)                                                                         \
-    case L: {                                                                             \
-      constexpr int M = 1 << L; constexpr int R = Tile<T>::ELEMS / M;                     \
-      size_t smem = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);                            \
-      auto kern = stft_pow2_kernel<T, L, EPI>;                                            \
-      static bool attr_done = false;                                                      \
-      if (!attr_done) {                                                                   \
-        SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                       (int)smem));                                       \
-        attr_done = true;                                                                 \
-      }                                                                                   \
-      kern<<<(unsigned)((total + R - 1) / R), Tile<T>::NT, smem, st>>>(A);                \
-      SSQB_LAUNCH_CHECK();                                                                \
-      return 0; }
-    SSQB_S(1) SSQB_S(2) SSQB_S(3) SSQB_S(4) SSQB_S(5) SSQB_S(6) SSQB_S(7) SSQB_S(8)
-    SSQB_S(9) SSQB_S(10) SSQB_S(11) SSQB_S(12)
-#undef SSQB_S
-    default: return -1;
-  }
+static int launch_stft_pow2(const StftArgs<T>& A, cudaStream_t st) {
+  const long long total = (long long)A.B * A.n_hops;
+  return dispatch_log2<1, 12>(ilog2_exact(A.n_fft), [&](auto L) {
+    constexpr int M = 1 << L; constexpr int R = Tile<T>::ELEMS / M;
+    const size_t smem = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);
+    auto kern = stft_pow2_kernel<T, L, EPI>;
+    SSQB_CUDA(opt_in_smem(kern, smem));
+    kern<<<(unsigned)((total + R - 1) / R), Tile<T>::NT, smem, st>>>(A);
+    SSQB_LAUNCH_CHECK();
+    return 0;
+  });
 }
 
 // n_fft that is not a power of two (e.g. 598 = 2 * 13 * 23, the reference's own benchmark
-// size): frames -> batched mixed-radix / Bluestein FFT -> Hermitian split + epilogue, in
-// chunks of frames that keep the two frame buffers below ~128 MB each.
+// size): frames -> batched mixed-radix / Bluestein FFT -> Hermitian split + epilogue.
 template <typename T> struct StftGeneric {
   Gfft<T> fft; DevBuf<cx<T>> c, C;
 };
@@ -75,49 +63,55 @@ static std::mutex g_gen_mu;
 template <typename T> static std::map<std::pair<int, int>, std::unique_ptr<StftGeneric<T>>>& gen_cache() {
   static std::map<std::pair<int, int>, std::unique_ptr<StftGeneric<T>>> m; return m;
 }
-template <typename T, int EPI>
-static int launch_stft_generic(const StftArgs<T>& A, cudaStream_t st) {
+// The frame loop of every generic-length route, in chunks of frames that keep each of the two
+// buffers at ~128 MB: pre(c, f0, nf) writes `seqs` sequences of n_fft points per frame, one
+// batched Gfft of the given sign takes c to C, post(C, f0, nf) reads them.  The FFT plan and
+// buffers are cached per (device, n_fft) and shared by every caller, one at a time.
+template <typename T, typename Pre, typename Post>
+static int generic_frames(int n_fft, long long total, int seqs, int sign, Pre pre, Post post,
+                          cudaStream_t st) {
   int dev = 0; SSQB_CUDA(cudaGetDevice(&dev));
   std::lock_guard<std::mutex> lk(g_gen_mu);            // one caller at a time per process
-  auto& slot = gen_cache<T>()[{dev, A.n_fft}];
+  auto& slot = gen_cache<T>()[{dev, n_fft}];
   if (!slot) {
     slot.reset(new StftGeneric<T>());
-    int rc = slot->fft.init(A.n_fft);
+    int rc = slot->fft.init(n_fft);
     if (rc) { slot.reset(); return rc; }
   }
   StftGeneric<T>& G = *slot;
-  const long long total = (long long)A.B * A.n_hops, M = A.n_fft, nrows = M / 2 + 1;
-  long long chunk = ((128ll << 20) / (long long)sizeof(cx<T>)) / M; if (chunk < 1) chunk = 1;
+  const long long M = n_fft;
+  long long chunk = ((128ll << 20) / (long long)sizeof(cx<T>)) / (seqs * M); if (chunk < 1) chunk = 1;
   if (chunk > total) chunk = total;
-  SSQB_CUDA(G.c.ensure((size_t)chunk * (size_t)M)); SSQB_CUDA(G.C.ensure((size_t)chunk * (size_t)M));
+  SSQB_CUDA(G.c.ensure((size_t)chunk * seqs * (size_t)M)); SSQB_CUDA(G.C.ensure((size_t)chunk * seqs * (size_t)M));
   for (long long f0 = 0; f0 < total; f0 += chunk) {
     const long long nf = total - f0 < chunk ? total - f0 : chunk;
-    stft_frames_kernel<T, EPI><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(A, G.c.p, f0, nf);
-    SSQB_LAUNCH_CHECK();
-    int rc = G.fft.exec(G.c.p, G.C.p, nf, -1, (T)1, st); if (rc) return rc;
-    stft_emit_kernel<T, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(A, G.C.p, f0, nf);
-    SSQB_LAUNCH_CHECK();
+    int rc = pre(G.c.p, f0, nf); if (rc) return rc;
+    rc = G.fft.exec(G.c.p, G.C.p, seqs * nf, sign, (T)1, st); if (rc) return rc;
+    rc = post(G.C.p, f0, nf); if (rc) return rc;
   }
   SSQB_CUDA(cudaStreamSynchronize(st));                // buffers are shared by later callers
   return 0;
 }
 
-// n_fft-th roots exp(+2 pi i m / n_fft): computed once per (length, dtype), not on every call
-template <typename T>
-static const std::vector<cx<T>>& roots(int M) {
-  static std::mutex tw_mu;
-  static std::map<int, std::vector<cx<T>>> tw_cache;
-  std::lock_guard<std::mutex> lk(tw_mu);
-  auto it = tw_cache.find(M);
-  if (it == tw_cache.end()) {
-    std::vector<cx<T>> v((size_t)M);
-    for (int m = 0; m < M; ++m) {
-      double ang = 2.0 * M_PI * (double)m / (double)M;
-      v[m] = mkc<T>((T)cos(ang), (T)sin(ang));
-    }
-    it = tw_cache.emplace(M, std::move(v)).first;
-  }
-  return it->second;                         // map nodes are stable
+template <typename T, int EPI>
+static int launch_stft_generic(const StftArgs<T>& A, cudaStream_t st) {
+  const long long M = A.n_fft, nrows = M / 2 + 1;
+  return generic_frames<T>(A.n_fft, (long long)A.B * A.n_hops, 1, -1,
+      [&](cx<T>* c, long long f0, long long nf) {
+        stft_frames_kernel<T, EPI><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(A, c, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      },
+      [&](const cx<T>* C, long long f0, long long nf) {
+        stft_emit_kernel<T, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(A, C, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      }, st);
+}
+
+template <typename T, int EPI>
+static int launch_stft(const StftArgs<T>& A, cudaStream_t st) {
+  return stft_pow2_tile(A.n_fft) ? launch_stft_pow2<T, EPI>(A, st) : launch_stft_generic<T, EPI>(A, st);
 }
 
 // kappa = power of two that balances ||win|| and ||dwin||
@@ -148,38 +142,26 @@ static int stft_t(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const vo
   // device copies of the small tables: built on the host, cached on the device by content
   // (a streaming caller repeats the same window / grid thousands of times; without the
   // cache every call pays an allocation, a copy and a stream synchronisation)
-  size_t tb = sizeof(T) * (size_t)(2 * M + nrows) + sizeof(cx<T>) * (size_t)M + sizeof(double) * nrows;
-  std::vector<unsigned char> h(tb);
-  size_t off = 0;
-  auto put = [&](const void* src, size_t bytes) { memcpy(h.data() + off, src, bytes); size_t o = off; off += bytes; return o; };
-  const std::vector<cx<T>>& tw = roots<T>(M);
   std::vector<double> cst((size_t)nrows, 0.0);
   if (ssq) for (int i = 0; i < nrows; ++i) cst[i] = r->cst_host[i];
-  size_t o_tw = put(tw.data(), sizeof(cx<T>) * M);          // 16-byte aligned first
-  size_t o_cst = put(cst.data(), sizeof(double) * nrows);
-  size_t o_win = put(win, sizeof(T) * M);
-  size_t o_dwin = put(dwin, sizeof(T) * M);
-  size_t o_sfs = put(d->Sfs_host, sizeof(T) * nrows);
+  BlobBuilder bb;
+  const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
+  const size_t o_cst = bb.put(cst.data(), sizeof(double) * nrows);
+  const size_t o_win = bb.put(win, sizeof(T) * M);
+  const size_t o_dwin = bb.put(dwin, sizeof(T) * M);
+  const size_t o_sfs = bb.put(d->Sfs_host, sizeof(T) * nrows);
   unsigned char* blob = nullptr;
-  int rcb = table_blob(h, st, &blob); if (rcb) return rcb;
+  int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
   A.tw = (const cx<T>*)(blob + o_tw); A.cst = (const double*)(blob + o_cst);
   A.win = (const T*)(blob + o_win); A.dwin = (const T*)(blob + o_dwin);
   A.Sfs = (const T*)(blob + o_sfs);
   if (ssq) {
-    int rc = fill_grid(r, nrows, &A.grid); if (rc) return rc;
+    rc = fill_grid(r, nrows, &A.grid); if (rc) return rc;
     A.grid.kind = 3;
     SSQB_CUDA(cudaMemsetAsync(Tx, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(cx<T>), st));
   }
-  int logm = ilog2_exact(M);
-  int rc;
-  const bool pow2 = logm >= 1 && logm <= 12 && (Tile<T>::ELEMS >> logm) >= 1;
-  if (ssq && !Sx)        // Tx only
-    rc = pow2 ? launch_stft_pow2<T, STFT_EPI_SSQ_TX>(A, logm, st) : launch_stft_generic<T, STFT_EPI_SSQ_TX>(A, st);
-  else if (pow2)
-    rc = ssq ? launch_stft_pow2<T, STFT_EPI_SSQ>(A, logm, st) : launch_stft_pow2<T, STFT_EPI_PLAIN>(A, logm, st);
-  else
-    rc = ssq ? launch_stft_generic<T, STFT_EPI_SSQ>(A, st) : launch_stft_generic<T, STFT_EPI_PLAIN>(A, st);
-  return rc;
+  if (ssq && !Sx) return launch_stft<T, STFT_EPI_SSQ_TX>(A, st);      // Tx only
+  return ssq ? launch_stft<T, STFT_EPI_SSQ>(A, st) : launch_stft<T, STFT_EPI_PLAIN>(A, st);
 }
 
 int run_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const void* x, long long B,
@@ -193,69 +175,35 @@ int run_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const void* x
 }
 
 // ---- backward passes (torch.autograd) --------------------------------------------------------
-// Table blob with every piece starting on a 16-byte boundary.
-struct BlobBuilder {
-  std::vector<unsigned char> h;
-  size_t put(const void* src, size_t bytes) {
-    size_t o = (h.size() + 15) & ~(size_t)15;
-    h.resize(o + bytes);
-    if (bytes) memcpy(h.data() + o, src, bytes);
-    return o;
-  }
-};
-
 template <typename T>
-static int launch_stft_bwd_pow2(const StftBwdArgs<T>& A, int logm, cudaStream_t st) {
+static int launch_stft_bwd_pow2(const StftBwdArgs<T>& A, cudaStream_t st) {
   const long long total = (long long)A.B * A.n_hops;
-  switch (logm) {
-#define SSQB_SB(L)                                                                        \
-    case L: {                                                                             \
-      constexpr int M = 1 << L; constexpr int R = Tile<T>::ELEMS / M;                     \
-      size_t smem = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);                            \
-      auto kern = stft_bwd_pow2_kernel<T, L>;                                             \
-      static bool attr_done = false;                                                      \
-      if (!attr_done) {                                                                   \
-        SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                       (int)smem));                                       \
-        attr_done = true;                                                                 \
-      }                                                                                   \
-      kern<<<(unsigned)((total + R - 1) / R), Tile<T>::NT, smem, st>>>(A);                \
-      SSQB_LAUNCH_CHECK();                                                                \
-      return 0; }
-    SSQB_SB(1) SSQB_SB(2) SSQB_SB(3) SSQB_SB(4) SSQB_SB(5) SSQB_SB(6) SSQB_SB(7) SSQB_SB(8)
-    SSQB_SB(9) SSQB_SB(10) SSQB_SB(11) SSQB_SB(12)
-#undef SSQB_SB
-    default: return -1;
-  }
+  return dispatch_log2<1, 12>(ilog2_exact(A.n_fft), [&](auto L) {
+    constexpr int M = 1 << L; constexpr int R = Tile<T>::ELEMS / M;
+    const size_t smem = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);
+    auto kern = stft_bwd_pow2_kernel<T, L>;
+    SSQB_CUDA(opt_in_smem(kern, smem));
+    kern<<<(unsigned)((total + R - 1) / R), Tile<T>::NT, smem, st>>>(A);
+    SSQB_LAUNCH_CHECK();
+    return 0;
+  });
 }
 
 // other n_fft: packed spectra -> inverse Gfft -> epilogue, in the forward's chunks and buffers
 template <typename T>
 static int launch_stft_bwd_generic(const StftBwdArgs<T>& A, cudaStream_t st) {
-  int dev = 0; SSQB_CUDA(cudaGetDevice(&dev));
-  std::lock_guard<std::mutex> lk(g_gen_mu);
-  auto& slot = gen_cache<T>()[{dev, A.n_fft}];
-  if (!slot) {
-    slot.reset(new StftGeneric<T>());
-    int rc = slot->fft.init(A.n_fft);
-    if (rc) { slot.reset(); return rc; }
-  }
-  StftGeneric<T>& G = *slot;
-  const long long total = (long long)A.B * A.n_hops, M = A.n_fft;
-  long long chunk = ((128ll << 20) / (long long)sizeof(cx<T>)) / M; if (chunk < 1) chunk = 1;
-  if (chunk > total) chunk = total;
-  SSQB_CUDA(G.c.ensure((size_t)chunk * (size_t)M)); SSQB_CUDA(G.C.ensure((size_t)chunk * (size_t)M));
-  for (long long f0 = 0; f0 < total; f0 += chunk) {
-    const long long nf = total - f0 < chunk ? total - f0 : chunk;
-    const unsigned nb = (unsigned)((nf * M + 255) / 256);
-    stft_bwd_spec_kernel<T><<<nb, 256, 0, st>>>(A, G.c.p, f0, nf);
-    SSQB_LAUNCH_CHECK();
-    int rc = G.fft.exec(G.c.p, G.C.p, nf, +1, (T)1, st); if (rc) return rc;
-    stft_bwd_frames_kernel<T><<<nb, 256, 0, st>>>(A, G.C.p, f0, nf);
-    SSQB_LAUNCH_CHECK();
-  }
-  SSQB_CUDA(cudaStreamSynchronize(st));                // buffers are shared by later callers
-  return 0;
+  const long long M = A.n_fft;
+  return generic_frames<T>(A.n_fft, (long long)A.B * A.n_hops, 1, +1,
+      [&](cx<T>* c, long long f0, long long nf) {
+        stft_bwd_spec_kernel<T><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(A, c, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      },
+      [&](const cx<T>* C, long long f0, long long nf) {
+        stft_bwd_frames_kernel<T><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(A, C, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      }, st);
 }
 
 template <typename T>
@@ -275,8 +223,7 @@ static int stft_bwd_t(const ssqb_stft_desc* d, const void* gS, const void* gdS, 
   const std::vector<long long>& off = pg.off; const std::vector<long long>& js = pg.j;
   const std::vector<long long>& ts = pg.t;
   BlobBuilder bb;
-  const std::vector<cx<T>>& tw = roots<T>(M);
-  const size_t o_tw = bb.put(tw.data(), sizeof(cx<T>) * M);
+  const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
   const size_t o_win = bb.put(win, sizeof(T) * M);
   const size_t o_dwin = bb.put(dwin, sizeof(T) * M);
   const size_t o_off = bb.put(off.data(), sizeof(long long) * off.size());
@@ -291,9 +238,7 @@ static int stft_bwd_t(const ssqb_stft_desc* d, const void* gS, const void* gdS, 
   A.n_pad_groups = (long long)js.size();
   // frame buffer: B * n_hops * n_fft reals, no larger than gSx
   SSQB_CUDA(cudaMallocAsync((void**)&A.ybuf, sizeof(T) * (size_t)B * (size_t)A.n_hops * (size_t)M, st));
-  const int logm = ilog2_exact(M);
-  if (logm >= 1 && logm <= 12 && (Tile<T>::ELEMS >> logm) >= 1) rc = launch_stft_bwd_pow2<T>(A, logm, st);
-  else rc = launch_stft_bwd_generic<T>(A, st);
+  rc = stft_pow2_tile(M) ? launch_stft_bwd_pow2<T>(A, st) : launch_stft_bwd_generic<T>(A, st);
   if (rc == 0) {
     const unsigned gy = (unsigned)(B < 65535 ? B : 65535);
     stft_bwd_gather_kernel<T><<<dim3((unsigned)((A.N + 255) / 256), gy), 256, 0, st>>>(A);
@@ -336,8 +281,7 @@ static int istft_bwd_t(const ssqb_istft_desc* d, const void* gx, long long B, vo
     if (wexp) win[l] = wexp[m];
   }
   BlobBuilder bb;
-  const std::vector<cx<T>>& tw = roots<T>(M);
-  const size_t o_tw = bb.put(tw.data(), sizeof(cx<T>) * M);
+  const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
   const size_t o_win = bb.put(win.data(), sizeof(T) * M);
   const size_t o_wpow = bb.put(d->wpow_host, sizeof(T) * M);
   unsigned char* blob = nullptr;
@@ -354,11 +298,7 @@ static int istft_bwd_t(const ssqb_istft_desc* d, const void* gx, long long B, vo
   A.x = gp; A.win = (const T*)(blob + o_win); A.dwin = nullptr;
   A.kappa = (T)1; A.inv_kappa = (T)1;
   A.Sx = (cx<T>*)gS; A.tw = (const cx<T>*)(blob + o_tw);
-  const int logm = ilog2_exact(M);
-  if (logm >= 1 && logm <= 12 && (Tile<T>::ELEMS >> logm) >= 1)
-    rc = launch_stft_pow2<T, STFT_EPI_ISTFT_BWD>(A, logm, st);
-  else
-    rc = launch_stft_generic<T, STFT_EPI_ISTFT_BWD>(A, st);
+  rc = launch_stft<T, STFT_EPI_ISTFT_BWD>(A, st);
   cudaFreeAsync(gp, st);
   return rc;
 }
@@ -380,62 +320,43 @@ int run_istft_backward(const ssqb_istft_desc* d, const void* gx, long long B, vo
 // batched Gfft of 3 transforms per frame -> emit, in chunks that keep each buffer at ~128 MB.
 static constexpr size_t kMaxBlockSmem = 227u << 10;    // sm_90 opt-in limit per block
 
-template <typename T, int L, int EPI>
-static int launch_stft2_tile(const Stft2Args<T>& P, cudaStream_t st) {
-  using TL = Stft2Tile<T, L>;
-  if constexpr (TL::SMEM > kMaxBlockSmem) {
-    return set_error(SSQB_E_UNSUPP, "n_fft = 2^%d does not fit one CTA", L);
-  } else {
-    const long long total = (long long)P.A.B * P.A.n_hops;
-    auto kern = stft2_pow2_kernel<T, L, EPI>;
-    static bool attr_done = false;
-    if (!attr_done) {
-      SSQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TL::SMEM));
-      attr_done = true;
-    }
-    kern<<<(unsigned)((total + TL::F - 1) / TL::F), Tile<T>::NT, TL::SMEM, st>>>(P);
-    SSQB_LAUNCH_CHECK();
-    return 0;
-  }
-}
-
-template <typename T, int L = 1>
+template <typename T>
 static bool stft2_pow2_fits(int logm) {
-  if constexpr (L > 12) return false;
-  else return logm == L ? Stft2Tile<T, L>::SMEM <= kMaxBlockSmem : stft2_pow2_fits<T, L + 1>(logm);
+  return logm >= 1 && logm <= 12 &&
+         dispatch_log2<1, 12>(logm, [](auto L) { return Stft2Tile<T, L>::SMEM <= kMaxBlockSmem ? 1 : 0; });
 }
 
-template <typename T, int EPI, int L = 1>
+template <typename T, int EPI>
 static int launch_stft2_pow2(const Stft2Args<T>& P, int logm, cudaStream_t st) {
-  if constexpr (L > 12) return set_error(SSQB_E_ARG, "n_fft is not a power of two <= 4096");
-  else return logm == L ? launch_stft2_tile<T, L, EPI>(P, st) : launch_stft2_pow2<T, EPI, L + 1>(P, logm, st);
+  return dispatch_log2<1, 12>(logm, [&](auto L) {
+    using TL = Stft2Tile<T, L>;
+    if constexpr (TL::SMEM > kMaxBlockSmem) {
+      return set_error(SSQB_E_UNSUPP, "n_fft = 2^%d does not fit one CTA", (int)L);
+    } else {
+      const long long total = (long long)P.A.B * P.A.n_hops;
+      auto kern = stft2_pow2_kernel<T, L, EPI>;
+      SSQB_CUDA(opt_in_smem(kern, TL::SMEM));
+      kern<<<(unsigned)((total + TL::F - 1) / TL::F), Tile<T>::NT, TL::SMEM, st>>>(P);
+      SSQB_LAUNCH_CHECK();
+      return 0;
+    }
+  });
 }
 
 template <typename T, int EPI>
 static int launch_stft2_generic(const Stft2Args<T>& P, cudaStream_t st) {
-  int dev = 0; SSQB_CUDA(cudaGetDevice(&dev));
-  std::lock_guard<std::mutex> lk(g_gen_mu);            // buffers shared with the first order
-  auto& slot = gen_cache<T>()[{dev, P.A.n_fft}];
-  if (!slot) {
-    slot.reset(new StftGeneric<T>());
-    int rc = slot->fft.init(P.A.n_fft);
-    if (rc) { slot.reset(); return rc; }
-  }
-  StftGeneric<T>& G = *slot;
-  const long long total = (long long)P.A.B * P.A.n_hops, M = P.A.n_fft, nrows = M / 2 + 1;
-  long long chunk = ((128ll << 20) / (long long)sizeof(cx<T>)) / (3 * M); if (chunk < 1) chunk = 1;
-  if (chunk > total) chunk = total;
-  SSQB_CUDA(G.c.ensure((size_t)chunk * 3 * (size_t)M)); SSQB_CUDA(G.C.ensure((size_t)chunk * 3 * (size_t)M));
-  for (long long f0 = 0; f0 < total; f0 += chunk) {
-    const long long nf = total - f0 < chunk ? total - f0 : chunk;
-    stft2_frames_kernel<T><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(P, G.c.p, f0, nf);
-    SSQB_LAUNCH_CHECK();
-    int rc = G.fft.exec(G.c.p, G.C.p, 3 * nf, -1, (T)1, st); if (rc) return rc;
-    stft2_emit_kernel<T, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(P, G.C.p, f0, nf);
-    SSQB_LAUNCH_CHECK();
-  }
-  SSQB_CUDA(cudaStreamSynchronize(st));                // buffers are shared by later callers
-  return 0;
+  const long long M = P.A.n_fft, nrows = M / 2 + 1;
+  return generic_frames<T>(P.A.n_fft, (long long)P.A.B * P.A.n_hops, 3, -1,
+      [&](cx<T>* c, long long f0, long long nf) {
+        stft2_frames_kernel<T><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(P, c, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      },
+      [&](const cx<T>* C, long long f0, long long nf) {
+        stft2_emit_kernel<T, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(P, C, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      }, st);
 }
 
 template <typename T, int EPI>
@@ -466,8 +387,7 @@ static int stft2_t(const ssqb_stft_desc* d, const ssqb_stft2_tables* t2, const s
   A.kappa = (T)kap; A.inv_kappa = (T)(1.0 / kap);
   P.kappa2 = (T)kap2; P.inv_kappa2 = (T)(1.0 / kap2);
   BlobBuilder bb;
-  const std::vector<cx<T>>& tw = roots<T>(M);
-  const size_t o_tw = bb.put(tw.data(), sizeof(cx<T>) * M);
+  const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
   const size_t o_cst = bb.put(r->cst_host, sizeof(double) * nrows);
   const size_t o_win = bb.put(win, sizeof(T) * M);
   const size_t o_dwin = bb.put(dwin, sizeof(T) * M);
