@@ -181,6 +181,22 @@ int ssqb_ssqueeze_backward(int dtype, const void* Wx_dev, const void* dWx_dev,
 int ssqb_indexed_sum_backward(int dtype, const void* w_dev, const void* gTx_dev,
                               const void* gWx_dev, void* gWout_dev, int64_t B, int na,
                               int64_t N, const ssqb_reassign_desc* r, void* stream);
+/* reassignment of the second-order ssq_cwt (not in the reference): the first order's gamma test,
+ * bins and typed accumulation with the frequency estimate corrected by the local frequency
+ * modulation, exact for linear chirps.  Five [B][na][N] complex planes of one plan:
+ *   Wx  = ifft(psih_a xh)               dWx = ifft(i Om psih_a xh)        (Om = xi / dt)
+ *   A   = ifft(a psih'(a xi) xh)        dA  = ifft(i Om a psih'(a xi) xh)
+ *   D2  = ifft(-Om^2 psih_a xh)
+ * w2 = |Re((dW + q i dt A) / (i W))| / (2 pi), q = (D2 W - dW^2) / (W^2 + i dt (dW A - W dA)),
+ * where that denominator exceeds 1e-3 |W|^2 in modulus and w2 is finite; else the first-order w.
+ * Exactly one of Tx_dev, w_dev is set.  Tx_dev [B][na][N]: zeroed and accumulated here by one
+ * thread per column in ascending row order (no atomics: bit-deterministic, batch-invariant).
+ * w_dev [B][na][N] real: w2 in the data type, inf where |Wx| < gamma (as ssqb_phase_cwt).
+ * r: a CWT grid (not SSQB_GRID_STFT); only its gamma is read in w mode.                   */
+int ssqb_ssq_cwt2_reassign(int dtype, const void* Wx_dev, const void* dWx_dev, const void* A_dev,
+                           const void* dA_dev, const void* D2_dev, double dt, int64_t B, int na,
+                           int64_t N, const ssqb_reassign_desc* r, void* Tx_dev, void* w_dev,
+                           void* stream);
 /* phase_cwt_cpu / phase_cwt_gpu (algos.py:706-781); total = number of elements */
 int ssqb_phase_cwt(int dtype, const void* Wx_dev, const void* dWx_dev, void* w_dev,
                    int64_t total, double gamma, void* stream);

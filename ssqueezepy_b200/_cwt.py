@@ -78,22 +78,33 @@ class CwtPlan:
     _cache = OrderedDict()
     _CACHE_MAX = 8
 
-    def __init__(self, wavelet, scales, N, n_up, n1, padtype, dt):
+    def __init__(self, wavelet, scales, N, n_up, n1, padtype, dt, table=None):
+        """`table`: a device [na, n_up] real table of the wavelet dtype to use instead of the
+        wavelet's own samples (whole band, no overlap-save blocks)."""
         self.lib = Bk.require_cuda()
         self.dtype = wavelet.dtype
         self.N, self.n_up, self.n1 = int(N), int(n_up), int(n1)
+        self.padtype, self.dt = padtype, float(dt)
         self.na = len(scales)
         sc64 = np.ascontiguousarray(np.asarray(scales, dtype=np.float64).reshape(-1))
-        lo, ln = _band_limits(wavelet, np.asarray(scales, dtype=self.dtype), n_up)
+        if table is None:
+            lo, ln = _band_limits(wavelet, np.asarray(scales, dtype=self.dtype), n_up)
+        else:
+            lo = np.zeros(self.na, dtype=np.int64)
+            ln = np.full(self.na, n_up, dtype=np.int64)
         d = _lib.CwtDesc()
         d.dtype = Bk.dtype_code(self.dtype)
         d.N, d.n_up, d.n1 = self.N, self.n_up, self.n1
         d.padtype = _lib.PAD[padtype]
         d.na = self.na
-        spec = wavelet.device_spec()
+        spec = wavelet.device_spec() if table is None else None
         self._table = None
         self._fn_ref = wavelet.fn        # a cached plan pins the function, so its id stays unique
-        if spec is None:
+        if table is not None:
+            self._table = table
+            d.wavelet = _lib.WAV_TABLE
+            d.psih_table_dev = self._table.data_ptr()
+        elif spec is None:
             # any other wavelet: sample it once on the host exactly as the
             # reference does (`wavelet(scale=scales, nohalf=False)`, _cwt.py:171)
             sc_t = np.asarray(scales, dtype=self.dtype).reshape(-1, 1)
@@ -114,7 +125,8 @@ class CwtPlan:
         d.scales_host = sc64.ctypes.data_as(C.POINTER(C.c_double))
         d.band_lo_host = lo.ctypes.data_as(C.POINTER(C.c_int64))
         d.band_len_host = ln.ctypes.data_as(C.POINTER(C.c_int64))
-        ts = _time_supports(wavelet, np.asarray(scales, dtype=self.dtype))
+        ts = (_time_supports(wavelet, np.asarray(scales, dtype=self.dtype)) if table is None
+              else np.zeros(self.na, dtype=np.int64))
         d.tsupport_host = ts.ctypes.data_as(C.POINTER(C.c_int64))
         h = C.c_void_p()
         _lib.check(self.lib.ssqb_cwt_plan_create(C.byref(d), C.byref(h)))
@@ -189,6 +201,14 @@ class CwtPlan:
                                               Wx.data_ptr(), Bk.ptr(dWx), mul,
                                               int(bool(rpadded)), Bk.stream_ptr()))
         return Wx, dWx
+
+    def cwt_into(self, xd, Wx, dWx=None):
+        """`ssqb_cwt_exec` of the [B, N] device signals `xd` into the given contiguous
+        [B, na, N] outputs (dWx may be None)."""
+        with self._lock:
+            _lib.check(self.lib.ssqb_cwt_exec(self.handle, xd.data_ptr(), xd.shape[0],
+                                              Wx.data_ptr(), Bk.ptr(dWx), None, 0,
+                                              Bk.stream_ptr()))
 
     def ssq_cwt(self, x, get_dWx=False, get_Wx=True):
         """(Tx, Wx, dWx); Wx is None (never stored) with get_Wx=False, dWx without get_dWx."""

@@ -33,7 +33,7 @@ SYMBOLS = [
     'ssqb_ssq_stft_exec', 'ssqb_ssq_stft_exec_host', 'ssqb_ssq_stft2_exec',
     'ssqb_colsum_real', 'ssqb_invert_components', 'ssqb_istft_exec', 'ssqb_extract_ridges', 'ssqb_cwt_backward',
     'ssqb_stft_backward', 'ssqb_istft_backward', 'ssqb_ssqueeze_backward',
-    'ssqb_indexed_sum_backward', 'ssqb_colsum_real_backward',
+    'ssqb_indexed_sum_backward', 'ssqb_colsum_real_backward', 'ssqb_ssq_cwt2_reassign',
 ]
 
 
@@ -109,6 +109,8 @@ def _bind(lib):
                                               C.POINTER(ReassignDesc), vp]
     lib.ssqb_colsum_real_backward.argtypes = [ci, ci, vp, i64, ci, i64, C.POINTER(dbl), dbl, ci,
                                               vp, vp]
+    lib.ssqb_ssq_cwt2_reassign.argtypes = [ci, vp, vp, vp, vp, vp, dbl, i64, ci, i64,
+                                           C.POINTER(ReassignDesc), vp, vp, vp]
     lib.ssqb_phase_cwt.argtypes = [ci, vp, vp, vp, i64, dbl, vp]
     lib.ssqb_phase_stft.argtypes = [ci, vp, vp, vp, vp, i64, ci, i64, dbl, vp]
     lib.ssqb_stft_exec.argtypes = [C.POINTER(StftDesc), vp, i64, vp, vp, vp]

@@ -11,8 +11,9 @@ import numpy as np
 import torch
 
 from . import _lib, backend as Bk
-from ._cwt import (cwt, CwtPlan, _clean_input, _pad_geometry_for,
+from ._cwt import (cwt, CwtPlan, _CwtFn, _clean_input, _pad_geometry_for,
                    cached_process_scales, wavelet_key, _CACHE_LOCK)
+from ._ssq_cwt2 import psih_pair, order2_of
 from .algos import (phase_cwt_gpu, make_reassign_desc, colsum_real, invert_components,
                     reassign_backward)
 from .ssqueezing import (ssqueeze, _check_ssqueezing_args,
@@ -30,7 +31,7 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
             difftype='trig', difforder=None, gamma=None, vectorized=True,
             preserve_transform=None, astensor=True, order=0, nan_checks=None,
             patience=0, flipud=True, cache_wavelet=None, get_w=False,
-            get_dWx=False, get_Wx=True):
+            get_dWx=False, get_Wx=True, ssq_order=1):
     """Returns `(Tx, Wx, ssq_freqs, scales[, w][, dWx])` like the reference.
     `Tx`, `Wx` (and `w`, `dWx`) are CUDA tensors when `astensor=True`, numpy
     arrays otherwise; `ssq_freqs` is a float64 numpy array; `Wx` is never
@@ -44,7 +45,18 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
     `ssqueeze`; they compute it as usual and drop it before returning, so they
     save no peak memory, nor does `padtype=None` on a length that is not a power
     of two (its plan keeps `Wx` in a buffer of its own).  With `x.requires_grad`, `Wx` and `dWx` are still kept
-    for the backward."""
+    for the backward.
+
+    `ssq_order=2` reassigns by the second-order frequency estimate, which corrects the
+    first-order bias in proportion to the frequency modulation: exact for linear chirps.
+    The gamma test, bins, weights and `ssq_freqs` are the first order's, so the column sums
+    of `Tx` (hence `issq_cwt`) are unchanged.  Morlet and order-0 GMW (L1 or L2) wavelets
+    only (`NotImplementedError` for others), `order=0` only.  `get_w` then returns the
+    second-order `w`; with `x.requires_grad` the gradient holds every bin where the forward
+    put it, as at first order.  It costs three transforms per row and a pass over five
+    planes; a batch runs in groups of signals, so only `Tx` and `Wx` cover the whole batch."""
+    if ssq_order not in (1, 2) or isinstance(ssq_order, bool):
+        raise ValueError("`ssq_order` must be 1 or 2 (got %s)" % (ssq_order,))
     if not hasattr(x, 'ndim'):
         raise TypeError("`x` must be a numpy array or torch Tensor "
                         "(got %s)" % type(x))
@@ -53,12 +65,16 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
     difforder = _check_ssqueezing_args(squeezing, maprange, wavelet, difftype,
                                        difforder, get_w, transform='cwt')
     higher = isinstance(order, (tuple, list, range)) or order > 0
+    if ssq_order == 2 and higher:
+        raise ValueError("`ssq_order=2` needs `order=0` (got order=%s)" % (order,))
     if nv is None and not isinstance(scales, np.ndarray):
         nv = 32
     N = x.shape[-1]
     dt, fs, t = _process_fs_and_t(fs, t, N)
     wavelet = Wavelet._init_if_not_isinstance(wavelet, N=N)
     dtype = wavelet.dtype
+    if ssq_order == 2:
+        psih_pair(wavelet)                   # NotImplementedError for other wavelets
 
     scales, cwt_scaletype, *_ = cached_process_scales(scales, N, wavelet, nv)
     if gamma is None:
@@ -68,7 +84,11 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
     was_padded = bool(padtype is not None)
 
     fused = (squeezing == 'sum') and not get_w and not higher
-    if not fused:
+    if ssq_order == 2:
+        Tx, Wx, ssq_freqs, sc, w, dWx = _ssq_cwt2(
+            x, wavelet, scales, ssq_freqs, N, fs, dt, padtype, squeezing,
+            maprange, gamma, nan_checks, flipud, get_w, get_dWx, get_Wx)
+    elif not fused:
         # two-step route: cwt -> (phase transform) -> ssqueeze operator
         # (higher-order GMWs, reference _ssq_cwt.py:227-241: one transform per order,
         # averaged over a tuple of orders; the derivative is taken per order in the
@@ -130,6 +150,61 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
     elif get_dWx:
         return Tx, Wx, ssq_freqs, sc, dWx
     return Tx, Wx, ssq_freqs, sc
+
+
+def _ssq_cwt2(x, wavelet, scales, ssq_freqs, N, fs, dt, padtype, squeezing, maprange,
+              gamma, nan_checks, flipud, get_w, get_dWx, get_Wx):
+    """`ssq_cwt(..., ssq_order=2)` on every route; returns (Tx, Wx, ssq_freqs, scales, w, dWx)
+    with None for what was not asked for.  Fused (`squeezing='sum'`, no `get_w`, no grad):
+    `ssqb_ssq_cwt2_reassign` writes Tx.  Otherwise it writes the second-order w, and
+    `ssqueeze(Wx, w, ...)` reassigns; with `x.requires_grad`, Wx comes from the differentiable
+    transform and w from a detached call, so the gradient is the frozen-bin `indexed_sum`
+    backward followed by the cwt adjoint."""
+    was_padded = bool(padtype is not None)
+    dtype = wavelet.dtype
+    x = _clean_input(x, nan_checks)
+    n_up, n1, pad_kind = _pad_geometry_for(N, padtype)
+    hp = ssq_cwt_host_params(N, wavelet, scales, ssq_freqs, maprange, was_padded, dt)
+    plan = CwtPlan.get(wavelet, hp['scales'], N, n_up, n1, pad_kind, dt)
+    o2 = order2_of(plan, wavelet, dt)
+    desc = make_reassign_desc(hp['ssq_freqs'], hp['const'], plan.na, hp['logscale'], flipud,
+                              gamma, dtype)
+    xd = plan._x2d(x)
+    shape = (xd.shape[0], plan.na, N)
+    cdt, rdt = Bk.cplx_dtype(dtype), Bk.real_dtype(dtype)
+    new = lambda dt_, on=True: torch.empty(shape, dtype=dt_, device='cuda') if on else None
+    grad = torch.is_tensor(x) and x.requires_grad
+    sc = plan.scales_tensor().clone()            # fresh arrays: callers may modify them in place
+    w = None
+    if squeezing == 'sum' and not get_w and not grad:
+        Tx, Wx, dWx = new(cdt), new(cdt, get_Wx), new(cdt, get_dWx)
+        o2.run(plan, xd, desc, Tx=Tx, Wx=Wx, dWx=dWx)
+        # `scales` go high -> low, so the returned frequencies are reversed
+        f = hp['ssq_freqs']
+        ssq_freqs = f.flip(0) if Bk.is_tensor(f) else np.asarray(f)[::-1].copy()
+    else:
+        w = new(rdt)
+        if grad:
+            # the differentiable transform's own (W, dW) feed the w-only kernel
+            Wx, dWx = _CwtFn.apply(xd, plan, True, None, False)
+            o2.run(plan, xd.detach(), desc, w=w, Wx=Wx.detach(), dWx=dWx.detach(),
+                   W_given=True)
+            if not get_dWx:
+                dWx = None
+        else:
+            Wx, dWx = new(cdt), new(cdt, get_dWx)
+            o2.run(plan, xd, desc, w=w, Wx=Wx, dWx=dWx)
+        Tx, ssq_freqs = ssqueeze(Wx, w, ssq_freqs, sc,
+                                 fs=fs, squeezing=squeezing, maprange=maprange,
+                                 wavelet=wavelet, gamma=gamma, was_padded=was_padded,
+                                 flipud=flipud, transform='cwt')
+        if not get_w:
+            w = None
+    if not get_Wx:
+        Wx = None
+    if x.ndim == 1:
+        Tx, Wx, w, dWx = [None if v is None else v[0] for v in (Tx, Wx, w, dWx)]
+    return Tx, Wx, ssq_freqs, sc, w, dWx
 
 
 class _SsqCwtFn(torch.autograd.Function):

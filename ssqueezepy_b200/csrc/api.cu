@@ -169,6 +169,14 @@ int ssqb_indexed_sum_backward(int dtype, const void* w, const void* gTx, const v
                                nullptr, (cudaStream_t)stream);
 }
 
+int ssqb_ssq_cwt2_reassign(int dtype, const void* Wx, const void* dWx, const void* A,
+                           const void* dA, const void* D2, double dt, int64_t B, int na,
+                           int64_t N, const ssqb_reassign_desc* r, void* Tx, void* w,
+                           void* stream) {
+  const void* planes[5] = {Wx, dWx, A, dA, D2};
+  return run_ssq2_cwt(dtype, planes, dt, B, na, N, r, Tx, w, (cudaStream_t)stream);
+}
+
 int ssqb_phase_cwt(int dtype, const void* Wx, const void* dWx, void* w, int64_t total,
                    double gamma, void* stream) {
   return run_phase(dtype, false, Wx, dWx, nullptr, w, total, 1, 1, gamma, (cudaStream_t)stream);

@@ -190,6 +190,9 @@ int run_reassign_backward(int dtype, const void* Wx, const void* dWx, const void
                           const void* gTx, const void* gWx, void* gWout, long long B, int na,
                           long long N, const ssqb_reassign_desc* r, const void* Sfs,
                           cudaStream_t st);
+// second-order ssq_cwt reassignment; planes = {W, dW, A, dA, D2}
+int run_ssq2_cwt(int dtype, const void* const* planes, double dt, long long B, int na,
+                 long long N, const ssqb_reassign_desc* r, void* Tx, void* w, cudaStream_t st);
 int run_phase(int dtype, bool stft, const void* Wx, const void* dWx, const void* Sfs, void* out,
               long long total, long long ncols, int nrows, double gamma, cudaStream_t st);
 int run_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const void* x, long long B,

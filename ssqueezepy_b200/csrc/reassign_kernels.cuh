@@ -10,6 +10,8 @@
 //   phase_stft_kernel          <- algos.py:784-816 `_phase_stft_par`
 //   ssqueeze_bwd_kernel,
 //   indexed_sum_bwd_kernel     backward of the two reassignments for torch.autograd (bins held)
+//   ssq2_cwt_colowner_kernel   second-order ssq_cwt reassignment from five transform planes
+//                              (not in the reference)
 //
 // Layout: Wx, dWx, Tx are [B][na][N] complex (row-major); thread j of a warp reads
 // 32 consecutive complex values of a row (256/512 B, coalesced).
@@ -227,6 +229,85 @@ phase_kernel(const cx<T>* __restrict__ Wx, const cx<T>* __restrict__ dWx,
     r = (double)Sfs[i] - r;
   }
   out[idx] = (T)fabs(r);
+}
+
+// ---- second-order ssq_cwt ---------------------------------------------------------------
+// Five planes per point, of the same [B][na][N] layout:
+//   W  = ifft(psih_a xh)                dW = ifft(i Om psih_a xh)            (Om = xi / dt)
+//   A  = ifft(a psih'(a xi) xh)         dA = ifft(i Om a psih'(a xi) xh)
+//   D2 = ifft(-Om^2 psih_a xh)
+// With Wt = i dt A and dWt = i dt dA (the transform with the kernel u h_a(u) and its time
+// derivative), on a linear chirp q = (D2 W - dW^2) / Den is i phi'' and
+//   Den = W^2 + dW Wt - W dWt,   om2 = (dW + q Wt) / (i W) = phi'(b)   (rad/s)
+// w2 = |Re om2| / 2 pi where |Den|^2 > eps^2 |W|^4 and w2 is finite, else the first-order w1.
+// Every operation is one IEEE float64 rounding, in the order written (no contraction), so a
+// float64 NumPy restatement of this function gives the same bits.
+struct Z64 { double r, i; };
+__device__ __forceinline__ Z64 z64_mul(Z64 a, Z64 b) {
+  return { __dsub_rn(__dmul_rn(a.r, b.r), __dmul_rn(a.i, b.i)),
+           __dadd_rn(__dmul_rn(a.r, b.i), __dmul_rn(a.i, b.r)) };
+}
+__device__ __forceinline__ Z64 z64_add(Z64 a, Z64 b) { return { __dadd_rn(a.r, b.r), __dadd_rn(a.i, b.i) }; }
+__device__ __forceinline__ Z64 z64_sub(Z64 a, Z64 b) { return { __dsub_rn(a.r, b.r), __dsub_rn(a.i, b.i) }; }
+// i dt a
+__device__ __forceinline__ Z64 z64_idt(Z64 a, double dt) { return { -__dmul_rn(a.i, dt), __dmul_rn(a.r, dt) }; }
+template <typename T> __device__ __forceinline__ Z64 z64_of(cx<T> v) { return { (double)v.x, (double)v.y }; }
+
+#define SSQB_SSQ2_CWT_EPS2 1e-6      // (SSQB_SSQ2_EPS = 1e-3 of the STFT order 2) squared
+
+template <typename T>
+__device__ __forceinline__ double ssq2_cwt_w(cx<T> Wc, cx<T> dWc, cx<T> Ac, cx<T> dAc,
+                                             cx<T> D2c, double dt, double w1) {
+  const Z64 W = z64_of<T>(Wc), dW = z64_of<T>(dWc), A = z64_of<T>(Ac), dA = z64_of<T>(dAc);
+  const Z64 D2 = z64_of<T>(D2c);
+  const double ww = __dadd_rn(__dmul_rn(W.r, W.r), __dmul_rn(W.i, W.i));
+  const Z64 E = z64_sub(z64_mul(dW, A), z64_mul(W, dA));
+  const Z64 Den = z64_add(z64_mul(W, W), z64_idt(E, dt));
+  const double DD = __dadd_rn(__dmul_rn(Den.r, Den.r), __dmul_rn(Den.i, Den.i));
+  if (!(DD > __dmul_rn(__dmul_rn(SSQB_SSQ2_CWT_EPS2, ww), ww))) return w1;
+  const Z64 Num = z64_sub(z64_mul(D2, W), z64_mul(dW, dW));
+  const Z64 q = { __ddiv_rn(__dadd_rn(__dmul_rn(Num.r, Den.r), __dmul_rn(Num.i, Den.i)), DD),
+                  __ddiv_rn(__dsub_rn(__dmul_rn(Num.i, Den.r), __dmul_rn(Num.r, Den.i)), DD) };
+  const Z64 U = z64_add(dW, z64_idt(z64_mul(q, A), dt));
+  const double im = __ddiv_rn(__dsub_rn(__dmul_rn(U.i, W.r), __dmul_rn(U.r, W.i)),
+                              __dmul_rn(ww, SSQB_TWO_PI));
+  return isfinite(im) ? fabs(im) : w1;
+}
+
+// Column owner, grid (ceil(N / 256), B): thread j owns column j of one signal.
+// Tx mode (Tx set): zeroes its column of Tx, then walks the rows in ascending order and adds
+// const_i W at the bin of w2 (the first order's gamma test, bins and typed accumulation), so Tx
+// is bit-deterministic and independent of the batch.  w mode (w set): the real w2 plane, inf
+// where |W| < gamma (gamma in the data type, as phase_cwt).
+template <typename T>
+__global__ void __launch_bounds__(256)
+ssq2_cwt_colowner_kernel(const cx<T>* __restrict__ Wx, const cx<T>* __restrict__ dWx,
+                         const cx<T>* __restrict__ Ax, const cx<T>* __restrict__ dAx,
+                         const cx<T>* __restrict__ D2x, double dt, cx<T>* __restrict__ Tx,
+                         T* __restrict__ w, const double* __restrict__ cst, int na,
+                         long long N, const ReassignGrid g) {
+  const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= N) return;
+  const long long base = (long long)blockIdx.y * na * N + j;
+  if (Tx) {
+    for (int k = 0; k < na; ++k) Tx[base + (long long)k * N] = mkc<T>((T)0, (T)0);
+  }
+  const T gamma_t = (T)g.gamma;
+#pragma unroll 1
+  for (int i = 0; i < na; ++i) {
+    const long long o = base + (long long)i * N;
+    const cx<T> W = Wx[o];
+    if (Tx ? !is_active_exact(W.x, W.y, g.gamma) : is_below_exact(W.x, W.y, gamma_t)) {
+      if (!Tx) w[o] = t_inf<T>();
+      continue;
+    }
+    const cx<T> dW = dWx[o];
+    const double w1 = fabs(phase_ratio_exact<T>(dW.x, dW.y, W.x, W.y));
+    const double w2 = ssq2_cwt_w<T>(W, dW, Ax[o], dAx[o], D2x[o], dt, w1);
+    if (!Tx) { w[o] = (T)w2; continue; }
+    const int k = bin_from_w_exact(w2, g);
+    accumulate_exact<T>(&Tx[base + (long long)k * N], W, cst[i], g.const_wide);
+  }
 }
 
 }  // namespace ssqb

@@ -131,6 +131,39 @@ int run_reassign_backward(int dtype, const void* Wx, const void* dWx, const void
 }
 
 template <typename T>
+static int ssq2_cwt_t(const void* const* planes, double dt, long long B, int na, long long N,
+                      const ssqb_reassign_desc* r, void* Tx, void* w, cudaStream_t st) {
+  ReassignGrid g;
+  int rc = fill_grid(r, na, &g); if (rc) return rc;
+  if (g.kind == 3) return set_error(SSQB_E_ARG, "SSQB_GRID_STFT is not a CWT grid");
+  if (B > 65535) return set_error(SSQB_E_UNSUPP, "batch of %lld > 65535", B);
+  double* cst = nullptr;
+  if (Tx) {
+    SSQB_CUDA(cudaMallocAsync((void**)&cst, sizeof(double) * na, st));
+    SSQB_CUDA(cudaMemcpyAsync(cst, r->cst_host, sizeof(double) * na, cudaMemcpyHostToDevice, st));
+  }
+  dim3 grid((unsigned)((N + 255) / 256), (unsigned)B);
+  ssq2_cwt_colowner_kernel<T><<<grid, 256, 0, st>>>(
+      (const cx<T>*)planes[0], (const cx<T>*)planes[1], (const cx<T>*)planes[2],
+      (const cx<T>*)planes[3], (const cx<T>*)planes[4], dt, (cx<T>*)Tx, (T*)w, cst, na, N, g);
+  SSQB_LAUNCH_CHECK();
+  if (cst) SSQB_CUDA(cudaFreeAsync(cst, st));
+  return 0;
+}
+
+int run_ssq2_cwt(int dtype, const void* const* planes, double dt, long long B, int na,
+                 long long N, const ssqb_reassign_desc* r, void* Tx, void* w, cudaStream_t st) {
+  for (int p = 0; p < 5; ++p)
+    if (!planes[p]) return set_error(SSQB_E_ARG, "null plane %d", p);
+  if (!r || (Tx && !r->cst_host)) return set_error(SSQB_E_ARG, "null reassign descriptor");
+  if ((Tx == nullptr) == (w == nullptr)) return set_error(SSQB_E_ARG, "exactly one of Tx, w");
+  if (B < 1 || na < 1 || N < 1) return set_error(SSQB_E_ARG, "bad shape");
+  if (!(dt > 0)) return set_error(SSQB_E_ARG, "dt must be > 0");
+  return dtype == SSQB_F32 ? ssq2_cwt_t<float>(planes, dt, B, na, N, r, Tx, w, st)
+                           : ssq2_cwt_t<double>(planes, dt, B, na, N, r, Tx, w, st);
+}
+
+template <typename T>
 static int phase_t(bool stft, const void* Wx, const void* dWx, const void* Sfs, void* out,
                    long long total, long long ncols, int nrows, double gamma, cudaStream_t st) {
   unsigned blocks = (unsigned)((total + 255) / 256);
