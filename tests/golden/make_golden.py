@@ -30,6 +30,10 @@ Fixtures (all inputs are seeded; see `_signal`):
                        (`python make_golden.py ridges`)
   experimental.npz     experimental.phase_ssqueeze (fused / two-step / flipud; CWT and STFT)
                        on the stored `Wx, dWx` / `Sx, dSx`
+  table_wavelets.npz   bump / cmhat / hhhat values, sampled tables, host scales and ssq_freqs
+                       ('log', 'log-piecewise', 'linear'), cwt and ssq_cwt at N=1500, nv=8
+                       (rows as +-1 projections and norms, Tx as column sums)
+                       (`python make_golden.py table`)
 """
 import os
 import sys
@@ -352,6 +356,58 @@ def gen_gmw_variants():
     save('gmw_variants', **out)
 
 
+# host-table wavelets (no device evaluation): name -> (spec, parameters), defaults and one other set
+TABLE_WAVELETS = {'bump': ('bump', {}), 'bump_m3': ('bump', dict(mu=3, s=.5)),
+                  'cmhat': ('cmhat', {}), 'cmhat_m2': ('cmhat', dict(mu=2, s=.7)),
+                  'hhhat': ('hhhat', {}), 'hhhat_m2': ('hhhat', dict(mu=2))}
+TABLE_SCALES = np.array([.7, 2., 9., 40.])
+
+
+def gen_table_wavelets():
+    """bump / cmhat / hhhat: function values, sampled tables, host scales and `ssq_freqs`, and
+    cwt / ssq_cwt outputs (`python make_golden.py table`)."""
+    out = {'w': np.linspace(-2, 14, 1601)}
+    for dtype in ('float32', 'float64'):
+        for tag, (name, opts) in TABLE_WAVELETS.items():
+            wav = Wavelet((name, dict(opts, dtype=dtype)))
+            out[f'fn_{tag}_{dtype}'] = np.asarray(wav.fn(out['w'].astype(dtype)))
+            for n in (512, 511):
+                out[f'tab_{tag}_{dtype}_{n}'] = np.asarray(wav(
+                    scale=TABLE_SCALES.astype(dtype).reshape(-1, 1), N=n, nohalf=False))
+    # scales and ssq_freqs as ssq_cwt derives them (float32 wavelets)
+    N = 2000
+    x = _signal(N, 41, 'float32')
+    for tag, (name, opts) in TABLE_WAVELETS.items():
+        for st in ('log', 'log-piecewise', 'linear'):
+            _, _, fr, sc = ssq_cwt(x, (name, dict(opts)), scales=st, nv=16)
+            out[f'hp_scales_{tag}_{st}'] = np.asarray(sc)
+            out[f'hp_freqs_{tag}_{st}'] = np.ascontiguousarray(fr)
+    out['hp_N'] = np.array([N])
+    # transforms: chirp + noise, N = 1500, 'log' scales with nv = 8.  To keep the file small,
+    # every row of Wx and dWx is stored as NPROJ fixed +-1 projections and its 2-norm (as the
+    # BASELINE-shape fixtures are, make_golden_shapes.py), and Tx as its column sums
+    from make_golden_shapes import signs, reduce_plane
+    N = 1500
+    R = signs(N)
+    out['sign_seed'] = np.array([99])
+    for dtype in ('float32', 'float64'):
+        for k, name in enumerate(('bump', 'cmhat', 'hhhat')):
+            batch = dtype == 'float32' and name == 'cmhat'
+            x = (np.stack([_signal(N, 50 + k + b, dtype) for b in range(2)]) if batch
+                 else _signal(N, 50 + k, dtype))
+            wav = Wavelet((name, {'dtype': dtype}))
+            Tx, _, fr, sc = ssq_cwt(x, wav, scales='log', nv=8)
+            Wx, _, dWx = cwt(x, wav, scales=sc, derivative=True)
+            tag = f'{name}_{dtype}'
+            for key, plane in (('Wx', Wx), ('dWx', dWx)):
+                red = [reduce_plane(p, R) for p in plane.reshape(-1, len(sc), N)]
+                out[f'{key}_proj_{tag}'] = np.stack([r[0] for r in red])
+                out[f'{key}_norm_{tag}'] = np.stack([r[1] for r in red])
+            out.update({f'x_{tag}': x, f'Txsum_{tag}': Tx.sum(-2),
+                        f'freqs_{tag}': np.ascontiguousarray(fr), f'scales_{tag}': sc})
+    save('table_wavelets', **out)
+
+
 def gen_ridges():
     """extract_ridges (ridge_extraction.py:11-146, serial kernels: `parallel=False`) on the
     stored synchrosqueezed planes and on an STFT; `python make_golden.py ridges`."""
@@ -388,6 +444,9 @@ if __name__ == '__main__':
     if sys.argv[1:] == ['ridges']:
         gen_ridges()
         sys.exit(0)
+    if sys.argv[1:] == ['table']:
+        gen_table_wavelets()
+        sys.exit(0)
     gen_cwt('cwt_morlet_f32', 'morlet', 1500, 48, 'float32')
     gen_cwt('cwt_gmw_f64', ('gmw', {'beta': 12, 'gamma': 3, 'dtype': 'float64'}),
             1000, 40, 'float64', fs=2.0)
@@ -406,3 +465,4 @@ if __name__ == '__main__':
     gen_inverse()
     gen_experimental()
     gen_gmw_variants()
+    gen_table_wavelets()

@@ -26,7 +26,8 @@ GMW = {'beta': 12, 'gamma': 3}
 # sampled on the host into a table (`Wavelet.device_spec() is None`)
 WAVELETS = {'morlet': ('morlet', {}), 'gmw': ('gmw', GMW), 'gmw60': ('gmw', {}),
             'gmw_l2': ('gmw', dict(GMW, norm='energy')), 'gmw_k1': ('gmw', dict(GMW, order=1)),
-            'gmw_k2': ('gmw', dict(GMW, order=2))}
+            'gmw_k2': ('gmw', dict(GMW, order=2)),
+            'bump': ('bump', {}), 'cmhat': ('cmhat', {}), 'hhhat': ('hhhat', {})}
 
 
 def _custom(w):
@@ -218,6 +219,9 @@ GRAD_CASES = [
     ('custom', 'wrap', 1500, 3, 'on', 1., False),
     ('custom', 'symmetric', 10, 1, 'dW', 2.5, True),
     ('custom', None, 97, 3, 'off', 1., False),
+    ('bump', 'reflect', 700, 3, 'on', 2.5, False),
+    ('cmhat', None, 97, 1, 'on', 1., False),
+    ('hhhat', 'zero', 1500, 1, 'dW', 1., True),
 ]
 
 
