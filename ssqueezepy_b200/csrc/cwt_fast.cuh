@@ -181,9 +181,9 @@ __device__ __forceinline__ void ssq_num_den(float2 W, float2 dW, float& num, flo
   num = sub_rn(q.x, q.y);
 }
 
-// flush-to-zero MUFU forms: denormal inputs / results behave as 0 (bin 0 after the
-// clamp, which is also what the exact formula gives for w < 2^-126 on the grids that
-// fill_grid admits to the fast path)
+// flush-to-zero MUFU forms: denormal inputs / results behave as 0.  A quotient of 0 (a
+// subnormal num, a divisor >= 2^126, an underflowing w) is never trusted: those points take
+// ssq_point_exact (w_estimate_ok, ssq_common.cuh)
 __device__ __forceinline__ float fdiv_ftz(float a, float b) {
   float r; asm("div.approx.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r;
 }
@@ -207,7 +207,7 @@ __device__ __forceinline__ bool ssq_point_fast(cx<T> W, cx<T> dW, cx<T>* __restr
   else                wf = (float)(fabs((double)num) / ((double)den * SSQB_TWO_PI));
   const float lf = lg2_ftz(wf);
   float v;
-  bool ok = fast_ok && (den > g2hi);
+  bool ok = fast_ok && (den > g2hi) && w_estimate_ok(wf);
   if (g.kind == 0) {
     v = (lf - g.fa0) * g.fid0;
   } else {
@@ -459,11 +459,8 @@ __device__ __forceinline__ void cwt_rows_body(const FastArgs<T>& P) {
   } else if (NARR == 2) {
     const double cwide = A.cst[a];
     const T cre = (T)cwide;
-    const T g2 = (T)(A.grid.gamma * A.grid.gamma);
-    const T g2tol = g2 * (T)(sizeof(T) == 4 ? 1e-5 : 1e-13);
-    const T g2lo = g2 - g2tol;
-    // fast path only for den clear of gamma^2 AND of the flush-to-zero range
-    const T g2hi = fmax(g2 + g2tol, (T)1e-30);
+    T g2lo, g2hi;
+    fast_gamma_band<T>(A.grid.gamma, g2lo, g2hi);
     const bool fast_ok = (A.grid.kind <= 1) && (A.grid.ftol < 0.25f);
     const unsigned rowbytes = (unsigned)Nout * (unsigned)sizeof(cx<T>);
     cx<T>* __restrict__ Zrow = (sig < A.zero_next) ? A.Tx + row * A.Nout + A.zero_off : nullptr;

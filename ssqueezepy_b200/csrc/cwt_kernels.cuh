@@ -252,17 +252,15 @@ template <> __device__ __forceinline__ void atomic_add_cx<double>(double2* p, do
 }
 
 // |W| > gamma with the reference's typing; cheap test + exact test in a guard band
-__device__ __forceinline__ bool is_active_fast(float C, float D, double gamma) {
-  float dd = C * C + D * D;
-  float g2 = (float)(gamma * gamma);
-  if (fabsf(dd - g2) <= 1e-5f * g2) return is_active_exact(C, D, gamma);
-  return dd > g2;
-}
-__device__ __forceinline__ bool is_active_fast(double C, double D, double gamma) {
-  double dd = C * C + D * D;
-  double g2 = gamma * gamma;
-  if (fabs(dd - g2) <= 1e-13 * g2) return is_active_exact(C, D, gamma);
-  return dd > g2;
+// (fast_gamma_band, the band of the row kernels)
+template <typename T>
+__device__ __forceinline__ bool is_active_fast(T C, T D, double gamma) {
+  T g2lo, g2hi;
+  fast_gamma_band<T>(gamma, g2lo, g2hi);
+  const T dd = C * C + D * D;
+  if (dd < g2lo) return false;
+  if (dd > g2hi) return true;
+  return is_active_exact(C, D, gamma);
 }
 
 template <typename T, int LOG_F, int NARR, int EPI>
@@ -342,7 +340,7 @@ cwt_pass2_kernel(const CwtArgs<T> A, const int write_dWx) {
       if (EPI == EPI_SSQ) A.Wx[o] = W;
       if (write_dWx) A.dWx[o] = dW;
       if (b < A.zero_next) A.Tx[o + A.zero_off] = mkc<T>((T)0, (T)0);
-      if (is_active_fast(W.x, W.y, A.grid.gamma)) {
+      if (is_active_fast<T>(W.x, W.y, A.grid.gamma)) {
         int k = bin_fused<T>(dW.x, dW.y, W.x, W.y, A.grid);
         T re, im;
         if (A.grid.const_wide) {

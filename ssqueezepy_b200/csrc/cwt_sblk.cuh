@@ -341,10 +341,7 @@ __device__ __forceinline__ void sblk_rows_body(const SblkArgs<T>& S) {
     T g2lo = 0, g2hi = 0; bool fast_ok = false; unsigned rowbytes = 0;
     if (SSQ) {
       cwide = A.cst[a]; cre = (T)cwide;
-      const T g2 = (T)(A.grid.gamma * A.grid.gamma);
-      const T g2tol = g2 * (T)(sizeof(T) == 4 ? 1e-5 : 1e-13);
-      g2lo = g2 - g2tol;
-      g2hi = fmax(g2 + g2tol, (T)1e-30);
+      fast_gamma_band<T>(A.grid.gamma, g2lo, g2hi);
       fast_ok = (A.grid.kind <= 1) && (A.grid.ftol < 0.25f);
       rowbytes = (unsigned)Nout * (unsigned)sizeof(cx<T>);
     }

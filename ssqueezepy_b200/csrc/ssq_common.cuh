@@ -194,15 +194,35 @@ __device__ __forceinline__ float w_estimate(double num, double den) {
   return (float)(fabs(num) / (den * SSQB_TWO_PI));
 }
 
+// The range in which the fused paths' shortcuts hold (tests/test_gpu_range_edges.py):
+// - the bin estimate needs den > 1e-30 (normal products, and a normal divisor for the
+//   flush-to-zero division) and a normal float32 quotient w.  The flush-to-zero division
+//   returns 0 for a divisor >= 2^126 (|Wx| >= 2^61.7) and for a subnormal num; IEEE division
+//   returns 0 once den * 2 pi overflows (|Wx| >= 2^62.9); a subnormal w has lost the bits the
+//   error bound `ftol` assumes.  Every such point takes the exact formula.
+// - the cheap activity test (den against gamma^2 in a relative band of 1e-5 / 1e-13) needs
+//   (T)gamma^2 >= 2^-120: below that the band underflows and a den near gamma^2 is made of
+//   subnormal products.  There g2lo = 0, so no point leaves early as inactive, and the
+//   1e-30 floor of g2hi sends every den <= g2hi to the exact test.
+// den < g2lo: inactive; den > g2hi: active; in between the exact test decides.
+template <typename T>
+__device__ __forceinline__ void fast_gamma_band(double gamma, T& g2lo, T& g2hi) {
+  const T g2 = (T)(gamma * gamma);
+  const T g2tol = g2 * (T)(sizeof(T) == 4 ? 1e-5 : 1e-13);
+  g2lo = (g2 >= (T)0x1p-120) ? g2 - g2tol : (T)0;
+  g2hi = fmax(g2 + g2tol, (T)1e-30);
+}
+__device__ __forceinline__ bool w_estimate_ok(float wf) { return wf >= 0x1p-126f; }
+
 template <typename T>
 __device__ __forceinline__ int bin_fused(T A, T B, T C, T D, const ReassignGrid& g) {
   T num = sub_rn(mul_rn(B, C), mul_rn(A, D));
   T den = add_rn(mul_rn(C, C), mul_rn(D, D));
-  if (g.kind <= 1 && g.ftol < 0.25f) {
+  if (g.kind <= 1 && g.ftol < 0.25f && den > (T)1e-30) {
     float wf = w_estimate(num, den);
     float lf = __log2f(wf);
     float v;
-    bool ok = true;
+    bool ok = w_estimate_ok(wf);
     int k = 0;
     if (g.kind == 0) {
       v = (lf - g.fa0) * g.fid0;
