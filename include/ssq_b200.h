@@ -144,6 +144,20 @@ int ssqb_cwt_debug_xh(ssqb_cwt_plan* plan, const void* x_dev, int64_t B,
 int ssqb_cwt_backward(ssqb_cwt_plan* plan, const void* gWx_dev, const void* gdWx_dev, int64_t B,
                       const double* out_mul_host, int rpadded, void* gx_dev, void* stream);
 
+/* time-decimated forms of the three calls above: every plane of the call ([B][na][..] Wx, dWx,
+ * Tx and their gradients) holds only the columns j * hop, j < Nh = (N - 1) / hop + 1, i.e. the
+ * full call's plane[..., ::hop], bit for bit for Wx / dWx (Tx: the same bins, atomic order aside).
+ * hop >= 1 (hop = 1 is the call above; hop >= N leaves one column), rpadded must be 0 when
+ * hop > 1; SSQB_E_ARG otherwise.                                                       */
+int ssqb_cwt_exec_hop(ssqb_cwt_plan* plan, const void* x_dev, int64_t B,
+                      void* Wx_dev, void* dWx_dev, const double* out_mul_host,
+                      int rpadded, int64_t hop, void* stream);
+int ssqb_ssq_cwt_exec_hop(ssqb_cwt_plan* plan, const void* x_dev, int64_t B,
+                          void* Wx_dev, void* Tx_dev, void* dWx_dev, int64_t hop, void* stream);
+int ssqb_cwt_backward_hop(ssqb_cwt_plan* plan, const void* gWx_dev, const void* gdWx_dev,
+                          int64_t B, const double* out_mul_host, int rpadded, int64_t hop,
+                          void* gx_dev, void* stream);
+
 /* measurement hook (bench.py roofline): when on, CUDA events are recorded on the
  * launch stream around every kernel group; get_profile sums them per kind
  * k = 0 forward-FFT passes, 1 pass 1 of the two-pass rows, 2 row kernels (direct /

@@ -185,10 +185,15 @@ class CwtPlan:
         xd = Bk.to_device(x, self.dtype)
         return xd if xd.ndim == 2 else xd.unsqueeze(0)
 
-    def cwt(self, x, derivative=False, out_mul=None, rpadded=False):
+    def n_cols(self, hop=1):
+        """Columns of an unpadded output plane of a call with `hop`: (N - 1) // hop + 1."""
+        return (self.N - 1) // hop + 1
+
+    def cwt(self, x, derivative=False, out_mul=None, rpadded=False, hop_len=1):
+        hop = check_hop_len(hop_len, rpadded)
         xd = self._x2d(x)
         B = xd.shape[0]
-        Nout = self.n_up if rpadded else self.N
+        Nout = self.n_up if rpadded else self.n_cols(hop)
         cdt = Bk.cplx_dtype(self.dtype)
         Wx = torch.empty((B, self.na, Nout), dtype=cdt, device='cuda')
         dWx = torch.empty_like(Wx) if derivative else None
@@ -197,32 +202,35 @@ class CwtPlan:
             mul_arr = np.ascontiguousarray(out_mul, dtype=np.float64)
             mul = mul_arr.ctypes.data_as(C.POINTER(C.c_double))
         with self._lock:
-            _lib.check(self.lib.ssqb_cwt_exec(self.handle, xd.data_ptr(), B,
-                                              Wx.data_ptr(), Bk.ptr(dWx), mul,
-                                              int(bool(rpadded)), Bk.stream_ptr()))
+            _lib.check(self.lib.ssqb_cwt_exec_hop(self.handle, xd.data_ptr(), B,
+                                                  Wx.data_ptr(), Bk.ptr(dWx), mul,
+                                                  int(bool(rpadded)), hop, Bk.stream_ptr()))
         return Wx, dWx
 
-    def cwt_into(self, xd, Wx, dWx=None):
-        """`ssqb_cwt_exec` of the [B, N] device signals `xd` into the given contiguous
-        [B, na, N] outputs (dWx may be None)."""
+    def cwt_into(self, xd, Wx, dWx=None, hop_len=1):
+        """`ssqb_cwt_exec_hop` of the [B, N] device signals `xd` into the given contiguous
+        [B, na, (N - 1) // hop_len + 1] outputs (dWx may be None)."""
+        hop = check_hop_len(hop_len)
         with self._lock:
-            _lib.check(self.lib.ssqb_cwt_exec(self.handle, xd.data_ptr(), xd.shape[0],
-                                              Wx.data_ptr(), Bk.ptr(dWx), None, 0,
-                                              Bk.stream_ptr()))
+            _lib.check(self.lib.ssqb_cwt_exec_hop(self.handle, xd.data_ptr(), xd.shape[0],
+                                                  Wx.data_ptr(), Bk.ptr(dWx), None, 0, hop,
+                                                  Bk.stream_ptr()))
 
-    def ssq_cwt(self, x, get_dWx=False, get_Wx=True):
-        """(Tx, Wx, dWx); Wx is None (never stored) with get_Wx=False, dWx without get_dWx."""
+    def ssq_cwt(self, x, get_dWx=False, get_Wx=True, hop_len=1):
+        """(Tx, Wx, dWx); Wx is None (never stored) with get_Wx=False, dWx without get_dWx.
+        Every plane holds the columns j * hop_len only."""
+        hop = check_hop_len(hop_len)
         xd = self._x2d(x)
         B = xd.shape[0]
         cdt = Bk.cplx_dtype(self.dtype)
-        shape = (B, self.na, self.N)
+        shape = (B, self.na, self.n_cols(hop))
         Wx = torch.empty(shape, dtype=cdt, device='cuda') if get_Wx else None
         Tx = torch.empty(shape, dtype=cdt, device='cuda')
         dWx = torch.empty_like(Tx) if get_dWx else None
         with self._lock:
-            _lib.check(self.lib.ssqb_ssq_cwt_exec(self.handle, xd.data_ptr(), B,
-                                                  Bk.ptr(Wx), Tx.data_ptr(),
-                                                  Bk.ptr(dWx), Bk.stream_ptr()))
+            _lib.check(self.lib.ssqb_ssq_cwt_exec_hop(self.handle, xd.data_ptr(), B,
+                                                      Bk.ptr(Wx), Tx.data_ptr(),
+                                                      Bk.ptr(dWx), hop, Bk.stream_ptr()))
         return Tx, Wx, dWx
 
     def debug_xh(self, x):
@@ -324,12 +332,12 @@ class _CwtFn(torch.autograd.Function):
     reach Wx or dWx arrives as None and is passed to the library as NULL."""
 
     @staticmethod
-    def forward(ctx, x2d, plan, derivative, out_mul, rpadded):
+    def forward(ctx, x2d, plan, derivative, out_mul, rpadded, hop):
         ctx.set_materialize_grads(False)
-        ctx.plan, ctx.out_mul, ctx.rpadded = plan, out_mul, rpadded
+        ctx.plan, ctx.out_mul, ctx.rpadded, ctx.hop = plan, out_mul, rpadded, hop
         ctx.derivative = derivative
         Wx, dWx = plan.cwt(x2d.detach(), derivative=derivative, out_mul=out_mul,
-                           rpadded=rpadded)
+                           rpadded=rpadded, hop_len=hop)
         if derivative:
             return Wx, dWx
         return Wx
@@ -337,7 +345,7 @@ class _CwtFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gW, gdW=None):
         if gW is None and gdW is None:
-            return None, None, None, None, None
+            return None, None, None, None, None, None
         plan = ctx.plan
         cdt = Bk.cplx_dtype(plan.dtype)
         gW = None if gW is None else gW.to(cdt).contiguous()
@@ -349,25 +357,40 @@ class _CwtFn(torch.autograd.Function):
             mul_arr = np.ascontiguousarray(ctx.out_mul, dtype=np.float64)
             mul = mul_arr.ctypes.data_as(C.POINTER(C.c_double))
         with plan._lock:
-            _lib.check(plan.lib.ssqb_cwt_backward(plan.handle, Bk.ptr(gW), Bk.ptr(gdW), B, mul,
-                                                  int(bool(ctx.rpadded)), gx.data_ptr(),
-                                                  Bk.stream_ptr()))
-        return gx, None, None, None, None
+            _lib.check(plan.lib.ssqb_cwt_backward_hop(plan.handle, Bk.ptr(gW), Bk.ptr(gdW), B,
+                                                      mul, int(bool(ctx.rpadded)), ctx.hop,
+                                                      gx.data_ptr(), Bk.stream_ptr()))
+        return gx, None, None, None, None, None
+
+
+def check_hop_len(hop_len, rpadded=False):
+    """`hop_len` of `cwt` / `ssq_cwt`: an int >= 1 (not a bool), and 1 with `rpadded=True`."""
+    if (isinstance(hop_len, bool) or not isinstance(hop_len, (int, np.integer))
+            or hop_len < 1):
+        raise ValueError("`hop_len` must be an int >= 1 (got %r)" % (hop_len,))
+    if rpadded and hop_len > 1:
+        raise ValueError("`rpadded=True` needs `hop_len=1` (got %s)" % hop_len)
+    return int(hop_len)
 
 
 def cwt(x, wavelet='gmw', scales='log-piecewise', fs=None, t=None, nv=32,
         l1_norm=True, derivative=False, padtype='reflect', rpadded=False,
         vectorized=True, astensor=True, cache_wavelet=None, order=0, average=None,
-        nan_checks=None, patience=0):
+        nan_checks=None, patience=0, hop_len=1):
     """CWT of `x` ([N] or [B, N]; numpy or torch).  Returns `(Wx, scales)` or
     `(Wx, scales, dWx)`; `Wx` is [na, N] / [B, na, N] complex64/128 in the
     precision of `wavelet.dtype`.  `vectorized`, `cache_wavelet`, `patience` are
     accepted for compatibility and have no effect (plans and device tables are
-    cached internally)."""
+    cached internally).
+
+    `hop_len=h` computes and stores only every h-th column: `Wx` (and `dWx`) have
+    `(N - 1) // h + 1` columns and equal the full transform's `[..., ::h]` bit for bit,
+    at a fraction of its memory and HBM traffic.  Not with `rpadded=True`."""
+    hop_len = check_hop_len(hop_len, rpadded)
     if isinstance(order, (tuple, list, range)) or order > 0:
         kw = dict(wavelet=wavelet, scales=scales, fs=fs, t=t, nv=nv, l1_norm=l1_norm,
                   derivative=derivative, padtype=padtype, rpadded=rpadded,
-                  nan_checks=nan_checks)
+                  nan_checks=nan_checks, hop_len=hop_len)
         return cwt_higher_order(x, order=order, average=average, astensor=astensor, **kw)
     x = _clean_input(x, nan_checks)
     if not isinstance(scales, str):
@@ -388,10 +411,10 @@ def cwt(x, wavelet='gmw', scales='log-piecewise', fs=None, t=None, nv=32,
     rp = bool(rpadded and padtype is not None)
     if torch.is_tensor(x) and x.requires_grad:
         x2 = plan._x2d(x)                       # differentiable cast / move / reshape
-        out = _CwtFn.apply(x2, plan, bool(derivative), out_mul, rp)
+        out = _CwtFn.apply(x2, plan, bool(derivative), out_mul, rp, hop_len)
         Wx, dWx = out if derivative else (out, None)
     else:
-        Wx, dWx = plan.cwt(x, derivative=derivative, out_mul=out_mul, rpadded=rp)
+        Wx, dWx = plan.cwt(x, derivative=derivative, out_mul=out_mul, rpadded=rp, hop_len=hop_len)
     if not is_2D:
         Wx = Wx[0]
         dWx = dWx[0] if derivative else None

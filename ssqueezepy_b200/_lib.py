@@ -34,6 +34,7 @@ SYMBOLS = [
     'ssqb_colsum_real', 'ssqb_invert_components', 'ssqb_istft_exec', 'ssqb_extract_ridges', 'ssqb_cwt_backward',
     'ssqb_stft_backward', 'ssqb_istft_backward', 'ssqb_ssqueeze_backward',
     'ssqb_indexed_sum_backward', 'ssqb_colsum_real_backward', 'ssqb_ssq_cwt2_reassign',
+    'ssqb_cwt_exec_hop', 'ssqb_ssq_cwt_exec_hop', 'ssqb_cwt_backward_hop',
 ]
 
 
@@ -96,6 +97,9 @@ def _bind(lib):
     lib.ssqb_ssq_cwt_exec_host.argtypes = [vp, vp, i64, vp, vp, vp, vp]
     lib.ssqb_cwt_debug_xh.argtypes = [vp, vp, i64, vp, vp]
     lib.ssqb_cwt_backward.argtypes = [vp, vp, vp, i64, C.POINTER(dbl), ci, vp, vp]
+    lib.ssqb_cwt_exec_hop.argtypes = [vp, vp, i64, vp, vp, C.POINTER(dbl), ci, i64, vp]
+    lib.ssqb_ssq_cwt_exec_hop.argtypes = [vp, vp, i64, vp, vp, vp, i64, vp]
+    lib.ssqb_cwt_backward_hop.argtypes = [vp, vp, vp, i64, C.POINTER(dbl), ci, i64, vp, vp]
     lib.ssqb_cwt_plan_set_profiling.argtypes = [vp, ci]
     lib.ssqb_cwt_plan_get_profile.argtypes = [vp, C.POINTER(dbl), C.POINTER(C.c_longlong),
                                               C.POINTER(C.c_longlong)]

@@ -12,7 +12,7 @@ import torch
 
 from . import _lib, backend as Bk
 from ._cwt import (cwt, CwtPlan, _CwtFn, _clean_input, _pad_geometry_for,
-                   cached_process_scales, wavelet_key, _CACHE_LOCK)
+                   cached_process_scales, wavelet_key, check_hop_len, _CACHE_LOCK)
 from ._ssq_cwt2 import psih_pair, order2_of
 from .algos import (phase_cwt_gpu, make_reassign_desc, colsum_real, invert_components,
                     reassign_backward)
@@ -31,7 +31,7 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
             difftype='trig', difforder=None, gamma=None, vectorized=True,
             preserve_transform=None, astensor=True, order=0, nan_checks=None,
             patience=0, flipud=True, cache_wavelet=None, get_w=False,
-            get_dWx=False, get_Wx=True, ssq_order=1):
+            get_dWx=False, get_Wx=True, ssq_order=1, hop_len=1):
     """Returns `(Tx, Wx, ssq_freqs, scales[, w][, dWx])` like the reference.
     `Tx`, `Wx` (and `w`, `dWx`) are CUDA tensors when `astensor=True`, numpy
     arrays otherwise; `ssq_freqs` is a float64 numpy array; `Wx` is never
@@ -54,9 +54,16 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
     only (`NotImplementedError` for others), `order=0` only.  `get_w` then returns the
     second-order `w`; with `x.requires_grad` the gradient holds every bin where the forward
     put it, as at first order.  It costs three transforms per row and a pass over five
-    planes; a batch runs in groups of signals, so only `Tx` and `Wx` cover the whole batch."""
+    planes; a batch runs in groups of signals, so only `Tx` and `Wx` cover the whole batch.
+
+    `hop_len=h` computes and stores only every h-th column of every plane (`Tx`, `Wx`, `w`,
+    `dWx`: `(N - 1) // h + 1` columns), on every route: synchrosqueezing works column by
+    column, so they are the full call's planes `[..., ::h]` (`Wx` and `dWx` bit for bit; `Tx`
+    with the same bins, up to the order of the atomic sums).  `ssq_freqs` and `scales` are
+    those of the full call."""
     if ssq_order not in (1, 2) or isinstance(ssq_order, bool):
         raise ValueError("`ssq_order` must be 1 or 2 (got %s)" % (ssq_order,))
+    hop_len = check_hop_len(hop_len)
     if not hasattr(x, 'ndim'):
         raise TypeError("`x` must be a numpy array or torch Tensor "
                         "(got %s)" % type(x))
@@ -87,7 +94,7 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
     if ssq_order == 2:
         Tx, Wx, ssq_freqs, sc, w, dWx = _ssq_cwt2(
             x, wavelet, scales, ssq_freqs, N, fs, dt, padtype, squeezing,
-            maprange, gamma, nan_checks, flipud, get_w, get_dWx, get_Wx)
+            maprange, gamma, nan_checks, flipud, get_w, get_dWx, get_Wx, hop_len)
     elif not fused:
         # two-step route: cwt -> (phase transform) -> ssqueeze operator
         # (higher-order GMWs, reference _ssq_cwt.py:227-241: one transform per order,
@@ -97,12 +104,13 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
         Wx, sc, dWx = cwt(x, wavelet, scales=scales, fs=fs, nv=nv, l1_norm=True,
                           derivative=True, padtype=padtype, astensor=True,
                           nan_checks=nan_checks, order=order if higher else 0,
-                          average=isinstance(order, (tuple, list, range)) if higher else None)
+                          average=isinstance(order, (tuple, list, range)) if higher else None,
+                          hop_len=hop_len)
         w = phase_cwt(Wx, dWx, difftype, gamma) if get_w else None
         Tx, ssq_freqs = ssqueeze(Wx, w, ssq_freqs, sc, fs=fs, squeezing=squeezing,
                                  maprange=maprange, wavelet=wavelet, gamma=gamma,
                                  was_padded=was_padded, flipud=flipud,
-                                 dWx=None if get_w else dWx, transform='cwt')
+                                 dWx=None if get_w else dWx, transform='cwt', N=N)
         if not get_dWx:
             dWx = None
         if not get_Wx:
@@ -120,13 +128,13 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
         key = (np.asarray(ssq_freqs).tobytes(), np.asarray(const).tobytes(),
                logscale, bool(flipud), float(gamma))
         if torch.is_tensor(x) and x.requires_grad:
-            Tx, Wx, dWx = _SsqCwtFn.apply(plan._x2d(x), plan, desc, key)
+            Tx, Wx, dWx = _SsqCwtFn.apply(plan._x2d(x), plan, desc, key, hop_len)
             dWx = dWx if get_dWx else None
             Wx = Wx if get_Wx else None       # the backward keeps its own reference
         else:
             with plan._lock:                 # grid + launch belong together
                 plan.set_reassign(desc, key)
-                Tx, Wx, dWx = plan.ssq_cwt(x, get_dWx=get_dWx, get_Wx=get_Wx)
+                Tx, Wx, dWx = plan.ssq_cwt(x, get_dWx=get_dWx, get_Wx=get_Wx, hop_len=hop_len)
         if x.ndim == 1:
             Tx = Tx[0]
             Wx = Wx[0] if get_Wx else None
@@ -153,7 +161,7 @@ def ssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
 
 
 def _ssq_cwt2(x, wavelet, scales, ssq_freqs, N, fs, dt, padtype, squeezing, maprange,
-              gamma, nan_checks, flipud, get_w, get_dWx, get_Wx):
+              gamma, nan_checks, flipud, get_w, get_dWx, get_Wx, hop_len=1):
     """`ssq_cwt(..., ssq_order=2)` on every route; returns (Tx, Wx, ssq_freqs, scales, w, dWx)
     with None for what was not asked for.  Fused (`squeezing='sum'`, no `get_w`, no grad):
     `ssqb_ssq_cwt2_reassign` writes Tx.  Otherwise it writes the second-order w, and
@@ -170,7 +178,7 @@ def _ssq_cwt2(x, wavelet, scales, ssq_freqs, N, fs, dt, padtype, squeezing, mapr
     desc = make_reassign_desc(hp['ssq_freqs'], hp['const'], plan.na, hp['logscale'], flipud,
                               gamma, dtype)
     xd = plan._x2d(x)
-    shape = (xd.shape[0], plan.na, N)
+    shape = (xd.shape[0], plan.na, plan.n_cols(hop_len))
     cdt, rdt = Bk.cplx_dtype(dtype), Bk.real_dtype(dtype)
     new = lambda dt_, on=True: torch.empty(shape, dtype=dt_, device='cuda') if on else None
     grad = torch.is_tensor(x) and x.requires_grad
@@ -178,7 +186,7 @@ def _ssq_cwt2(x, wavelet, scales, ssq_freqs, N, fs, dt, padtype, squeezing, mapr
     w = None
     if squeezing == 'sum' and not get_w and not grad:
         Tx, Wx, dWx = new(cdt), new(cdt, get_Wx), new(cdt, get_dWx)
-        o2.run(plan, xd, desc, Tx=Tx, Wx=Wx, dWx=dWx)
+        o2.run(plan, xd, desc, Tx=Tx, Wx=Wx, dWx=dWx, hop=hop_len)
         # `scales` go high -> low, so the returned frequencies are reversed
         f = hp['ssq_freqs']
         ssq_freqs = f.flip(0) if Bk.is_tensor(f) else np.asarray(f)[::-1].copy()
@@ -186,18 +194,18 @@ def _ssq_cwt2(x, wavelet, scales, ssq_freqs, N, fs, dt, padtype, squeezing, mapr
         w = new(rdt)
         if grad:
             # the differentiable transform's own (W, dW) feed the w-only kernel
-            Wx, dWx = _CwtFn.apply(xd, plan, True, None, False)
+            Wx, dWx = _CwtFn.apply(xd, plan, True, None, False, hop_len)
             o2.run(plan, xd.detach(), desc, w=w, Wx=Wx.detach(), dWx=dWx.detach(),
-                   W_given=True)
+                   W_given=True, hop=hop_len)
             if not get_dWx:
                 dWx = None
         else:
             Wx, dWx = new(cdt), new(cdt, get_dWx)
-            o2.run(plan, xd, desc, w=w, Wx=Wx, dWx=dWx)
+            o2.run(plan, xd, desc, w=w, Wx=Wx, dWx=dWx, hop=hop_len)
         Tx, ssq_freqs = ssqueeze(Wx, w, ssq_freqs, sc,
                                  fs=fs, squeezing=squeezing, maprange=maprange,
                                  wavelet=wavelet, gamma=gamma, was_padded=was_padded,
-                                 flipud=flipud, transform='cwt')
+                                 flipud=flipud, transform='cwt', N=N)
         if not get_w:
             w = None
     if not get_Wx:
@@ -215,19 +223,19 @@ class _SsqCwtFn(torch.autograd.Function):
     Gradients that do not arrive are None, as in `_CwtFn`."""
 
     @staticmethod
-    def forward(ctx, x2d, plan, desc, key):
+    def forward(ctx, x2d, plan, desc, key, hop):
         ctx.set_materialize_grads(False)
-        ctx.plan, ctx.desc = plan, desc
+        ctx.plan, ctx.desc, ctx.hop = plan, desc, hop
         with plan._lock:
             plan.set_reassign(desc, key)
-            Tx, Wx, dWx = plan.ssq_cwt(x2d.detach(), get_dWx=True)
+            Tx, Wx, dWx = plan.ssq_cwt(x2d.detach(), get_dWx=True, hop_len=hop)
         ctx.save_for_backward(Wx, dWx)
         return Tx, Wx, dWx
 
     @staticmethod
     def backward(ctx, gT, gW, gdW):
         if gT is None and gW is None and gdW is None:
-            return None, None, None, None
+            return None, None, None, None, None
         plan = ctx.plan
         Wx, dWx = ctx.saved_tensors
         if gT is not None:
@@ -236,13 +244,14 @@ class _SsqCwtFn(torch.autograd.Function):
         gW = None if gW is None else gW.to(cdt).contiguous()
         gdW = None if gdW is None else gdW.to(cdt).contiguous()
         if gW is None and gdW is None:
-            return None, None, None, None
+            return None, None, None, None, None
         B = Wx.shape[0]
         gx = torch.empty((B, plan.N), dtype=Bk.real_dtype(plan.dtype), device='cuda')
         with plan._lock:
-            _lib.check(plan.lib.ssqb_cwt_backward(plan.handle, Bk.ptr(gW), Bk.ptr(gdW), B, None,
-                                                  0, gx.data_ptr(), Bk.stream_ptr()))
-        return gx, None, None, None
+            _lib.check(plan.lib.ssqb_cwt_backward_hop(plan.handle, Bk.ptr(gW), Bk.ptr(gdW), B,
+                                                      None, 0, ctx.hop, gx.data_ptr(),
+                                                      Bk.stream_ptr()))
+        return gx, None, None, None, None
 
 
 _HP_CACHE = {}

@@ -106,26 +106,29 @@ class _Order2:
         self._scratch = None
         self._done = None                 # event after the last call that used the scratch
 
-    def _get_scratch(self, g):
-        if self._scratch is None or self._scratch.shape[1] < g:
+    def _get_scratch(self, g, ncol):
+        """[5, g, na, ncol] view of the scratch (ncol <= N)."""
+        size = 5 * g * self.na * ncol
+        if self._scratch is None or self._scratch.numel() < size:
             self._scratch = None
-            self._scratch = torch.empty((5, g, self.na, self.N), dtype=Bk.cplx_dtype(self.dtype),
+            self._scratch = torch.empty(5 * g * self.na * self.N, dtype=Bk.cplx_dtype(self.dtype),
                                         device='cuda')
-        return self._scratch
+        return self._scratch[:size].view(5, g, self.na, ncol)
 
-    def run(self, plan, xd, desc, Tx=None, w=None, Wx=None, dWx=None, W_given=False):
+    def run(self, plan, xd, desc, Tx=None, w=None, Wx=None, dWx=None, W_given=False, hop=1):
         """`plan`: the base plan this companion belongs to; `xd` [B, N] device signals of its
-        dtype.  Exactly one of `Tx` (complex) and `w` (real), [B, na, N], receives the result;
-        `Wx` / `dWx` [B, na, N], when given, receive W / dW (otherwise they stay in the scratch).
+        dtype.  Exactly one of `Tx` (complex) and `w` (real), [B, na, Nh], receives the result;
+        `Wx` / `dWx` [B, na, Nh], when given, receive W / dW (otherwise they stay in the scratch).
         `W_given`: `Wx` and `dWx` already hold this plan's transform of `xd`, which is then not
-        computed again."""
+        computed again.  Every plane holds the columns j * hop, Nh = (N - 1) // hop + 1."""
         lib = Bk.require_cuda()
         B = xd.shape[0]
         g = min(self.group, B)
+        ncol = plan.n_cols(hop)
         with plan._lock:
             if self._done is not None:    # the scratch of a call on another stream
                 torch.cuda.current_stream().wait_event(self._done)
-            S = self._get_scratch(g)
+            S = self._get_scratch(g, ncol)
             for b0 in range(0, B, g):
                 b1 = min(B, b0 + g)
                 n = b1 - b0
@@ -134,12 +137,12 @@ class _Order2:
                 A, dA, D2 = S[2, :n], S[3, :n], S[4, :n]
                 xg = xd[b0:b1]
                 if not W_given:
-                    plan.cwt_into(xg, W, dW)
-                self.pA.cwt_into(xg, A, dA)
-                self.pB.cwt_into(xg, D2)
+                    plan.cwt_into(xg, W, dW, hop_len=hop)
+                self.pA.cwt_into(xg, A, dA, hop_len=hop)
+                self.pB.cwt_into(xg, D2, hop_len=hop)
                 _lib.check(lib.ssqb_ssq_cwt2_reassign(
                     Bk.dtype_code(self.dtype), W.data_ptr(), dW.data_ptr(), A.data_ptr(),
-                    dA.data_ptr(), D2.data_ptr(), self.dt, n, self.na, self.N, C.byref(desc),
+                    dA.data_ptr(), D2.data_ptr(), self.dt, n, self.na, ncol, C.byref(desc),
                     None if Tx is None else Tx[b0:b1].data_ptr(),
                     None if w is None else w[b0:b1].data_ptr(), Bk.stream_ptr()))
             self._done = torch.cuda.Event()

@@ -101,13 +101,25 @@ int ssqb_cwt_plan_set_reassign(ssqb_cwt_plan* p, const ssqb_reassign_desc* r) {
 int ssqb_cwt_exec(ssqb_cwt_plan* p, const void* x, int64_t B, void* Wx, void* dWx,
                   const double* out_mul_host, int rpadded, void* stream) {
   if (!p) return set_error(SSQB_E_ARG, "null plan");
-  return p->impl->exec(x, B, Wx, dWx, nullptr, false, out_mul_host, rpadded != 0, (cudaStream_t)stream);
+  return p->impl->exec(x, B, Wx, dWx, nullptr, false, out_mul_host, rpadded != 0, 1, (cudaStream_t)stream);
 }
 
 int ssqb_ssq_cwt_exec(ssqb_cwt_plan* p, const void* x, int64_t B, void* Wx, void* Tx, void* dWx,
                       void* stream) {
   if (!p) return set_error(SSQB_E_ARG, "null plan");
-  return p->impl->exec(x, B, Wx, dWx, Tx, true, nullptr, false, (cudaStream_t)stream);
+  return p->impl->exec(x, B, Wx, dWx, Tx, true, nullptr, false, 1, (cudaStream_t)stream);
+}
+
+int ssqb_cwt_exec_hop(ssqb_cwt_plan* p, const void* x, int64_t B, void* Wx, void* dWx,
+                      const double* out_mul_host, int rpadded, int64_t hop, void* stream) {
+  if (!p) return set_error(SSQB_E_ARG, "null plan");
+  return p->impl->exec(x, B, Wx, dWx, nullptr, false, out_mul_host, rpadded != 0, hop, (cudaStream_t)stream);
+}
+
+int ssqb_ssq_cwt_exec_hop(ssqb_cwt_plan* p, const void* x, int64_t B, void* Wx, void* Tx, void* dWx,
+                          int64_t hop, void* stream) {
+  if (!p) return set_error(SSQB_E_ARG, "null plan");
+  return p->impl->exec(x, B, Wx, dWx, Tx, true, nullptr, false, hop, (cudaStream_t)stream);
 }
 
 int ssqb_cwt_exec_host(ssqb_cwt_plan* p, const void* x, int64_t B, void* Wx, void* dWx,
@@ -130,7 +142,14 @@ int ssqb_cwt_debug_xh(ssqb_cwt_plan* p, const void* x, int64_t B, void* xh, void
 int ssqb_cwt_backward(ssqb_cwt_plan* p, const void* gWx, const void* gdWx, int64_t B,
                       const double* out_mul_host, int rpadded, void* gx, void* stream) {
   if (!p || !gx || (!gWx && !gdWx)) return set_error(SSQB_E_ARG, "null argument");
-  return p->impl->backward(gWx, gdWx, B, out_mul_host, rpadded != 0, gx, (cudaStream_t)stream);
+  return p->impl->backward(gWx, gdWx, B, out_mul_host, rpadded != 0, 1, gx, (cudaStream_t)stream);
+}
+
+int ssqb_cwt_backward_hop(ssqb_cwt_plan* p, const void* gWx, const void* gdWx, int64_t B,
+                          const double* out_mul_host, int rpadded, int64_t hop, void* gx,
+                          void* stream) {
+  if (!p || !gx || (!gWx && !gdWx)) return set_error(SSQB_E_ARG, "null argument");
+  return p->impl->backward(gWx, gdWx, B, out_mul_host, rpadded != 0, hop, gx, (cudaStream_t)stream);
 }
 
 int ssqb_cwt_plan_set_profiling(ssqb_cwt_plan* p, int on) {

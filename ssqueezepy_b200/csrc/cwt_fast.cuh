@@ -244,7 +244,9 @@ struct RowsTile {
 };
 
 // STORE_W = false: the fused epilogue without the Wx store (cwt_rows_tx_kernel)
-template <typename T, int LOGE, int LOG_F, int NARR, int GEN, int QMAX, bool SSQ, int BPT, bool STORE_W>
+// HOP: the epilogue runs on the columns of a time-decimated call only (CwtArgs::hop)
+template <typename T, int LOGE, int LOG_F, int NARR, int GEN, int QMAX, bool SSQ, int BPT, bool STORE_W,
+          bool HOP = false>
 __device__ __forceinline__ void cwt_rows_body(const FastArgs<T>& P) {
   // Length-F inverse transform over i1 (F = 8, 64 or 512 = one, two or three radix-8
   // stages; narrow-band rows use the shortest F that still holds their band), for
@@ -431,6 +433,8 @@ __device__ __forceinline__ void cwt_rows_body(const FastArgs<T>& P) {
   // whole-signal mode: output j = t - out_off, kept if j < Nout;
   // block mode: block sample t -> j = k*hop + (t - h2), kept if (t - h2) < hop and j < Nout
   int sig = b, eoff = (int)A.out_off, elim = (int)A.Nout, eshift = 0;
+  const int Nlim = HOP ? (int)A.Nout * A.hop : (int)A.Nout;   // bound of the full column
+  if (HOP) elim = Nlim;
   if (GEN == GEN_DIRECT && P.blk_n > 0) {
     sig = b / P.blk_n;
     eshift = (b - sig * P.blk_n) * P.blk_hop;
@@ -449,8 +453,9 @@ __device__ __forceinline__ void cwt_rows_body(const FastArgs<T>& P) {
 #pragma unroll
       for (int q = 0; q < 8; ++q) {
         const int jj = ((j[bb] + F8 * q) << logI2) + jbase;
-        const int jo = jj + eshift;
-        if ((unsigned)jj < (unsigned)elim && jo < Nout) {
+        int jo = jj + eshift;
+        if ((unsigned)jj < (unsigned)elim && jo < Nlim) {
+          if (HOP) { jo = hop_col(jo, A.hop); if (jo < 0) continue; }
           Wrow[jo] = cscale<T>(v[0][bb][q], mlt);
           if (NARR == 2 && P.write_dWx) dWrow[jo] = cscale<T>(v[1][bb][q], mlt);
         }
@@ -470,8 +475,9 @@ __device__ __forceinline__ void cwt_rows_body(const FastArgs<T>& P) {
 #pragma unroll
       for (int q = 0; q < 8; ++q) {
         const int jj = ((j[bb] + F8 * q) << logI2) + jbase;
-        const int jo = jj + eshift;
-        if ((unsigned)jj < (unsigned)elim && jo < Nout) {
+        int jo = jj + eshift;
+        if ((unsigned)jj < (unsigned)elim && jo < Nlim) {
+          if (HOP) { jo = hop_col(jo, A.hop); if (jo < 0) continue; }
           if (STORE_W) Wrow[jo] = v[0][bb][q];
           if (P.write_dWx) dWrow[jo] = v[1][bb][q];
           if (Zrow) Zrow[jo] = mkc<T>((T)0, (T)0);
@@ -496,6 +502,13 @@ template <typename T, int LOGE, int LOG_F, int GEN, int QMAX, int BPT>
 __global__ void __launch_bounds__((1 << LOGE) / (8 * BPT), (BPT == 1 && LOGE <= 12 && sizeof(T) == 4) ? 2 : 1)
 cwt_rows_tx_kernel(const FastArgs<T> P) {
   cwt_rows_body<T, LOGE, LOG_F, 2, GEN, QMAX, true, BPT, false>(P);
+}
+
+// time-decimated call (CwtArgs::hop > 1): either of the two above on the wanted columns only
+template <typename T, int LOGE, int LOG_F, int NARR, int GEN, int QMAX, bool SSQ, int BPT, bool STORE_W>
+__global__ void __launch_bounds__((1 << LOGE) / (8 * BPT), (BPT == 1 && LOGE <= 12 && sizeof(T) == 4) ? 2 : 1)
+cwt_rows_hop_kernel(const FastArgs<T> P) {
+  cwt_rows_body<T, LOGE, LOG_F, NARR, GEN, QMAX, SSQ, BPT, STORE_W, true>(P);
 }
 
 // ---- (3) pass 1 of the two-pass route for wide-band rows ---------------------------

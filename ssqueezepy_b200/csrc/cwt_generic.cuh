@@ -160,6 +160,18 @@ gen_unpad_kernel(const cx<T>* __restrict__ src, cx<T>* __restrict__ dst, long lo
   const T m = out_mul ? out_mul[(r0 + rl) % na] : (T)1;
   dst[(r0 + rl) * Nout + j] = cscale<T>(src[rl * n + off + j], m);
 }
+// the same for a time-decimated call: dst column j holds unpadded column j * hop
+template <typename T>
+__global__ void __launch_bounds__(256)
+gen_unpad_hop_kernel(const cx<T>* __restrict__ src, cx<T>* __restrict__ dst, long long n, long long off,
+                     long long Nout, long long hop, long long nr, long long r0,
+                     const T* __restrict__ out_mul, int na) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= nr * Nout) return;
+  const long long rl = idx / Nout, j = idx - rl * Nout;
+  const T m = out_mul ? out_mul[(r0 + rl) % na] : (T)1;
+  dst[(r0 + rl) * Nout + j] = cscale<T>(src[rl * n + off + j * hop], m);
+}
 
 // ---- pieces shared by the power-of-two plan (cwt_impl.cuh) and the generic-length plan ---------
 // descriptor checks that hold at every transform length
@@ -171,6 +183,13 @@ inline int check_cwt_desc(const ssqb_cwt_desc& d) {
   if (d.wavelet < 0 || d.wavelet > 2) return set_error(SSQB_E_ARG, "bad wavelet kind");
   if (d.wavelet == SSQB_WAV_TABLE && !d.psih_table_dev)
     return set_error(SSQB_E_ARG, "SSQB_WAV_TABLE needs psih_table_dev");
+  return 0;
+}
+
+// time decimation of an exec / backward call: hop >= 1, and only on the unpadded part
+inline int check_hop(long long hop, bool rpadded) {
+  if (hop < 1) return set_error(SSQB_E_ARG, "hop=%lld must be >= 1", hop);
+  if (rpadded && hop > 1) return set_error(SSQB_E_ARG, "hop > 1 needs rpadded = 0");
   return 0;
 }
 
@@ -251,7 +270,7 @@ struct HostStaging {
       cx<T>* Ts = ssq ? Tx_stage.p + sl * nout : nullptr;
       SSQB_CUDA(cudaMemcpyAsync(xs, xh_ + (size_t)b0 * (size_t)d.N, cx_ * sizeof(T),
                                 cudaMemcpyHostToDevice, st));
-      rc = plan.exec(xs, nb, Ws, dWs, Ts, ssq, out_mul_host, rpadded, st);
+      rc = plan.exec(xs, nb, Ws, dWs, Ts, ssq, out_mul_host, rpadded, 1, st);
       if (rc) break;
       SSQB_CUDA(cudaEventRecord(ev_comp[sl], st));
       SSQB_CUDA(cudaStreamWaitEvent(copy_st, ev_comp[sl], 0));
@@ -290,6 +309,23 @@ adj_pad_kernel(const cx<T>* __restrict__ G, cx<T>* __restrict__ Z, long long n, 
   if (t >= off && t < off + Nout) {
     const T m = out_mul ? out_mul[(r0 + rl) % na] : (T)1;
     v = cscale<T>(G[(r0 + rl) * Nout + (t - off)], m);
+  }
+  Z[idx] = v;
+}
+// the same for a time-decimated gradient G [..][Nout] (column j = unpadded column j * hop): U^T
+// inserts zeros, Z[r][t] = mul_a * G[row][(t - off) / hop] where hop divides t - off (< N)
+template <typename T>
+__global__ void __launch_bounds__(256)
+adj_pad_hop_kernel(const cx<T>* __restrict__ G, cx<T>* __restrict__ Z, long long n, long long off,
+                   long long N, long long Nout, long long hop, long long r0, long long nr,
+                   const T* __restrict__ out_mul, int na) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= nr * n) return;
+  const long long rl = idx / n, t = idx - rl * n, s = t - off, j = s / hop;
+  cx<T> v = mkc<T>((T)0, (T)0);
+  if (s >= 0 && s < N && j * hop == s) {
+    const T m = out_mul ? out_mul[(r0 + rl) % na] : (T)1;
+    v = cscale<T>(G[(r0 + rl) * Nout + j], m);
   }
   Z[idx] = v;
 }
@@ -349,10 +385,12 @@ struct CwtAdjoint {
   DevBuf<cx<T>> Z, Zh, acc, gp;
   DevBuf<T> mul_d;
   DevBuf<long long> pad_tab; long long n_groups = 0;
-  // gW / gdW [B][na][Nout] (either may be null), gx [B][N] (overwritten)
+  // gW / gdW [B][na][Nout] (either may be null), gx [B][N] (overwritten); hop > 1: gradients of a
+  // time-decimated call, Nout = (N - 1) / hop + 1 (never with rpadded)
   int run(const ssqb_cwt_desc& d, CwtArgs<T> A, const cx<T>* gW, const cx<T>* gdW, long long B,
-          const double* out_mul_host, bool rpadded, T* gx, cudaStream_t st) {
-    const long long n = d.n_up, Nout = rpadded ? n : d.N, off = rpadded ? 0 : d.n1;
+          const double* out_mul_host, bool rpadded, long long hop, T* gx, cudaStream_t st) {
+    const long long n = d.n_up, off = rpadded ? 0 : d.n1;
+    const long long Nout = rpadded ? n : (d.N - 1) / hop + 1;
     if (!ready) {
       int rc = fft.init(n); if (rc) return rc;
       const PadGroups pg = pad_groups(d.N, d.n1, n, d.padtype);
@@ -380,7 +418,11 @@ struct CwtAdjoint {
         for (int a0 = 0; a0 < d.na; a0 += (int)chunk) {
           const int nr = d.na - a0 < chunk ? d.na - a0 : (int)chunk;
           const long long r0 = b * d.na + a0;
-          adj_pad_kernel<T><<<(unsigned)(((long long)nr * n + 255) / 256), 256, 0, st>>>(G, Z.p, n, off, Nout, r0, nr, out_mul, d.na);
+          const unsigned nblk = (unsigned)(((long long)nr * n + 255) / 256);
+          if (hop > 1)
+            adj_pad_hop_kernel<T><<<nblk, 256, 0, st>>>(G, Z.p, n, off, d.N, Nout, hop, r0, nr, out_mul, d.na);
+          else
+            adj_pad_kernel<T><<<nblk, 256, 0, st>>>(G, Z.p, n, off, Nout, r0, nr, out_mul, d.na);
           SSQB_LAUNCH_CHECK();
           rc = fft.exec(Z.p, Zh.p, nr, -1, (T)1, st); if (rc) return rc;
           adj_accum_kernel<T><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(A, Zh.p, acc.p + b * n, a0, nr, pass);
@@ -425,11 +467,14 @@ struct GenericCwtPlan : public CwtPlanBase {
     return 0;
   }
   int exec(const void* xv, long long B, void* Wxv, void* dWxv, void* Txv, bool ssq,
-           const double* out_mul_host, bool rpadded, cudaStream_t st) override {
+           const double* out_mul_host, bool rpadded, long long hop, cudaStream_t st) override {
     if (B < 1 || !xv || (!Wxv && !ssq)) return set_error(SSQB_E_ARG, "bad arguments");
     if (ssq && (!Txv || !have_grid)) return set_error(SSQB_E_ARG, "ssq needs Tx and a reassignment grid");
     if (ssq && rpadded) return set_error(SSQB_E_ARG, "ssq works on the unpadded part");
-    const long long n = d.n_up, Nout = rpadded ? n : d.N, off = rpadded ? 0 : d.n1;
+    { int rc = check_hop(hop, rpadded); if (rc) return rc; }
+    if (hop > d.N) hop = d.N;                       // one column either way
+    const long long n = d.n_up, off = rpadded ? 0 : d.n1;
+    const long long Nout = rpadded ? n : (d.N - 1) / hop + 1;
     const long long rows = B * d.na;
     cx<T>* Wx = (cx<T>*)Wxv; cx<T>* dWx = (cx<T>*)dWxv;
     // the column-owner ssqueeze reads Wx and dWx: planes the caller did not ask for are internal
@@ -454,12 +499,19 @@ struct GenericCwtPlan : public CwtPlanBase {
       const long long nr = rows - r0 < chunk ? rows - r0 : chunk;
       gen_mul_kernel<T><<<(unsigned)((nr * n + 255) / 256), 256, 0, st>>>(A, ZW.p, deriv ? ZD.p : nullptr, r0, nr);
       SSQB_LAUNCH_CHECK();
+      const unsigned nblk = (unsigned)((nr * Nout + 255) / 256);
+      auto unpad = [&](const cx<T>* src, cx<T>* dst) {
+        if (hop > 1)
+          gen_unpad_hop_kernel<T><<<nblk, 256, 0, st>>>(src, dst, n, off, Nout, hop, nr, r0, out_mul, d.na);
+        else
+          gen_unpad_kernel<T><<<nblk, 256, 0, st>>>(src, dst, n, off, Nout, nr, r0, out_mul, d.na);
+      };
       rc = fft.exec(ZW.p, OW.p, nr, +1, (T)1, st); if (rc) return rc;
-      gen_unpad_kernel<T><<<(unsigned)((nr * Nout + 255) / 256), 256, 0, st>>>(OW.p, Wx, n, off, Nout, nr, r0, out_mul, d.na);
+      unpad(OW.p, Wx);
       SSQB_LAUNCH_CHECK();
       if (deriv) {
         rc = fft.exec(ZD.p, OD.p, nr, +1, (T)1, st); if (rc) return rc;
-        gen_unpad_kernel<T><<<(unsigned)((nr * Nout + 255) / 256), 256, 0, st>>>(OD.p, dWx, n, off, Nout, nr, r0, out_mul, d.na);
+        unpad(OD.p, dWx);
         SSQB_LAUNCH_CHECK();
       }
     }
@@ -481,9 +533,11 @@ struct GenericCwtPlan : public CwtPlanBase {
   }
   CwtAdjoint<T> adj;
   int backward(const void* gWx, const void* gdWx, long long B, const double* out_mul_host,
-               bool rpadded, void* gx, cudaStream_t st) override {
+               bool rpadded, long long hop, void* gx, cudaStream_t st) override {
+    { int rc = check_hop(hop, rpadded); if (rc) return rc; }
     CwtArgs<T> A; cwt_common_args(d, scales_d.p, A);
-    return adj.run(d, A, (const cx<T>*)gWx, (const cx<T>*)gdWx, B, out_mul_host, rpadded, (T*)gx, st);
+    return adj.run(d, A, (const cx<T>*)gWx, (const cx<T>*)gdWx, B, out_mul_host, rpadded,
+                   hop < d.N ? hop : d.N, (T*)gx, st);
   }
   int set_profiling(int) override { return 0; }
   int get_profile(double* ms, long long* launches, long long* rows) override {

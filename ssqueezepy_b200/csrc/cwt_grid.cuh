@@ -291,8 +291,44 @@ template <typename T, int K, int PPK> struct InterpGeom {
   static constexpr int NT = 256;
 };
 
+// Geometry of a time-decimated interpolation (hop h > 1) on a row of U = 2^logU fine samples per
+// coarse sample; the host sizes the launch with the same function.  The wanted outputs are
+// t = t0 + j h.  With g = gcd(h, U) (h's largest power-of-two factor, at most U), they sit on the
+// phases u = t0 (mod g), and on such a phase at every q-th coarse sample, q = h / g.  The CTAs
+// launch the phases u = u0 + s v, s = min(g, U / 16) (a CTA needs 16 of them), u0 = t0 mod s.
+// q = 1 and s = g (h a power of two, h <= U / 16): every launched output is wanted and the
+// threads slide their window as at h = 1 ("phase mode").  Otherwise ("stride mode") a thread
+// of a wanted phase evaluates every q-th coarse sample of its window from the taps in shared memory.
+struct GridHopGeom { int logV, logs, u0, lg, q; bool stride; };
+__host__ __device__ inline GridHopGeom grid_hop_geom(int hop, int t0, int logU) {
+  GridHopGeom g;
+  int lg = 0;
+  while (lg < logU && !((hop >> lg) & 1)) ++lg;       // g = 2^lg = gcd(h, U)
+  g.lg = lg; g.q = hop >> lg;
+  g.logs = lg < logU - 4 ? lg : logU - 4;
+  g.logV = logU - g.logs;
+  g.u0 = t0 & ((1 << g.logs) - 1);
+  g.stride = (g.q != 1) || (g.logs != lg);
+  return g;
+}
+// inverse of a modulo m (a, m coprime, m >= 1)
+__host__ __device__ inline long long mod_inverse(long long a, long long m) {
+  long long t = 0, nt = 1, r = m, nr = a % m;
+  while (nr) {
+    const long long k = r / nr, t2 = t - k * nt, r2 = r - k * nr;
+    t = nt; nt = t2; r = nr; nr = r2;
+  }
+  return ((t % m) + m) % m;
+}
+
 // STORE_W = false: the fused epilogue without the Wx store (grid_interp_tx_kernel)
-template <typename T, int K, int PPK, int NARR, bool SSQ, bool STORE_W>
+// HOP: a time-decimated call (CwtArgs::hop = h; the window t0, tcount stays the full one) computes
+// only the wanted outputs t = t0 + j h, stored at column j (grid_hop_geom): phase mode slides the
+// window over the launched phases; stride mode evaluates every q-th coarse sample of a thread's
+// window from the taps in shared memory, in the sliding window's order (h[0] v0, then caxpy for
+// k = 1 .. K - 1), so every output is the same sequence of operations as at h = 1.  A CTA whose
+// tile of coarse samples holds no wanted output returns before loading its window.
+template <typename T, int K, int PPK, int NARR, bool SSQ, bool STORE_W, bool HOP = false>
 __device__ __forceinline__ void grid_interp_body(const GridArgs<T>& G) {
   constexpr int PP = K * PPK;
   constexpr int NT = 256;
@@ -304,10 +340,14 @@ __device__ __forceinline__ void grid_interp_body(const GridArgs<T>& G) {
   const int b = y / G.n_rows;
   const GridRow ri = G.rows[y - b * G.n_rows];
   const int logM = ri.logM, logU = A.logn - logM;
-  const int logUT = logU < 8 ? logU : 8;
+  GridHopGeom hg;                                     // h = 1: logV = logU, phase mode
+  if (HOP) hg = grid_hop_geom(A.hop, (int)A.out_off, logU);
+  else { hg.logV = logU; hg.logs = 0; hg.u0 = 0; hg.lg = 0; hg.q = 1; hg.stride = false; }
+  const int logV = hg.logV;                           // log2 of the phases launched per coarse sample
+  const int logUT = logV < 8 ? logV : 8;
   const int UT = 1 << logUT, PG = NT >> logUT;
   const int PTILE = PG * PP;                          // coarse samples per CTA
-  const int n_ut = 1 << (logU - logUT);
+  const int n_ut = 1 << (logV - logUT);
   const int p_first = G.t0 >> logU;
   const int p_last = (G.t0 + G.tcount - 1) >> logU;
   const int n_pt = (p_last - p_first + PTILE) / PTILE;
@@ -315,6 +355,13 @@ __device__ __forceinline__ void grid_interp_body(const GridArgs<T>& G) {
   if (tile >= n_ut * n_pt) return;
   const int ut = tile % n_ut, pt = tile / n_ut;
   const int p_cta = p_first + pt * PTILE;             // first coarse sample of this CTA
+  if (HOP && hg.stride) {                             // skip a tile without wanted outputs
+    const int hop = A.hop, joff = (int)A.out_off;
+    int ts = p_cta << logU, te = (p_cta + PTILE) << logU;
+    if (ts < G.t0) ts = G.t0;
+    if (te > G.t0 + G.tcount) te = G.t0 + G.tcount;
+    if ((ts - joff + hop - 1) / hop >= (te - joff + hop - 1) / hop) return;
+  }
   V4* Vs = reinterpret_cast<V4*>(smem_raw);           // [PTILE + K - 1]
   cx<T>* As = reinterpret_cast<cx<T>*>(Vs + (PTILE + K - 1));   // [PTILE] e^{2 pi i c p / M}
   const unsigned Mm = (1u << logM) - 1u;
@@ -341,7 +388,7 @@ __device__ __forceinline__ void grid_interp_body(const GridArgs<T>& G) {
     }
   }
   const int ul = tid & (UT - 1), pg = tid >> logUT;
-  const int u = ut * UT + ul;
+  const int u = HOP ? hg.u0 + ((ut * UT + ul) << hg.logs) : ut * UT + ul;
   T h[K];
   {
     const T* __restrict__ hp = G.htab + ((size_t)u << (G.log_umax - logU)) * K;
@@ -375,28 +422,63 @@ __device__ __forceinline__ void grid_interp_body(const GridArgs<T>& G) {
     if ((w0 >= 0) && (w0 + PTILE + K - 1 <= (1 << logM))) mbar_wait(&vbar, 0);   // window has landed
   }
   __syncthreads();
+  const int joff = (int)A.out_off;
+  // the stores and the fused reassignment of output column jo
+  auto put = [&](int jo, cx<T> W, cx<T> ad, cx<T> tw) {
+    if (!SSQ) {
+      Wrow[jo] = cscale<T>(W, mlt);
+      if (NARR == 2 && G.write_dWx) dWrow[jo] = cscale<T>(cmul<T>(ad, tw), mlt);
+    } else {
+      const cx<T> dW = cmul<T>(ad, tw);
+      if (STORE_W) Wrow[jo] = W;
+      if (G.write_dWx) dWrow[jo] = dW;
+      if (Zrow) Zrow[jo] = mkc<T>((T)0, (T)0);
+      ssq_point<T>(W, dW, Tb + jo, rowbytes, cre, cwide, g2lo, g2hi, fast_ok, A.grid);
+    }
+  };
   if (np <= 0) return;
+  if (HOP && hg.stride) {
+    // this phase is wanted when t0 = u (mod g); then at the coarse samples p = pw (mod q), with
+    // p U = t0 - u (mod h) <=> p (U / g) = ((t0 - u) mod h) / g (mod q)
+    const int hop = A.hop, q = hg.q, gm = (1 << hg.lg) - 1;
+    if (((joff - u) & gm) != 0) return;
+    int rr = (joff - u) % hop; if (rr < 0) rr += hop;
+    const long long inv = mod_inverse((long long)(1 << (logU - hg.lg)) % q, q);
+    const int pw = (int)(((long long)((rr >> hg.lg) % q) * inv) % q);
+    const int pbeg = p_cta + wl0;
+    int p = pbeg + ((pw - pbeg % q) % q + q) % q;     // first wanted coarse sample of the window
+    int jo = ((p << logU) + u - joff) / hop;           // exact: h divides t - t0
+    const int dj = 1 << (logU - hg.lg);               // q U / h: columns per step
+    for (; p < pbeg + np; p += q, jo += dj) {
+      const int t = (p << logU) + u;
+      if (t < G.t0 || t >= G.t0 + G.tcount) continue;
+      const int l = p - p_cta;
+      V4 v = Vs[l];
+      cx<T> aw = cscale<T>(mkc<T>(v.x, v.y), h[0]);
+      cx<T> ad = mkc<T>((T)0, (T)0);
+      if (NARR == 2) ad = cscale<T>(mkc<T>(v.z, v.w), h[0]);
+#pragma unroll
+      for (int k = 1; k < K; ++k) {
+        v = Vs[l + k];
+        aw = caxpy<T>(mkc<T>(v.x, v.y), h[k], aw);
+        if (NARR == 2) ad = caxpy<T>(mkc<T>(v.z, v.w), h[k], ad);
+      }
+      const cx<T> tw = cmul<T>(As[l], Bu);
+      put(jo, cmul<T>(aw, tw), ad, tw);
+    }
+    return;
+  }
 
   const int tbase = ((p_cta + wl0) << logU) + u;      // padded time index of output i = 0
   const int tlo = G.t0, thi = G.t0 + G.tcount;
-  const int joff = (int)A.out_off;
 
   auto emit = [&](int i, cx<T> aw, cx<T> ad) {
     const int t = tbase + (i << logU);
     if (i < np && t >= tlo && t < thi) {
       const cx<T> tw = cmul<T>(As[wl0 + i], Bu);
       const cx<T> W = cmul<T>(aw, tw);
-      const int jo = t - joff;
-      if (!SSQ) {
-        Wrow[jo] = cscale<T>(W, mlt);
-        if (NARR == 2 && G.write_dWx) dWrow[jo] = cscale<T>(cmul<T>(ad, tw), mlt);
-      } else {
-        const cx<T> dW = cmul<T>(ad, tw);
-        if (STORE_W) Wrow[jo] = W;
-        if (G.write_dWx) dWrow[jo] = dW;
-        if (Zrow) Zrow[jo] = mkc<T>((T)0, (T)0);
-        ssq_point<T>(W, dW, Tb + jo, rowbytes, cre, cwide, g2lo, g2hi, fast_ok, A.grid);
-      }
+      const int jo = (t - joff) >> hg.logs;           // phase mode: every launched t is wanted
+      put(jo, W, ad, tw);
     }
   };
 
@@ -436,6 +518,13 @@ template <typename T, int K, int PPK>
 __global__ void __launch_bounds__(256, (sizeof(T) == 4) ? 3 : 1)
 grid_interp_tx_kernel(const GridArgs<T> G) {
   grid_interp_body<T, K, PPK, 2, true, false>(G);
+}
+
+// time-decimated call (CwtArgs::hop > 1): either of the two above on the wanted columns only
+template <typename T, int K, int PPK, int NARR, bool SSQ, bool STORE_W>
+__global__ void __launch_bounds__(256, (sizeof(T) == 4) ? 3 : 1)
+grid_interp_hop_kernel(const GridArgs<T> G) {
+  grid_interp_body<T, K, PPK, NARR, SSQ, STORE_W, true>(G);
 }
 
 

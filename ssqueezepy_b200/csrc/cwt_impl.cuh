@@ -39,6 +39,7 @@ static int launch_pass2_t(const CwtArgs<T>& A, int write_dWx, cudaStream_t st) {
   constexpr int R2 = Tile<T>::ELEMS / F;
   size_t smem = ((size_t)NARR * Tile<T>::ELEMS + F) * sizeof(cx<T>);
   auto kern = cwt_pass2_kernel<T, LOG_F, NARR, EPI>;
+  if constexpr (EPI != EPI_FWD) if (A.hop > 1) kern = cwt_pass2_hop_kernel<T, LOG_F, NARR, EPI>;
   SSQB_CUDA(opt_in_smem(kern, smem));
   long long ncols = (long long)A.nrows << A.logI2;
   dim3 grid((unsigned)((ncols + R2 - 1) / R2));
@@ -78,6 +79,7 @@ static int launch_rows_b(const FastArgs<T>& P, unsigned grid_y, cudaStream_t st)
   if (LOG_F > 3) smem += (size_t)NARR * RowsTile<T, LOGE, LOG_F>::SARR * sizeof(cx<T>);
   if (GEN == GEN_DIRECT) smem += (size_t)QMAX * F * 4 * sizeof(T);
   auto kern = rows_kernel<T, LOGE, LOG_F, NARR, GEN, QMAX, SSQ, BPT, STORE_W>();
+  if (A.hop > 1) kern = cwt_rows_hop_kernel<T, LOGE, LOG_F, NARR, GEN, QMAX, SSQ, BPT, STORE_W>;
   SSQB_CUDA(opt_in_smem(kern, smem));
   long long nF = (long long)A.n_up >> LOG_F;         // output phases per row
   dim3 grid((unsigned)(nF / (ELEMS / F)), grid_y);
@@ -200,6 +202,7 @@ static int launch_sblk_rows_t(const SblkArgs<T>& S, SblkShare share, cudaStream_
   size_t smem = ((size_t)1 << LP) * (sizeof(V4) + sizeof(cx<T>));
   auto kern = sblk_rows_kernel<T, LP, SblkGeom<T>::LOG_R, NARR, SSQ>;
   if constexpr (!STORE_W) kern = sblk_rows_tx_kernel<T, LP, SblkGeom<T>::LOG_R>;
+  if (S.A.hop > 1) kern = sblk_rows_hop_kernel<T, LP, SblkGeom<T>::LOG_R, NARR, SSQ, STORE_W>;
   SSQB_CUDA(opt_in_smem(kern, smem));
   DeviceFacts dev;
   SSQB_CUDA(device_facts(&dev));
@@ -327,6 +330,7 @@ static int launch_grid_interp_t(const GridArgs<T>& G, unsigned max_tiles, cudaSt
   size_t smem = (size_t)(16 * PP + K - 1) * sizeof(V4) + (size_t)16 * PP * sizeof(cx<T>);
   auto kern = grid_interp_kernel<T, K, PPK, NARR, SSQ>;
   if constexpr (!STORE_W) kern = grid_interp_tx_kernel<T, K, PPK>;
+  if (G.A.hop > 1) kern = grid_interp_hop_kernel<T, K, PPK, NARR, SSQ, STORE_W>;
   SSQB_CUDA(opt_in_smem(kern, smem));
   dim3 grid(max_tiles, (unsigned)(G.B * G.n_rows));
   kern<<<grid, 256, smem, st>>>(G);
@@ -845,18 +849,18 @@ struct CwtPlan : public CwtPlanBase {
 
   // gridded rows: stage (A) needs xh only; stage (B) also the zeroed Tx (when ssq)
   void grid_args(GridArgs<T>& G, long long B, cx<T>* Wx, cx<T>* dWx, cx<T>* Tx, bool ssq,
-                 const T* out_mul, bool rpadded, long long Nout) {
+                 const T* out_mul, bool rpadded, long long Nout, int hop) {
     memset(&G, 0, sizeof(G));
     base_args(G.A);
     G.A.xh = xh_d.p; G.A.Wx = Wx; G.A.dWx = dWx; G.A.Tx = Tx;
-    G.A.Nout = Nout; G.A.out_off = rpadded ? 0 : d.n1; G.A.out_mul = out_mul;
+    G.A.Nout = Nout; G.A.hop = hop; G.A.out_off = rpadded ? 0 : d.n1; G.A.out_mul = out_mul;
     G.rows = grid_rows_d.p; G.n_rows = (int)grid_rows.size(); G.B = B;
     G.V = V_d.p; G.v_total = grid_v_total;
     G.gtab_p = gtab_p_d.p; G.gtab_pd = gtab_pd_d.p;
     G.rootsM = rootsM_d.p; G.rootsMh = rootsMh_d.p; G.log_mmax = GRID_BASE_LOGM;
     G.htab = htab_d.p; G.log_umax = grid_log_umax;
     G.write_dWx = dWx ? 1 : 0; G.ssq = ssq ? 1 : 0;
-    G.t0 = rpadded ? 0 : (int)d.n1; G.tcount = (int)Nout;
+    G.t0 = rpadded ? 0 : (int)d.n1; G.tcount = (int)(rpadded ? d.n_up : d.N);   // full window
   }
   // coarse-grid inverse FFTs: the two long classes (2^13, 2^12 points: a few CTAs each) and the
   // merged launch of all shorter ones go to three streams so that their latencies overlap
@@ -897,8 +901,15 @@ struct CwtPlan : public CwtPlanBase {
     unsigned max_tiles = 1;                               // tiles of the widest row class
     for (int lm = GRID_MIN_LOGM; lm <= GRID_MAX_LOGM; ++lm) {
       if (!grid_cls_n[lm]) continue;
-      const int logU = logn - lm, logUT = logU < 8 ? logU : 8;
-      const long long n_ut = 1ll << (logU - logUT), ptile = (256ll >> logUT) * PP;
+      const int logU = logn - lm;
+      int logUT = logU < 8 ? logU : 8;
+      long long n_ut = 1ll << (logU - logUT);
+      if (G.A.hop > 1) {                                  // the HOP kernel's geometry
+        const GridHopGeom hg = grid_hop_geom(G.A.hop, G.t0, logU);
+        logUT = hg.logV < 8 ? hg.logV : 8;
+        n_ut = 1ll << (hg.logV - logUT);
+      }
+      const long long ptile = (256ll >> logUT) * PP;
       const long long p_first = (long long)G.t0 >> logU, p_last = ((long long)G.t0 + G.tcount - 1) >> logU;
       const long long n_pt = (p_last - p_first + ptile) / ptile;
       if ((unsigned)(n_ut * n_pt) > max_tiles) max_tiles = (unsigned)(n_ut * n_pt);
@@ -1019,7 +1030,9 @@ struct CwtPlan : public CwtPlanBase {
   }
 
   int exec(const void* xv, long long B, void* Wxv, void* dWxv, void* Txv, bool ssq,
-           const double* out_mul_host, bool rpadded, cudaStream_t st) override {
+           const double* out_mul_host, bool rpadded, long long hop, cudaStream_t st) override {
+    { int rc = check_hop(hop, rpadded); if (rc) return rc; }
+    if (hop > d.N) hop = d.N;                       // one column either way
     if (!ev_done) SSQB_CUDA(ev_done.create());
     if (ev_done_valid) SSQB_CUDA(cudaStreamWaitEvent(st, ev_done, 0));
     const long long S = (B >= 1) ? group_size(B, ssq, rpadded) : B;
@@ -1032,9 +1045,10 @@ struct CwtPlan : public CwtPlanBase {
     int rc = 0;
     if (S >= B || S < 1) {
       zero_next_ = 0; zero_off_ = 0; zero_self_ = true;
-      rc = exec_body(xv, B, Wxv, dWxv, Txv, ssq, out_mul_host, rpadded, st);
+      rc = exec_body(xv, B, Wxv, dWxv, Txv, ssq, out_mul_host, rpadded, (int)hop, st);
     } else {
-      const size_t plane = (size_t)d.na * (size_t)d.N;            // ssq: outputs are unpadded
+      // ssq: outputs are unpadded, (N - 1) / hop + 1 columns
+      const size_t plane = (size_t)d.na * (size_t)((d.N - 1) / hop + 1);
       for (long long b0 = 0; b0 < B && rc == 0; b0 += S) {
         zero_self_ = (b0 == 0);
         zero_next_ = (b0 + S < B) ? (int)S : 0;
@@ -1042,7 +1056,7 @@ struct CwtPlan : public CwtPlanBase {
         rc = exec_body((const T*)xv + (size_t)b0 * (size_t)d.N, S,
                        Wxv ? (cx<T>*)Wxv + (size_t)b0 * plane : nullptr,
                        dWxv ? (cx<T>*)dWxv + (size_t)b0 * plane : nullptr,
-                       (cx<T>*)Txv + (size_t)b0 * plane, ssq, out_mul_host, rpadded, st);
+                       (cx<T>*)Txv + (size_t)b0 * plane, ssq, out_mul_host, rpadded, (int)hop, st);
       }
       zero_next_ = 0; zero_off_ = 0; zero_self_ = true;
     }
@@ -1062,7 +1076,7 @@ struct CwtPlan : public CwtPlanBase {
   }
 
   int exec_body(const void* xv, long long B, void* Wxv, void* dWxv, void* Txv, bool ssq,
-                const double* out_mul_host, bool rpadded, cudaStream_t st) {
+                const double* out_mul_host, bool rpadded, int hop, cudaStream_t st) {
     if (B < 1) return set_error(SSQB_E_ARG, "B must be >= 1");
     if (!xv || (!Wxv && !ssq)) return set_error(SSQB_E_ARG, "null x / Wx");   // ssq: Wx may be NULL
     if (ssq && (!Txv || !have_grid))
@@ -1072,7 +1086,7 @@ struct CwtPlan : public CwtPlanBase {
     cx<T>* Wx = (cx<T>*)Wxv; cx<T>* dWx = (cx<T>*)dWxv; cx<T>* Tx = (cx<T>*)Txv;
     long long total_rows = B * d.na;
     if (total_rows > 0x7fffffffll) return set_error(SSQB_E_UNSUPP, "too many rows");
-    long long Nout = rpadded ? d.n_up : d.N;
+    long long Nout = rpadded ? d.n_up : (d.N - 1) / hop + 1;
     const bool use_blocks = fast && have_blocks && !rpadded;
     bool need_join = false;
     int rc = 0;
@@ -1152,7 +1166,7 @@ struct CwtPlan : public CwtPlanBase {
     std::vector<int> sblk_tails;                             // classes launched beside the grid
     auto sblk_rows_args = [&](SblkArgs<T>& S, int c) {
       sblk_args(S, sblk[c], B);
-      S.A.Wx = Wx; S.A.dWx = dWx; S.A.Tx = Tx; S.A.Nout = Nout; S.A.out_mul = out_mul;
+      S.A.Wx = Wx; S.A.dWx = dWx; S.A.Tx = Tx; S.A.Nout = Nout; S.A.hop = hop; S.A.out_mul = out_mul;
       S.write_dWx = dWx ? 1 : 0;
       S.item_ctr = sblk_beside ? sblk_ctr_d.p + c : nullptr;   // alone: fixed stride, no counter
     };
@@ -1201,7 +1215,7 @@ struct CwtPlan : public CwtPlanBase {
           Job J; memset(&J.P, 0, sizeof(J.P));
           block_args(J.P.A, K);
           J.P.A.xh = K.Xb.p; J.P.A.Wx = Wx; J.P.A.dWx = dWx; J.P.A.Tx = Tx;
-          J.P.A.Nout = Nout; J.P.A.out_off = 0; J.P.A.out_mul = out_mul;
+          J.P.A.Nout = Nout; J.P.A.hop = hop; J.P.A.out_off = 0; J.P.A.out_mul = out_mul;
           J.P.rowinfo = K.rows[k].p; J.P.n_rows = K.n_rows[k];
           J.P.tab_off = K.off_d.p; J.P.tab_p = K.p_d.p; J.P.tab_pd = K.pd_d.p;
           J.P.write_dWx = dWx ? 1 : 0; J.P.ssq = ssq ? 1 : 0;
@@ -1251,7 +1265,7 @@ struct CwtPlan : public CwtPlanBase {
     // as Tx is zeroed
     if (fast && have_grid_rows) {
       SSQB_CUDA(V_d.ensure((size_t)B * (size_t)grid_v_total));
-      GridArgs<T> G; grid_args(G, B, Wx, dWx, Tx, ssq, out_mul, rpadded, Nout);
+      GridArgs<T> G; grid_args(G, B, Wx, dWx, Tx, ssq, out_mul, rpadded, Nout, hop);
       cudaStream_t s1 = st, s2 = st;
       if (lanes_on) { s1 = acquire(2, true, false); s2 = acquire(3, true, false); }
       rc = grid_stage_a(G, B, st, s1, s2); if (rc) return rc;
@@ -1272,7 +1286,7 @@ struct CwtPlan : public CwtPlanBase {
         A.row0 = (int)r0; A.nrows = (int)nr; A.rowmap = rowmap;
         A.xh = xh_d.p; A.G = G_d.p; A.G_arr_stride = arr_stride(nr);
         A.Wx = Wx; A.dWx = dWx; A.Tx = Tx;
-        A.Nout = Nout; A.out_off = rpadded ? 0 : d.n1;
+        A.Nout = Nout; A.hop = hop; A.out_off = rpadded ? 0 : d.n1;
         A.out_mul = out_mul;
         FastArgs<T> P; memset(&P, 0, sizeof(P));
         P.A = A; P.rowinfo = nullptr; P.n_rows = 0;
@@ -1306,7 +1320,7 @@ struct CwtPlan : public CwtPlanBase {
         Job J; memset(&J.P, 0, sizeof(J.P));
         base_args(J.P.A);
         J.P.A.xh = xh_d.p; J.P.A.Wx = Wx; J.P.A.dWx = dWx; J.P.A.Tx = Tx;
-        J.P.A.Nout = Nout; J.P.A.out_off = rpadded ? 0 : d.n1; J.P.A.out_mul = out_mul;
+        J.P.A.Nout = Nout; J.P.A.hop = hop; J.P.A.out_off = rpadded ? 0 : d.n1; J.P.A.out_mul = out_mul;
         J.P.rowinfo = qrows_d[c].p; J.P.n_rows = n_qrows[c];
         J.P.tab_off = tab_off_d.p; J.P.tab_p = tab_p_d.p; J.P.tab_pd = tab_pd_d.p;
         J.P.write_dWx = dWx ? 1 : 0; J.P.ssq = ssq ? 1 : 0; J.P.scratch_logR2 = 0;
@@ -1354,9 +1368,11 @@ struct CwtPlan : public CwtPlanBase {
   }
   CwtAdjoint<T> adj;
   int backward(const void* gWx, const void* gdWx, long long B, const double* out_mul_host,
-               bool rpadded, void* gx, cudaStream_t st) override {
+               bool rpadded, long long hop, void* gx, cudaStream_t st) override {
+    { int rc = check_hop(hop, rpadded); if (rc) return rc; }
     CwtArgs<T> A; base_args(A);
-    return adj.run(d, A, (const cx<T>*)gWx, (const cx<T>*)gdWx, B, out_mul_host, rpadded, (T*)gx, st);
+    return adj.run(d, A, (const cx<T>*)gWx, (const cx<T>*)gdWx, B, out_mul_host, rpadded,
+                   hop < d.N ? hop : d.N, (T*)gx, st);
   }
 };
 

@@ -70,8 +70,22 @@ struct CwtArgs {
   // so that only the first group needs a separate zero fill.  zero_next = signals of the next group (0: none), zero_off = elements
   // from this group's Tx[b][a][j] to the next group's
   int zero_next;
+  // time decimation (read by the HOP kernels only): output column j' holds full column j' * hop,
+  // and Nout = (N - 1) / hop + 1 is the stored row length.  Sits in the padding before zero_off,
+  // so the layout the hop = 1 kernels read is unchanged
+  int hop;
   long long zero_off;
 };
+
+// Output column of full column j >= 0 in a HOP kernel: j / hop when hop divides j, -1 otherwise.
+// With Nout = (N - 1) / hop + 1, a multiple of hop below Nout * hop is below N, so the kernels
+// bound j by Nout * hop
+__device__ __forceinline__ int hop_col(int j, int hop) {
+  if ((hop & (hop - 1)) == 0)                         // a power of two: mask and shift
+    return (j & (hop - 1)) ? -1 : j >> (__ffs(hop) - 1);
+  const unsigned q = (unsigned)j / (unsigned)hop;
+  return (q * (unsigned)hop == (unsigned)j) ? (int)q : -1;
+}
 
 // ---- wavelets (ssqueezepy/wavelets.py:525-527, ssqueezepy/_gmw.py:212-219) ----
 template <typename T> __device__ __forceinline__ T t_exp(T x);
@@ -263,9 +277,9 @@ __device__ __forceinline__ bool is_active_fast(T C, T D, double gamma) {
   return is_active_exact(C, D, gamma);
 }
 
-template <typename T, int LOG_F, int NARR, int EPI>
-__global__ void __launch_bounds__(Tile<T>::NT)
-cwt_pass2_kernel(const CwtArgs<T> A, const int write_dWx) {
+// HOP: stores only the columns of a time-decimated call (CwtArgs::hop)
+template <typename T, int LOG_F, int NARR, int EPI, bool HOP>
+__device__ __forceinline__ void cwt_pass2_body(const CwtArgs<T>& A, const int write_dWx) {
   constexpr int NT = Tile<T>::NT;
   constexpr int F = 1 << LOG_F;
   constexpr int R2 = Tile<T>::ELEMS / F;
@@ -324,6 +338,10 @@ cwt_pass2_kernel(const CwtArgs<T> A, const int write_dWx) {
       continue;
     }
     long long j = t - A.out_off;
+    if (HOP) {
+      if (j < 0 || j >= A.Nout * A.hop) continue;
+      j = hop_col((int)j, A.hop);
+    }
     if (j < 0 || j >= A.Nout) continue;
     int b = grow / A.na, a = grow - b * A.na;
     cx<T> dW = mkc<T>((T)0, (T)0);
@@ -354,6 +372,18 @@ cwt_pass2_kernel(const CwtArgs<T> A, const int write_dWx) {
       }
     }
   }
+}
+
+template <typename T, int LOG_F, int NARR, int EPI>
+__global__ void __launch_bounds__(Tile<T>::NT)
+cwt_pass2_kernel(const CwtArgs<T> A, const int write_dWx) {
+  cwt_pass2_body<T, LOG_F, NARR, EPI, false>(A, write_dWx);
+}
+
+template <typename T, int LOG_F, int NARR, int EPI>
+__global__ void __launch_bounds__(Tile<T>::NT)
+cwt_pass2_hop_kernel(const CwtArgs<T> A, const int write_dWx) {
+  cwt_pass2_body<T, LOG_F, NARR, EPI, true>(A, write_dWx);
 }
 
 }  // namespace ssqb

@@ -176,7 +176,8 @@ __device__ __forceinline__ void sblk_twiddles(const cx<T>* __restrict__ tws, int
 }
 
 // STORE_W = false: the fused epilogue without the Wx store (sblk_rows_tx_kernel)
-template <typename T, int LOG_P, int LOG_R, int NARR, bool SSQ, bool STORE_W>
+// HOP: the epilogue runs on the columns of a time-decimated call only (CwtArgs::hop)
+template <typename T, int LOG_P, int LOG_R, int NARR, bool SSQ, bool STORE_W, bool HOP = false>
 __device__ __forceinline__ void sblk_rows_body(const SblkArgs<T>& S) {
   constexpr int P = 1 << LOG_P, R = 1 << LOG_R, NT = P / R;
   static_assert(R == 8 || R == 16, "radix 8 or 16");
@@ -208,6 +209,7 @@ __device__ __forceinline__ void sblk_rows_body(const SblkArgs<T>& S) {
   if (it >= items) return;
 
   const int Nout = (int)A.Nout;
+  const int Nlim = HOP ? Nout * A.hop : Nout;          // bound of the full column
   const T xi_step = (T)(SSQB_TWO_PI / (double)P) / A.dt;
 
 #pragma unroll 1
@@ -354,8 +356,9 @@ __device__ __forceinline__ void sblk_rows_body(const SblkArgs<T>& S) {
 #pragma unroll
     for (int m = 0; m < NOUT; ++m) {
       const int t = j + NT * m;
-      const int jo = jbase + t;
-      if (t >= S.h2 && t < P - S.h2 && jo < Nout) {
+      int jo = jbase + t;
+      if (t >= S.h2 && t < P - S.h2 && jo < Nlim) {
+        if (HOP) { jo = hop_col(jo, A.hop); if (jo < 0) continue; }
         const cx<T> W = vw[m], dW = vd[m];
         if (!SSQ) {
           Wrow[jo] = cscale<T>(W, mlt);
@@ -378,7 +381,8 @@ __device__ __forceinline__ void sblk_rows_body(const SblkArgs<T>& S) {
       exact &= exact - 1;
       const int t = j + NT * m;
       const V4 v = s[t];
-      ssq_point_exact<T>(mkc<T>(v.x, v.y), mkc<T>(v.z, v.w), Tb + (jbase + t), rowbytes, cwide, A.grid);
+      const int jo = HOP ? hop_col(jbase + t, A.hop) : jbase + t;   // a wanted column
+      ssq_point_exact<T>(mkc<T>(v.x, v.y), mkc<T>(v.z, v.w), Tb + jo, rowbytes, cwide, A.grid);
     }
     if (it_next >= items) break;
     it = it_next;
@@ -396,6 +400,13 @@ template <typename T, int LOG_P, int LOG_R>
 __global__ void __launch_bounds__((1 << LOG_P) >> LOG_R, 2)
 sblk_rows_tx_kernel(const SblkArgs<T> S) {
   sblk_rows_body<T, LOG_P, LOG_R, 2, true, false>(S);
+}
+
+// time-decimated call (CwtArgs::hop > 1): either of the two above on the wanted columns only
+template <typename T, int LOG_P, int LOG_R, int NARR, bool SSQ, bool STORE_W>
+__global__ void __launch_bounds__((1 << LOG_P) >> LOG_R, 2)
+sblk_rows_hop_kernel(const SblkArgs<T> S) {
+  sblk_rows_body<T, LOG_P, LOG_R, NARR, SSQ, STORE_W, true>(S);
 }
 
 }  // namespace ssqb

@@ -162,14 +162,15 @@ struct DevBuf {
 struct CwtPlanBase {
   virtual ~CwtPlanBase() {}
   virtual int set_reassign(const ssqb_reassign_desc* r) = 0;
+  // hop: outputs hold every hop-th column, Nout = (N - 1) / hop + 1 (hop > 1 needs !rpadded)
   virtual int exec(const void* x, long long B, void* Wx, void* dWx, void* Tx, bool ssq,
-                   const double* out_mul_host, bool rpadded, cudaStream_t st) = 0;
+                   const double* out_mul_host, bool rpadded, long long hop, cudaStream_t st) = 0;
   virtual int exec_host(const void* x, long long B, void* Wx, void* dWx, void* Tx, bool ssq,
                         const double* out_mul_host, bool rpadded, cudaStream_t st) = 0;
   virtual int debug_xh(const void* x, long long B, void* xh, cudaStream_t st) = 0;
   // adjoint of cwt: gWx / gdWx [B][na][Nout] complex (either may be null) -> gx [B][N] real
   virtual int backward(const void* gWx, const void* gdWx, long long B, const double* out_mul_host,
-                       bool rpadded, void* gx, cudaStream_t st) = 0;
+                       bool rpadded, long long hop, void* gx, cudaStream_t st) = 0;
   virtual int set_profiling(int on) = 0;
   virtual int get_profile(double* ms, long long* launches, long long* rows) = 0;
 };

@@ -32,9 +32,10 @@ def ssq_const(scales, cwt_scaletype, nv, transform='cwt', ssq_freqs=None):
 
 def ssqueeze(Wx, w=None, ssq_freqs=None, scales=None, Sfs=None, fs=None, t=None,
              squeezing='sum', maprange='maximal', wavelet=None, gamma=None,
-             was_padded=True, flipud=False, dWx=None, transform='cwt'):
+             was_padded=True, flipud=False, dWx=None, transform='cwt', N=None):
     """Synchrosqueeze `Wx` ([na, N] or [B, na, N]).  Returns `(Tx, ssq_freqs)`;
-    `Tx` is a CUDA tensor."""
+    `Tx` is a CUDA tensor.  `N`: length of the signal the planes came from, when they
+    hold fewer columns (a `hop_len` transform); the frequencies are derived from it."""
     if w is None and (dWx is None or gamma is None):
         raise ValueError("if `w` is None, `dWx` and `gamma` must not be.")
     if w is not None and float(w.min()) < 0:
@@ -43,7 +44,7 @@ def ssqueeze(Wx, w=None, ssq_freqs=None, scales=None, Sfs=None, fs=None, t=None,
                            wavelet=wavelet)
     if scales is None and transform == 'cwt':
         raise ValueError("`scales` can't be None if `transform == 'cwt'`")
-    N = Wx.shape[-1]
+    N = Wx.shape[-1] if N is None else int(N)
     dt, *_ = _process_fs_and_t(fs, t, N)
 
     if transform == 'cwt':
