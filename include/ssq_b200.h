@@ -270,6 +270,36 @@ int ssqb_ssq_stft2_exec(const ssqb_stft_desc* d, const ssqb_stft2_tables* t,
 int ssqb_stft_backward(const ssqb_stft_desc* d, const void* gSx_dev, const void* gdSx_dev,
                        int64_t B, void* gx_dev, void* stream);
 
+/* ---- time-reassigned synchrosqueezing (TSST; He, Yu et al., MSSP 2019; not in the reference) --
+ * Each coefficient V[k][j] moves along time to its group-delay estimate and keeps its row:
+ *   Ts[k][jt] += V[k][j],   jt = rint((j hop + delay) / hop)      (no weight)
+ * where |V| > gamma (the exact test of ssqb_ssq_stft_exec), delay is finite and 0 <= jt < n_cols.
+ * Every other point is dropped (never clamped).  delay, in samples, is
+ *   STFT  Re(V^{tau g} conj(V^g)) / |V^g|^2,   tau g[l] = (l - n_fft/2) g[l]
+ *   CWT   Im(A / W),                           A = ifft(a psih'(a xi) xh)
+ * computed in float64, one rounding per operation in a fixed order, identically in the forward,
+ * the target planes and the backward.  Ts is zeroed here; its sums use atomics (the order of
+ * additions into one entry is not fixed).  Optional target planes: tgt_dev int32 (target column,
+ * -1 = dropped or below gamma) and, with it, tau_dev in the data dtype (j hop + delay in samples,
+ * inf where tgt is -1).                                                                        */
+/* STFT, fused: d as for ssqb_stft_exec (win_host = g); twin_host [n_fft] data dtype = tau g, in
+ * the layout of win_host (ifftshifted when modulated).  Sx_dev may be NULL (not stored); Vt_dev
+ * [B][n_fft/2+1][n_hops] receives V^{tau g} when not NULL.                                     */
+int ssqb_tssq_stft_exec(const ssqb_stft_desc* d, const void* twin_host, double gamma,
+                        const void* x_dev, int64_t B, void* Sx_dev, void* Ts_dev, void* Vt_dev,
+                        int32_t* tgt_dev, void* tau_dev, void* stream);
+/* CWT: W_dev, A_dev [B][na][n_cols] complex (the columns j * hop of the full planes); Ts_dev the
+ * same shape.                                                                                   */
+int ssqb_tssq_cwt_reassign(int dtype, const void* W_dev, const void* A_dev, int64_t B, int na,
+                           int64_t n_cols, int64_t hop, double gamma, void* Ts_dev,
+                           int32_t* tgt_dev, void* tau_dev, void* stream);
+/* backward of both (torch.autograd), targets held: gVout = gV + gTs[k][jt] at kept points, gV
+ * elsewhere (gV_dev may be NULL = 0 and may alias gVout_dev).  form 0 = STFT (P_dev = V^{tau g}),
+ * 1 = CWT (P_dev = A).  One thread per point, no atomics.  Planes [B][nrows][n_cols].          */
+int ssqb_tssq_backward(int dtype, int form, const void* V_dev, const void* P_dev,
+                       const void* gTs_dev, const void* gV_dev, void* gVout_dev, int64_t B,
+                       int nrows, int64_t n_cols, int64_t hop, double gamma, void* stream);
+
 /* ---- inverse transforms (column reductions / overlap-add) -------------------------- */
 /* Weighted real-part column sum, the core of
  *   issq_cwt  (_ssq_cwt.py:366-377: `Tx.real.sum(axis=0) * (2 / Css)`)

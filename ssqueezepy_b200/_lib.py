@@ -35,6 +35,7 @@ SYMBOLS = [
     'ssqb_stft_backward', 'ssqb_istft_backward', 'ssqb_ssqueeze_backward',
     'ssqb_indexed_sum_backward', 'ssqb_colsum_real_backward', 'ssqb_ssq_cwt2_reassign',
     'ssqb_cwt_exec_hop', 'ssqb_ssq_cwt_exec_hop', 'ssqb_cwt_backward_hop',
+    'ssqb_tssq_stft_exec', 'ssqb_tssq_cwt_reassign', 'ssqb_tssq_backward',
 ]
 
 
@@ -125,6 +126,10 @@ def _bind(lib):
                                             vp, i64, vp, vp, vp, vp]
     lib.ssqb_ssq_stft2_exec.argtypes = [C.POINTER(StftDesc), C.POINTER(Stft2Tables),
                                         C.POINTER(ReassignDesc), vp, i64, vp, vp, vp, vp, vp]
+    lib.ssqb_tssq_stft_exec.argtypes = [C.POINTER(StftDesc), vp, dbl, vp, i64, vp, vp, vp, vp,
+                                        vp, vp]
+    lib.ssqb_tssq_cwt_reassign.argtypes = [ci, vp, vp, i64, ci, i64, i64, dbl, vp, vp, vp, vp]
+    lib.ssqb_tssq_backward.argtypes = [ci, ci, vp, vp, vp, vp, vp, i64, ci, i64, i64, dbl, vp]
     lib.ssqb_colsum_real.argtypes = [ci, ci, vp, i64, ci, i64, C.POINTER(dbl), dbl, ci, vp, vp]
     lib.ssqb_invert_components.argtypes = [ci, vp, ci, i64, vp, vp, ci, dbl, vp, vp]
     lib.ssqb_istft_exec.argtypes = [C.POINTER(IstftDesc), vp, i64, vp, vp]

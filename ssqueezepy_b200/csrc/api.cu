@@ -298,6 +298,25 @@ int ssqb_istft_backward(const ssqb_istft_desc* d, const void* gx, int64_t B, voi
   return run_istft_backward(d, gx, B, gSx, (cudaStream_t)stream);
 }
 
+int ssqb_tssq_stft_exec(const ssqb_stft_desc* d, const void* twin_host, double gamma,
+                        const void* x, int64_t B, void* Sx, void* Ts, void* Vt, int32_t* tgt,
+                        void* tau, void* stream) {
+  return run_tssq_stft(d, twin_host, gamma, x, B, Sx, Ts, Vt, tgt, tau, (cudaStream_t)stream);
+}
+
+int ssqb_tssq_cwt_reassign(int dtype, const void* W, const void* A, int64_t B, int na,
+                           int64_t n_cols, int64_t hop, double gamma, void* Ts, int32_t* tgt,
+                           void* tau, void* stream) {
+  return run_tssq_cwt(dtype, W, A, B, na, n_cols, hop, gamma, Ts, tgt, tau, (cudaStream_t)stream);
+}
+
+int ssqb_tssq_backward(int dtype, int form, const void* V, const void* P, const void* gTs,
+                       const void* gV, void* gVout, int64_t B, int nrows, int64_t n_cols,
+                       int64_t hop, double gamma, void* stream) {
+  return run_tssq_backward(dtype, form, V, P, gTs, gV, gVout, B, nrows, n_cols, hop, gamma,
+                           (cudaStream_t)stream);
+}
+
 int ssqb_extract_ridges(int dtype, const void* Tf, int64_t B, int na, int64_t N, const double* ls_host,
                         const double* scales_host, double penalty, double eps, int n_ridges, int bw,
                         int64_t* idx_dev, void* f_dev, void* e_dev, void* stream) {

@@ -202,6 +202,14 @@ int run_stft2(const ssqb_stft_desc* d, const ssqb_stft2_tables* t2, const ssqb_r
               const void* x, long long B, void* Sx, void* Tx, void* dSx, void* w, cudaStream_t st);
 int run_stft_backward(const ssqb_stft_desc* d, const void* gSx, const void* gdSx, long long B,
                       void* gx, cudaStream_t st);
+// time-reassigned synchrosqueezing (stft_ops.cu, tssq_ops.cu)
+int run_tssq_stft(const ssqb_stft_desc* d, const void* twin_host, double gamma, const void* x,
+                  long long B, void* Sx, void* Ts, void* Vt, int* tgt, void* tau, cudaStream_t st);
+int run_tssq_cwt(int dtype, const void* W, const void* Ap, long long B, int na, long long ncols,
+                 long long hop, double gamma, void* Ts, int* tgt, void* tau, cudaStream_t st);
+int run_tssq_backward(int dtype, int form, const void* V, const void* P, const void* gTs,
+                      const void* gV, void* gVout, long long B, int nrows, long long ncols,
+                      long long hop, double gamma, cudaStream_t st);
 int run_istft_backward(const ssqb_istft_desc* d, const void* gx, long long B, void* gSx,
                        cudaStream_t st);
 // inverse_ops.cu

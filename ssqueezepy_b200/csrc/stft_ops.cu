@@ -1,6 +1,7 @@
 // Host dispatch of the STFT / ssq_stft kernels.
 #include "host_common.h"
 #include "stft_kernels.cuh"
+#include "tssq_kernels.cuh"
 #include "inverse_kernels.cuh"   // IstftArgs, istft_bwd_norm_kernel
 #include "cwt_generic.cuh"      // Gfft<T>: generic-length FFT
 #include <algorithm>
@@ -420,6 +421,84 @@ int run_stft2(const ssqb_stft_desc* d, const ssqb_stft2_tables* t2, const ssqb_r
   if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
   return d->dtype == SSQB_F32 ? stft2_t<float>(d, t2, r, x, B, Sx, Tx, dSx, w, st)
                               : stft2_t<double>(d, t2, r, x, B, Sx, Tx, dSx, w, st);
+}
+
+// ---- time-reassigned ssq_stft (tssq_kernels.cuh) ---------------------------------------------
+// The first order's routes with tau g in place of g': tssq_stft_pow2_kernel for n_fft = 2 .. 4096,
+// otherwise stft_frames_kernel -> Gfft -> tssq_stft_emit_kernel in generic_frames' chunks.
+template <typename T, int EPI>
+static int launch_tssq_stft(const TssqStftArgs<T>& P, cudaStream_t st) {
+  const StftArgs<T>& A = P.A;
+  const long long total = (long long)A.B * A.n_hops;
+  if (stft_pow2_tile(A.n_fft)) {
+    return dispatch_log2<1, 12>(ilog2_exact(A.n_fft), [&](auto L) {
+      constexpr int M = 1 << L; constexpr int R = Tile<T>::ELEMS / M;
+      const size_t smem = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);
+      auto kern = tssq_stft_pow2_kernel<T, L, EPI>;
+      SSQB_CUDA(opt_in_smem(kern, smem));
+      kern<<<(unsigned)((total + R - 1) / R), Tile<T>::NT, smem, st>>>(P);
+      SSQB_LAUNCH_CHECK();
+      return 0;
+    });
+  }
+  const long long M = A.n_fft, nrows = M / 2 + 1;
+  return generic_frames<T>(A.n_fft, total, 1, -1,
+      [&](cx<T>* c, long long f0, long long nf) {
+        stft_frames_kernel<T, STFT_EPI_PLAIN><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(A, c, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      },
+      [&](const cx<T>* C, long long f0, long long nf) {
+        tssq_stft_emit_kernel<T, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(P, C, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      }, st);
+}
+
+template <typename T>
+static int tssq_stft_t(const ssqb_stft_desc* d, const void* twin_host, double gamma, const void* x,
+                       long long B, void* Sx, void* Ts, void* Vt, int* tgt, void* tau,
+                       cudaStream_t st) {
+  const int M = d->n_fft, nrows = M / 2 + 1;
+  TssqStftArgs<T> P;
+  memset(&P, 0, sizeof(P));
+  StftArgs<T>& A = P.A;
+  A.N = d->N; A.n_fft = M; A.hop = d->hop; A.n1 = d->n1; A.padtype = d->padtype;
+  A.modulated = d->modulated; A.B = (int)B;
+  A.n_hops = (d->N - 1) / d->hop + 1;
+  A.x = (const T*)x; A.Sx = (cx<T>*)Sx; A.dSx = (cx<T>*)Vt; A.Tx = (cx<T>*)Ts;
+  A.write_dSx = Vt ? 1 : 0;
+  A.grid.gamma = gamma;
+  P.tgt = tgt; P.tau = (T*)tau;
+  const T* win = (const T*)d->win_host; const T* twin = (const T*)twin_host;
+  const double kap = pack_kappa(win, twin, M);
+  A.kappa = (T)kap; A.inv_kappa = (T)(1.0 / kap);
+  BlobBuilder bb;
+  const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
+  const size_t o_win = bb.put(win, sizeof(T) * M);
+  const size_t o_twin = bb.put(twin, sizeof(T) * M);
+  unsigned char* blob = nullptr;
+  int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
+  A.tw = (const cx<T>*)(blob + o_tw);
+  A.win = (const T*)(blob + o_win); A.dwin = (const T*)(blob + o_twin);
+  SSQB_CUDA(cudaMemsetAsync(Ts, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(cx<T>), st));
+  switch ((Sx ? TSSQ_EPI_SX : 0) | (tgt ? TSSQ_EPI_TGT : 0)) {
+    case 0: return launch_tssq_stft<T, 0>(P, st);
+    case TSSQ_EPI_SX: return launch_tssq_stft<T, TSSQ_EPI_SX>(P, st);
+    case TSSQ_EPI_TGT: return launch_tssq_stft<T, TSSQ_EPI_TGT>(P, st);
+    default: return launch_tssq_stft<T, TSSQ_EPI_SX | TSSQ_EPI_TGT>(P, st);
+  }
+}
+
+int run_tssq_stft(const ssqb_stft_desc* d, const void* twin_host, double gamma, const void* x,
+                  long long B, void* Sx, void* Ts, void* Vt, int* tgt, void* tau, cudaStream_t st) {
+  if (!d || !x || !Ts) return set_error(SSQB_E_ARG, "null pointer");
+  if (!d->win_host || !twin_host) return set_error(SSQB_E_ARG, "null table");
+  if (tau && !tgt) return set_error(SSQB_E_ARG, "tau needs the target plane");
+  if (!(gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
+  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
+  return d->dtype == SSQB_F32 ? tssq_stft_t<float>(d, twin_host, gamma, x, B, Sx, Ts, Vt, tgt, tau, st)
+                              : tssq_stft_t<double>(d, twin_host, gamma, x, B, Sx, Ts, Vt, tgt, tau, st);
 }
 
 }  // namespace ssqb
