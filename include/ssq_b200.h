@@ -300,6 +300,38 @@ int ssqb_tssq_backward(int dtype, int form, const void* V_dev, const void* P_dev
                        const void* gTs_dev, const void* gV_dev, void* gVout_dev, int64_t B,
                        int nrows, int64_t n_cols, int64_t hop, double gamma, void* stream);
 
+/* ---- reassigned spectrogram / scalogram (Auger & Flandrin, IEEE TSP 1995; not in the
+ * reference) -- the energy of every point moves in time and frequency at once:
+ *   Rx[kk][jt] += |V[k][j]|^2        (real plane of the data dtype, the shape of Tx)
+ * kk is the row the first-order fused ssq_* route gives the point (w = |Sfs[k] - r| for the
+ * STFT, |r| for the CWT, on the grid of r, flip included), jt the tssq_* target column.  A point
+ * is kept when |V| > gamma, its delay is finite and 0 <= jt < n_cols, exactly the kept set of
+ * tssq_*; every other point is dropped.  |V|^2 is formed in float64 and cast once to the data
+ * dtype.  Rx is zeroed here; its sums use atomics (the order of additions is not fixed).
+ * Optional target planes: kk_dev and jt_dev int32 (-1 = dropped), given together, and with them
+ * w_dev (the reassigned frequency in Hz) and tau_dev (j hop + delay in samples) in the data
+ * dtype, inf where dropped.                                                                    */
+/* STFT, fused: d and r as for ssqb_ssq_stft_exec; twin_host as for ssqb_tssq_stft_exec.  Sx_dev,
+ * dSx_dev and Vt_dev (V^{tau g}) [B][n_fft/2+1][n_hops] are stored when not NULL.              */
+int ssqb_rs_stft_exec(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reassign_desc* r,
+                      double gamma, const void* x_dev, int64_t B, void* Sx_dev, void* Rx_dev,
+                      void* dSx_dev, void* Vt_dev, int32_t* kk_dev, int32_t* jt_dev, void* w_dev,
+                      void* tau_dev, void* stream);
+/* CWT: W_dev, dW_dev, A_dev [B][na][n_cols] complex (the columns j * hop of the full planes), r
+ * the descriptor of the fused ssq_cwt; Rx_dev and the target planes the same shape.           */
+int ssqb_rs_cwt_reassign(int dtype, const void* W_dev, const void* dW_dev, const void* A_dev,
+                         const ssqb_reassign_desc* r, int64_t B, int na, int64_t n_cols,
+                         int64_t hop, double gamma, void* Rx_dev, int32_t* kk_dev,
+                         int32_t* jt_dev, void* w_dev, void* tau_dev, void* stream);
+/* backward of both (torch.autograd), targets held: gVout = gV + 2 gRx[kk][jt] V at kept points,
+ * gV elsewhere (gV_dev may be NULL = 0 and may alias gVout_dev).  form 0 = STFT (P1 = dSx,
+ * P2 = V^{tau g}, Sfs_dev [nrows] in the data dtype), 1 = CWT (P1 = dW, P2 = A, Sfs_dev NULL).
+ * One thread per point, no atomics.  Planes [B][nrows][n_cols]; gRx_dev real.                 */
+int ssqb_rs_backward(int dtype, int form, const void* V_dev, const void* P1_dev,
+                     const void* P2_dev, const void* Sfs_dev, const ssqb_reassign_desc* r,
+                     const void* gRx_dev, const void* gV_dev, void* gVout_dev, int64_t B,
+                     int nrows, int64_t n_cols, int64_t hop, double gamma, void* stream);
+
 /* ---- inverse transforms (column reductions / overlap-add) -------------------------- */
 /* Weighted real-part column sum, the core of
  *   issq_cwt  (_ssq_cwt.py:366-377: `Tx.real.sum(axis=0) * (2 / Css)`)

@@ -36,6 +36,7 @@ SYMBOLS = [
     'ssqb_indexed_sum_backward', 'ssqb_colsum_real_backward', 'ssqb_ssq_cwt2_reassign',
     'ssqb_cwt_exec_hop', 'ssqb_ssq_cwt_exec_hop', 'ssqb_cwt_backward_hop',
     'ssqb_tssq_stft_exec', 'ssqb_tssq_cwt_reassign', 'ssqb_tssq_backward',
+    'ssqb_rs_stft_exec', 'ssqb_rs_cwt_reassign', 'ssqb_rs_backward',
 ]
 
 
@@ -130,6 +131,12 @@ def _bind(lib):
                                         vp, vp]
     lib.ssqb_tssq_cwt_reassign.argtypes = [ci, vp, vp, i64, ci, i64, i64, dbl, vp, vp, vp, vp]
     lib.ssqb_tssq_backward.argtypes = [ci, ci, vp, vp, vp, vp, vp, i64, ci, i64, i64, dbl, vp]
+    lib.ssqb_rs_stft_exec.argtypes = [C.POINTER(StftDesc), vp, C.POINTER(ReassignDesc), dbl, vp,
+                                      i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.ssqb_rs_cwt_reassign.argtypes = [ci, vp, vp, vp, C.POINTER(ReassignDesc), i64, ci, i64,
+                                         i64, dbl, vp, vp, vp, vp, vp, vp]
+    lib.ssqb_rs_backward.argtypes = [ci, ci, vp, vp, vp, vp, C.POINTER(ReassignDesc), vp, vp, vp,
+                                     i64, ci, i64, i64, dbl, vp]
     lib.ssqb_colsum_real.argtypes = [ci, ci, vp, i64, ci, i64, C.POINTER(dbl), dbl, ci, vp, vp]
     lib.ssqb_invert_components.argtypes = [ci, vp, ci, i64, vp, vp, ci, dbl, vp, vp]
     lib.ssqb_istft_exec.argtypes = [C.POINTER(IstftDesc), vp, i64, vp, vp]

@@ -317,6 +317,29 @@ int ssqb_tssq_backward(int dtype, int form, const void* V, const void* P, const 
                            (cudaStream_t)stream);
 }
 
+int ssqb_rs_stft_exec(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reassign_desc* r,
+                      double gamma, const void* x, int64_t B, void* Sx, void* Rx, void* dSx,
+                      void* Vt, int32_t* kk, int32_t* jt, void* w, void* tau, void* stream) {
+  return run_rs_stft(d, twin_host, r, gamma, x, B, Sx, Rx, dSx, Vt, kk, jt, w, tau,
+                     (cudaStream_t)stream);
+}
+
+int ssqb_rs_cwt_reassign(int dtype, const void* W, const void* dW, const void* A,
+                         const ssqb_reassign_desc* r, int64_t B, int na, int64_t n_cols,
+                         int64_t hop, double gamma, void* Rx, int32_t* kk, int32_t* jt, void* w,
+                         void* tau, void* stream) {
+  return run_rs_cwt(dtype, W, dW, A, r, B, na, n_cols, hop, gamma, Rx, kk, jt, w, tau,
+                    (cudaStream_t)stream);
+}
+
+int ssqb_rs_backward(int dtype, int form, const void* V, const void* P1, const void* P2,
+                     const void* Sfs, const ssqb_reassign_desc* r, const void* gRx,
+                     const void* gV, void* gVout, int64_t B, int nrows, int64_t n_cols,
+                     int64_t hop, double gamma, void* stream) {
+  return run_rs_backward(dtype, form, V, P1, P2, Sfs, r, gRx, gV, gVout, B, nrows, n_cols, hop,
+                         gamma, (cudaStream_t)stream);
+}
+
 int ssqb_extract_ridges(int dtype, const void* Tf, int64_t B, int na, int64_t N, const double* ls_host,
                         const double* scales_host, double penalty, double eps, int n_ridges, int bw,
                         int64_t* idx_dev, void* f_dev, void* e_dev, void* stream) {

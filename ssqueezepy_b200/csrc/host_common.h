@@ -210,6 +210,17 @@ int run_tssq_cwt(int dtype, const void* W, const void* Ap, long long B, int na, 
 int run_tssq_backward(int dtype, int form, const void* V, const void* P, const void* gTs,
                       const void* gV, void* gVout, long long B, int nrows, long long ncols,
                       long long hop, double gamma, cudaStream_t st);
+// reassigned spectrogram / scalogram (stft_ops.cu, rs_ops.cu)
+int run_rs_stft(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reassign_desc* r,
+                double gamma, const void* x, long long B, void* Sx, void* Rx, void* dSx, void* Vt,
+                int* kk, int* jt, void* w, void* tau, cudaStream_t st);
+int run_rs_cwt(int dtype, const void* W, const void* dW, const void* Ap,
+               const ssqb_reassign_desc* r, long long B, int na, long long ncols, long long hop,
+               double gamma, void* Rx, int* kk, int* jt, void* w, void* tau, cudaStream_t st);
+int run_rs_backward(int dtype, int form, const void* V, const void* P1, const void* P2,
+                    const void* Sfs, const ssqb_reassign_desc* r, const void* gRx,
+                    const void* gV, void* gVout, long long B, int nrows, long long ncols,
+                    long long hop, double gamma, cudaStream_t st);
 int run_istft_backward(const ssqb_istft_desc* d, const void* gx, long long B, void* gSx,
                        cudaStream_t st);
 // inverse_ops.cu

@@ -2,6 +2,7 @@
 #include "host_common.h"
 #include "stft_kernels.cuh"
 #include "tssq_kernels.cuh"
+#include "rs_kernels.cuh"
 #include "inverse_kernels.cuh"   // IstftArgs, istft_bwd_norm_kernel
 #include "cwt_generic.cuh"      // Gfft<T>: generic-length FFT
 #include <algorithm>
@@ -499,6 +500,109 @@ int run_tssq_stft(const ssqb_stft_desc* d, const void* twin_host, double gamma, 
   if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
   return d->dtype == SSQB_F32 ? tssq_stft_t<float>(d, twin_host, gamma, x, B, Sx, Ts, Vt, tgt, tau, st)
                               : tssq_stft_t<double>(d, twin_host, gamma, x, B, Sx, Ts, Vt, tgt, tau, st);
+}
+
+// ---- reassigned spectrogram (rs_kernels.cuh) -------------------------------------------------
+// Power-of-two n_fft whose 2F transforms per tile fit one CTA (float32 up to 4096, float64 up to
+// 2048): rs_stft_pow2_kernel.  Every other n_fft: stft_frames_kernel (the g / g' sequences) and
+// rs_tau_frames_kernel (tau g) -> one batched Gfft of 2 transforms per frame -> the emit kernel.
+template <typename T>
+static bool rs_pow2_fits(int logm) {
+  return logm >= 1 && logm <= 12 &&
+         dispatch_log2<1, 12>(logm, [](auto L) { return RsTile<T, L>::SMEM <= kMaxBlockSmem ? 1 : 0; });
+}
+
+template <typename T, int EPI>
+static int launch_rs_stft(const RsStftArgs<T>& P, cudaStream_t st) {
+  const StftArgs<T>& A = P.A;
+  const long long total = (long long)A.B * A.n_hops;
+  const int logm = ilog2_exact(A.n_fft);
+  if (rs_pow2_fits<T>(logm)) {
+    return dispatch_log2<1, 12>(logm, [&](auto L) {
+      using TL = RsTile<T, L>;
+      if constexpr (TL::SMEM > kMaxBlockSmem) {
+        return set_error(SSQB_E_UNSUPP, "n_fft = 2^%d does not fit one CTA", (int)L);
+      } else {
+        auto kern = rs_stft_pow2_kernel<T, L, EPI>;
+        SSQB_CUDA(opt_in_smem(kern, TL::SMEM));
+        kern<<<(unsigned)((total + TL::F - 1) / TL::F), Tile<T>::NT, TL::SMEM, st>>>(P);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      }
+    });
+  }
+  const long long M = A.n_fft, nrows = M / 2 + 1;
+  return generic_frames<T>(A.n_fft, total, 2, -1,
+      [&](cx<T>* c, long long f0, long long nf) {
+        const unsigned nb = (unsigned)((nf * M + 255) / 256);
+        stft_frames_kernel<T, STFT_EPI_PLAIN><<<nb, 256, 0, st>>>(A, c, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        rs_tau_frames_kernel<T><<<nb, 256, 0, st>>>(P, c + nf * M, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      },
+      [&](const cx<T>* C, long long f0, long long nf) {
+        rs_stft_emit_kernel<T, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(P, C, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      }, st);
+}
+
+template <typename T>
+static int rs_stft_t(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reassign_desc* r,
+                     double gamma, const void* x, long long B, void* Sx, void* Rx, void* dSx,
+                     void* Vt, int* kk, int* jt, void* w, void* tau, cudaStream_t st) {
+  const int M = d->n_fft, nrows = M / 2 + 1;
+  RsStftArgs<T> P;
+  memset(&P, 0, sizeof(P));
+  StftArgs<T>& A = P.A;
+  A.N = d->N; A.n_fft = M; A.hop = d->hop; A.n1 = d->n1; A.padtype = d->padtype;
+  A.modulated = d->modulated; A.B = (int)B;
+  A.n_hops = (d->N - 1) / d->hop + 1;
+  A.x = (const T*)x; A.Sx = (cx<T>*)Sx; A.dSx = (cx<T>*)dSx;
+  A.write_dSx = dSx ? 1 : 0;
+  P.Rx = (T*)Rx; P.Vt = (cx<T>*)Vt;
+  P.tp.kk = kk; P.tp.jt = jt; P.tp.w = (T*)w; P.tp.tau = (T*)tau;
+  const T* win = (const T*)d->win_host; const T* dwin = (const T*)d->dwin_host;
+  const double kap = pack_kappa(win, dwin, M);                 // the packing of ssq_stft
+  A.kappa = (T)kap; A.inv_kappa = (T)(1.0 / kap);
+  BlobBuilder bb;
+  const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
+  const size_t o_win = bb.put(win, sizeof(T) * M);
+  const size_t o_dwin = bb.put(dwin, sizeof(T) * M);
+  const size_t o_twin = bb.put(twin_host, sizeof(T) * M);
+  const size_t o_sfs = bb.put(d->Sfs_host, sizeof(T) * nrows);
+  unsigned char* blob = nullptr;
+  int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
+  A.tw = (const cx<T>*)(blob + o_tw);
+  A.win = (const T*)(blob + o_win); A.dwin = (const T*)(blob + o_dwin);
+  A.Sfs = (const T*)(blob + o_sfs);
+  P.twin = (const T*)(blob + o_twin);
+  rc = fill_grid(r, nrows, &A.grid); if (rc) return rc;
+  A.grid.kind = 3;
+  A.grid.gamma = gamma;
+  SSQB_CUDA(cudaMemsetAsync(Rx, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(T), st));
+  switch ((Sx ? RS_EPI_SX : 0) | (jt ? RS_EPI_TGT : 0)) {
+    case 0: return launch_rs_stft<T, 0>(P, st);
+    case RS_EPI_SX: return launch_rs_stft<T, RS_EPI_SX>(P, st);
+    case RS_EPI_TGT: return launch_rs_stft<T, RS_EPI_TGT>(P, st);
+    default: return launch_rs_stft<T, RS_EPI_SX | RS_EPI_TGT>(P, st);
+  }
+}
+
+int run_rs_stft(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reassign_desc* r,
+                double gamma, const void* x, long long B, void* Sx, void* Rx, void* dSx, void* Vt,
+                int* kk, int* jt, void* w, void* tau, cudaStream_t st) {
+  if (!d || !r || !x || !Rx) return set_error(SSQB_E_ARG, "null pointer");
+  if (!d->win_host || !d->dwin_host || !d->Sfs_host || !twin_host)
+    return set_error(SSQB_E_ARG, "null table");
+  if (!kk != !jt) return set_error(SSQB_E_ARG, "kk and jt go together");
+  if ((w || tau) && !jt) return set_error(SSQB_E_ARG, "w and tau need the target planes");
+  if (!(gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
+  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
+  return d->dtype == SSQB_F32
+             ? rs_stft_t<float>(d, twin_host, r, gamma, x, B, Sx, Rx, dSx, Vt, kk, jt, w, tau, st)
+             : rs_stft_t<double>(d, twin_host, r, gamma, x, B, Sx, Rx, dSx, Vt, kk, jt, w, tau, st);
 }
 
 }  // namespace ssqb
