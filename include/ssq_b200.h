@@ -332,6 +332,40 @@ int ssqb_rs_backward(int dtype, int form, const void* V_dev, const void* P1_dev,
                      const void* gRx_dev, const void* gV_dev, void* gVout_dev, int64_t B,
                      int nrows, int64_t n_cols, int64_t hop, double gamma, void* stream);
 
+/* ---- multisynchrosqueezing (MSST; Yu, Wang & Zhao, IEEE Trans. Ind. Electron. 2019; not in
+ * the reference) -- the first-order frequency reassignment applied again at the row where the
+ * previous step put the coefficient.  For a point (k, j) with |V| > gamma (r->gamma):
+ *   beta = b(k, j); up to n_iter - 1 times: r = row_of_bin[beta]; stop if |V[r][j]| <= gamma;
+ *   beta = b(r, j).   Tx[flip(beta)][j] += V[k][j] cst[k]
+ * b is the bin the fused first-order ssq_* route gives the point before its flip (w = |Sfs[k] - r|
+ * for the STFT, |r| for the CWT, on the grid of r).  Weights, typing and the kept set are the
+ * first order's, so the column sums of Tx are those of ssq_*.  1 <= n_iter <= 64; the rows are at
+ * most 32767.  Optional tgt_dev: int32 plane with the shape of Tx, the final row after the flip,
+ * -1 where a point is dropped.                                                                */
+/* STFT, fused: d and r as for ssqb_ssq_stft_exec (row_of_bin is the identity).  Tx_dev is zeroed
+ * here and added with red.add; Sx_dev and dSx_dev are stored when not NULL (ssq_stft's bits on
+ * the power-of-two route).                                                                    */
+int ssqb_mssq_stft_exec(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, int n_iter,
+                        const void* x_dev, int64_t B, void* Sx_dev, void* Tx_dev, void* dSx_dev,
+                        int32_t* tgt_dev, void* stream);
+/* CWT: W_dev, dW_dev [B][na][n_cols] complex (any plan, any hop), r the descriptor of the fused
+ * ssq_cwt, row_of_bin_host [na] the scale row read after landing in each bin.  Every entry of
+ * Tx_dev is written (no zero fill needed); each entry adds its points in ascending source row,
+ * so Tx is bit-reproducible and independent of the batch.                                    */
+int ssqb_mssq_cwt_reassign(int dtype, const void* W_dev, const void* dW_dev,
+                           const ssqb_reassign_desc* r, const int32_t* row_of_bin_host,
+                           int n_iter, int64_t B, int na, int64_t n_cols, void* Tx_dev,
+                           int32_t* tgt_dev, void* stream);
+/* backward of both (torch.autograd), targets held: gVout = gV + cst[k] gTx[t(k, j)][j] at kept
+ * points, gV elsewhere (gV_dev may be NULL = 0 and may alias gVout_dev).  form 0 = STFT
+ * (Sfs_dev [nrows] in the data dtype, row_of_bin_host NULL), 1 = CWT (row_of_bin_host [nrows],
+ * Sfs_dev NULL).  No atomics.  Planes [B][nrows][n_cols].                                      */
+int ssqb_mssq_backward(int dtype, int form, const void* V_dev, const void* dV_dev,
+                       const void* Sfs_dev, const ssqb_reassign_desc* r,
+                       const int32_t* row_of_bin_host, int n_iter, const void* gTx_dev,
+                       const void* gV_dev, void* gVout_dev, int64_t B, int nrows, int64_t n_cols,
+                       void* stream);
+
 /* ---- inverse transforms (column reductions / overlap-add) -------------------------- */
 /* Weighted real-part column sum, the core of
  *   issq_cwt  (_ssq_cwt.py:366-377: `Tx.real.sum(axis=0) * (2 / Css)`)

@@ -16,6 +16,7 @@ from ._ssq_cwt import ssq_cwt, issq_cwt, phase_cwt
 from ._ssq_stft import ssq_stft, issq_stft, phase_stft
 from ._tssq import tssq_stft, tssq_cwt
 from ._reassigned import reassigned_stft, reassigned_cwt
+from ._mssq import mssq_stft, mssq_cwt
 from .ssqueezing import ssqueeze
 from .experimental import phase_ssqueeze, phase_transform
 from .ridge_extraction import extract_ridges

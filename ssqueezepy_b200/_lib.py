@@ -37,6 +37,7 @@ SYMBOLS = [
     'ssqb_cwt_exec_hop', 'ssqb_ssq_cwt_exec_hop', 'ssqb_cwt_backward_hop',
     'ssqb_tssq_stft_exec', 'ssqb_tssq_cwt_reassign', 'ssqb_tssq_backward',
     'ssqb_rs_stft_exec', 'ssqb_rs_cwt_reassign', 'ssqb_rs_backward',
+    'ssqb_mssq_stft_exec', 'ssqb_mssq_cwt_reassign', 'ssqb_mssq_backward',
 ]
 
 
@@ -137,6 +138,12 @@ def _bind(lib):
                                          i64, dbl, vp, vp, vp, vp, vp, vp]
     lib.ssqb_rs_backward.argtypes = [ci, ci, vp, vp, vp, vp, C.POINTER(ReassignDesc), vp, vp, vp,
                                      i64, ci, i64, i64, dbl, vp]
+    lib.ssqb_mssq_stft_exec.argtypes = [C.POINTER(StftDesc), C.POINTER(ReassignDesc), ci, vp, i64,
+                                        vp, vp, vp, vp, vp]
+    lib.ssqb_mssq_cwt_reassign.argtypes = [ci, vp, vp, C.POINTER(ReassignDesc), vp, ci, i64, ci,
+                                           i64, vp, vp, vp]
+    lib.ssqb_mssq_backward.argtypes = [ci, ci, vp, vp, vp, C.POINTER(ReassignDesc), vp, ci, vp, vp,
+                                       vp, i64, ci, i64, vp]
     lib.ssqb_colsum_real.argtypes = [ci, ci, vp, i64, ci, i64, C.POINTER(dbl), dbl, ci, vp, vp]
     lib.ssqb_invert_components.argtypes = [ci, vp, ci, i64, vp, vp, ci, dbl, vp, vp]
     lib.ssqb_istft_exec.argtypes = [C.POINTER(IstftDesc), vp, i64, vp, vp]

@@ -340,6 +340,27 @@ int ssqb_rs_backward(int dtype, int form, const void* V, const void* P1, const v
                          gamma, (cudaStream_t)stream);
 }
 
+int ssqb_mssq_stft_exec(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, int n_iter,
+                        const void* x, int64_t B, void* Sx, void* Tx, void* dSx, int32_t* tgt,
+                        void* stream) {
+  return run_mssq_stft(d, r, n_iter, x, B, Sx, Tx, dSx, tgt, (cudaStream_t)stream);
+}
+
+int ssqb_mssq_cwt_reassign(int dtype, const void* W, const void* dW, const ssqb_reassign_desc* r,
+                           const int32_t* row_of_bin, int n_iter, int64_t B, int na,
+                           int64_t n_cols, void* Tx, int32_t* tgt, void* stream) {
+  return run_mssq_cwt(dtype, W, dW, r, row_of_bin, n_iter, B, na, n_cols, Tx, tgt,
+                      (cudaStream_t)stream);
+}
+
+int ssqb_mssq_backward(int dtype, int form, const void* V, const void* dV, const void* Sfs,
+                       const ssqb_reassign_desc* r, const int32_t* row_of_bin, int n_iter,
+                       const void* gTx, const void* gV, void* gVout, int64_t B, int nrows,
+                       int64_t n_cols, void* stream) {
+  return run_mssq_backward(dtype, form, V, dV, Sfs, r, row_of_bin, n_iter, gTx, gV, gVout, B,
+                           nrows, n_cols, (cudaStream_t)stream);
+}
+
 int ssqb_extract_ridges(int dtype, const void* Tf, int64_t B, int na, int64_t N, const double* ls_host,
                         const double* scales_host, double penalty, double eps, int n_ridges, int bw,
                         int64_t* idx_dev, void* f_dev, void* e_dev, void* stream) {

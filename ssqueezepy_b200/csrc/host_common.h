@@ -221,6 +221,17 @@ int run_rs_backward(int dtype, int form, const void* V, const void* P1, const vo
                     const void* Sfs, const ssqb_reassign_desc* r, const void* gRx,
                     const void* gV, void* gVout, long long B, int nrows, long long ncols,
                     long long hop, double gamma, cudaStream_t st);
+// multisynchrosqueezing (stft_ops.cu, mssq_ops.cu)
+int run_mssq_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, int n_iter,
+                  const void* x, long long B, void* Sx, void* Tx, void* dSx, int* tgt,
+                  cudaStream_t st);
+int run_mssq_cwt(int dtype, const void* W, const void* dW, const ssqb_reassign_desc* r,
+                 const int* rob_host, int n_iter, long long B, int na, long long ncols, void* Tx,
+                 int* tgt, cudaStream_t st);
+int run_mssq_backward(int dtype, int form, const void* V, const void* dV, const void* Sfs,
+                      const ssqb_reassign_desc* r, const int* rob_host, int n_iter,
+                      const void* gTx, const void* gV, void* gVout, long long B, int nrows,
+                      long long ncols, cudaStream_t st);
 int run_istft_backward(const ssqb_istft_desc* d, const void* gx, long long B, void* gSx,
                        cudaStream_t st);
 // inverse_ops.cu

@@ -3,6 +3,7 @@
 #include "stft_kernels.cuh"
 #include "tssq_kernels.cuh"
 #include "rs_kernels.cuh"
+#include "mssq_kernels.cuh"
 #include "inverse_kernels.cuh"   // IstftArgs, istft_bwd_norm_kernel
 #include "cwt_generic.cuh"      // Gfft<T>: generic-length FFT
 #include <algorithm>
@@ -603,6 +604,106 @@ int run_rs_stft(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reass
   return d->dtype == SSQB_F32
              ? rs_stft_t<float>(d, twin_host, r, gamma, x, B, Sx, Rx, dSx, Vt, kk, jt, w, tau, st)
              : rs_stft_t<double>(d, twin_host, r, gamma, x, B, Sx, Rx, dSx, Vt, kk, jt, w, tau, st);
+}
+
+// ---- multisynchrosqueezed STFT (mssq_kernels.cuh) --------------------------------------------
+// Power-of-two n_fft whose ssq_stft tile and bins fit one CTA: mssq_stft_pow2_kernel.  Every other
+// n_fft: stft_frames_kernel -> Gfft -> mssq_stft_emit_kernel (one CTA per frame), in
+// generic_frames' chunks.
+template <typename T>
+static bool mssq_pow2_fits(int logm) {
+  return logm >= 1 && logm <= 12 &&
+         dispatch_log2<1, 12>(logm, [](auto L) { return MssqTile<T, L>::SMEM <= kMaxBlockSmem ? 1 : 0; });
+}
+
+template <typename T, int EPI>
+static int launch_mssq_stft(const MssqStftArgs<T>& P, cudaStream_t st) {
+  const StftArgs<T>& A = P.A;
+  const long long total = (long long)A.B * A.n_hops;
+  const int logm = ilog2_exact(A.n_fft);
+  if (mssq_pow2_fits<T>(logm)) {
+    return dispatch_log2<1, 12>(logm, [&](auto L) {
+      using TL = MssqTile<T, L>;
+      if constexpr (TL::SMEM > kMaxBlockSmem) {
+        return set_error(SSQB_E_UNSUPP, "n_fft = 2^%d does not fit one CTA", (int)L);
+      } else {
+        auto kern = mssq_stft_pow2_kernel<T, L, EPI>;
+        SSQB_CUDA(opt_in_smem(kern, TL::SMEM));
+        kern<<<(unsigned)((total + TL::R - 1) / TL::R), Tile<T>::NT, TL::SMEM, st>>>(P);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      }
+    });
+  }
+  const long long M = A.n_fft;
+  const size_t smem = sizeof(short) * (size_t)(M / 2 + 1);
+  if (smem > kMaxBlockSmem) return set_error(SSQB_E_UNSUPP, "n_fft = %d: the bins of a frame do not fit one CTA", A.n_fft);
+  SSQB_CUDA(opt_in_smem(mssq_stft_emit_kernel<T, EPI>, smem));
+  return generic_frames<T>(A.n_fft, total, 1, -1,
+      [&](cx<T>* c, long long f0, long long nf) {
+        stft_frames_kernel<T, STFT_EPI_PLAIN><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(A, c, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      },
+      [&](const cx<T>* C, long long f0, long long nf) {
+        mssq_stft_emit_kernel<T, EPI><<<(unsigned)nf, 256, smem, st>>>(P, C, f0);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      }, st);
+}
+
+template <typename T>
+static int mssq_stft_t(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, int n_iter,
+                       const void* x, long long B, void* Sx, void* Tx, void* dSx, int* tgt,
+                       cudaStream_t st) {
+  const int M = d->n_fft, nrows = M / 2 + 1;
+  MssqStftArgs<T> P;
+  memset(&P, 0, sizeof(P));
+  StftArgs<T>& A = P.A;
+  A.N = d->N; A.n_fft = M; A.hop = d->hop; A.n1 = d->n1; A.padtype = d->padtype;
+  A.modulated = d->modulated; A.B = (int)B;
+  A.n_hops = (d->N - 1) / d->hop + 1;
+  A.x = (const T*)x; A.Sx = (cx<T>*)Sx; A.dSx = (cx<T>*)dSx; A.Tx = (cx<T>*)Tx;
+  A.write_dSx = dSx ? 1 : 0;
+  P.n_iter = n_iter; P.tgt = tgt;
+  const T* win = (const T*)d->win_host; const T* dwin = (const T*)d->dwin_host;
+  const double kap = pack_kappa(win, dwin, M);                 // the packing of ssq_stft
+  A.kappa = (T)kap; A.inv_kappa = (T)(1.0 / kap);
+  BlobBuilder bb;
+  const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
+  const size_t o_cst = bb.put(r->cst_host, sizeof(double) * nrows);
+  const size_t o_win = bb.put(win, sizeof(T) * M);
+  const size_t o_dwin = bb.put(dwin, sizeof(T) * M);
+  const size_t o_sfs = bb.put(d->Sfs_host, sizeof(T) * nrows);
+  unsigned char* blob = nullptr;
+  int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
+  A.tw = (const cx<T>*)(blob + o_tw); A.cst = (const double*)(blob + o_cst);
+  A.win = (const T*)(blob + o_win); A.dwin = (const T*)(blob + o_dwin);
+  A.Sfs = (const T*)(blob + o_sfs);
+  rc = fill_grid(r, nrows, &A.grid); if (rc) return rc;
+  A.grid.kind = 3;
+  P.flipud = A.grid.flipud; A.grid.flipud = 0;                 // the chain works on unflipped bins
+  SSQB_CUDA(cudaMemsetAsync(Tx, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(cx<T>), st));
+  switch ((Sx ? MSSQ_EPI_SX : 0) | (tgt ? MSSQ_EPI_TGT : 0)) {
+    case 0: return launch_mssq_stft<T, 0>(P, st);
+    case MSSQ_EPI_SX: return launch_mssq_stft<T, MSSQ_EPI_SX>(P, st);
+    case MSSQ_EPI_TGT: return launch_mssq_stft<T, MSSQ_EPI_TGT>(P, st);
+    default: return launch_mssq_stft<T, MSSQ_EPI_SX | MSSQ_EPI_TGT>(P, st);
+  }
+}
+
+int run_mssq_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, int n_iter,
+                  const void* x, long long B, void* Sx, void* Tx, void* dSx, int* tgt,
+                  cudaStream_t st) {
+  if (!d || !r || !x || !Tx) return set_error(SSQB_E_ARG, "null pointer");
+  if (!d->win_host || !d->dwin_host || !d->Sfs_host || !r->cst_host)
+    return set_error(SSQB_E_ARG, "null table");
+  if (n_iter < 1 || n_iter > SSQB_MSSQ_MAX_ITER) return set_error(SSQB_E_ARG, "n_iter must be in [1, 64]");
+  if (!(r->gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
+  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
+  if (d->n_fft / 2 + 1 > SSQB_MSSQ_MAX_ROWS) return set_error(SSQB_E_UNSUPP, "n_fft must be < 65534");
+  return d->dtype == SSQB_F32 ? mssq_stft_t<float>(d, r, n_iter, x, B, Sx, Tx, dSx, tgt, st)
+                              : mssq_stft_t<double>(d, r, n_iter, x, B, Sx, Tx, dSx, tgt, st);
 }
 
 }  // namespace ssqb
