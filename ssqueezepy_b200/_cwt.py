@@ -176,6 +176,18 @@ class CwtPlan:
                 cls._cache.move_to_end(key)
         return plan
 
+    def companion(self, key, build):
+        """`build()`, built once per `key` and kept in this plan's `derived` dict (the A-table
+        plan, the variants' group runners, host tables).  A companion never references its
+        plan -- whoever needs the plan is given it -- so a plan evicted from the plan cache is
+        freed at once, with everything it owns, without the cyclic garbage collector."""
+        with self._lock:
+            derived = self.__dict__.setdefault('derived', {})
+            c = derived.get(key)
+            if c is None:
+                c = derived[key] = build()
+            return c
+
     def set_reassign(self, desc, key):
         if key != self._reassign_key:
             _lib.check(self.lib.ssqb_cwt_plan_set_reassign(self.handle, C.byref(desc)))
@@ -241,6 +253,60 @@ class CwtPlan:
                                               xd.shape[0], xh.data_ptr(),
                                               Bk.stream_ptr()))
         return xh
+
+
+# bound of the scratch that holds one group's planes in a `GroupRunner` (at least one signal's)
+SCRATCH_BYTES = 1 << 30
+
+
+class GroupRunner:
+    """Runs a variant's batch through a base plan in groups of signals: the second-order
+    `ssq_cwt`, `tssq_cwt`, `reassigned_cwt` and `mssq_cwt`.  A subclass is a companion of the
+    plan (`CwtPlan.companion`; it holds no reference to it) and sets N_PLANES, the complex
+    [na, n_cols] planes its step reads or writes per signal.  `group`, the signals per group,
+    is as many as fit SCRATCH_BYTES with every plane at N columns (at least one); it may be
+    set."""
+    N_PLANES = None
+
+    def __init__(self, plan):
+        per_signal = self.N_PLANES * plan.na * plan.N * torch.empty(
+            (), dtype=Bk.cplx_dtype(plan.dtype)).element_size()
+        self.group = max(1, SCRATCH_BYTES // per_signal)
+        self._scratch = None
+        self._done = None                 # event after the last call that used the scratch
+
+    def run_groups(self, plan, xd, hop, planes, step):
+        """Runs `step(b0, b1, views)` for the groups b0:b1 of the [B, N] device signals `xd`, in
+        order, under the plan's lock.  `planes` has N_PLANES entries: a full-batch
+        [B, na, n_cols(hop)] tensor, or None for a plane that lives in the scratch; `views`
+        holds each plane's rows of the group.  The group is the whole batch when every plane is
+        given.  The scratch only grows, to what the call keeps in it; a call on another stream
+        first waits for the last one that used it."""
+        B, na, ncol = xd.shape[0], plan.na, plan.n_cols(hop)
+        held = [i for i, p in enumerate(planes) if p is None]
+        g = min(self.group, B) if held else B
+        with plan._lock:
+            if self._done is not None:
+                torch.cuda.current_stream().wait_event(self._done)
+            S = None
+            if held:
+                size = len(held) * g * na * ncol
+                if self._scratch is None or self._scratch.numel() < size:
+                    self._scratch = None
+                    self._scratch = torch.empty(size, dtype=Bk.cplx_dtype(plan.dtype),
+                                                device='cuda')
+                S = self._scratch[:size].view(len(held), g, na, ncol)
+            for b0 in range(0, B, g):
+                b1 = min(B, b0 + g)
+                step(b0, b1, [S[held.index(i), :b1 - b0] if p is None else p[b0:b1]
+                              for i, p in enumerate(planes)])
+            self._done = torch.cuda.Event()
+            self._done.record()
+
+
+def rows_ptr(v, b0, b1):
+    """Device pointer of the rows b0:b1 of the full-batch plane `v`, or None."""
+    return None if v is None else v[b0:b1].data_ptr()
 
 
 _SCALES_CACHE = {}
@@ -346,21 +412,27 @@ class _CwtFn(torch.autograd.Function):
     def backward(ctx, gW, gdW=None):
         if gW is None and gdW is None:
             return None, None, None, None, None, None
-        plan = ctx.plan
-        cdt = Bk.cplx_dtype(plan.dtype)
-        gW = None if gW is None else gW.to(cdt).contiguous()
-        gdW = None if gdW is None else gdW.to(cdt).contiguous()
         B = (gW if gW is not None else gdW).shape[0]
-        gx = torch.empty((B, plan.N), dtype=Bk.real_dtype(plan.dtype), device='cuda')
-        mul = None
-        if ctx.out_mul is not None:
-            mul_arr = np.ascontiguousarray(ctx.out_mul, dtype=np.float64)
-            mul = mul_arr.ctypes.data_as(C.POINTER(C.c_double))
-        with plan._lock:
-            _lib.check(plan.lib.ssqb_cwt_backward_hop(plan.handle, Bk.ptr(gW), Bk.ptr(gdW), B,
-                                                      mul, int(bool(ctx.rpadded)), ctx.hop,
-                                                      gx.data_ptr(), Bk.stream_ptr()))
-        return gx, None, None, None, None, None
+        return (cwt_adjoint(ctx.plan, gW, gdW, B, ctx.hop, ctx.out_mul, ctx.rpadded),
+                None, None, None, None, None)
+
+
+def cwt_adjoint(plan, gW, gdW, B, hop, out_mul=None, rpadded=False):
+    """`ssqb_cwt_backward_hop`: the gradient [B, N] of the signals from the gradients of
+    the [B, na, ncol] Wx and dWx of `plan` (either may be None; not both)."""
+    cdt = Bk.cplx_dtype(plan.dtype)
+    gW = None if gW is None else gW.to(cdt).contiguous()
+    gdW = None if gdW is None else gdW.to(cdt).contiguous()
+    gx = torch.empty((B, plan.N), dtype=Bk.real_dtype(plan.dtype), device='cuda')
+    mul = None
+    if out_mul is not None:
+        mul_arr = np.ascontiguousarray(out_mul, dtype=np.float64)
+        mul = mul_arr.ctypes.data_as(C.POINTER(C.c_double))
+    with plan._lock:
+        _lib.check(plan.lib.ssqb_cwt_backward_hop(plan.handle, Bk.ptr(gW), Bk.ptr(gdW), B, mul,
+                                                  int(bool(rpadded)), hop, gx.data_ptr(),
+                                                  Bk.stream_ptr()))
+    return gx
 
 
 def check_hop_len(hop_len, rpadded=False):

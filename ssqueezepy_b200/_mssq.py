@@ -25,19 +25,16 @@ import numpy as np
 import torch
 
 from . import _lib, backend as Bk
-from ._cwt import CwtPlan, _clean_input, _pad_geometry_for, cached_process_scales, check_hop_len
-from ._ssq_cwt import ssq_cwt_host_params
-from ._ssq_cwt2 import SCRATCH_BYTES
-from ._stft import _get_call
-from ._tssq import _check_gamma, _default_gamma, _finish
+from ._cwt import GroupRunner, _clean_input, check_hop_len, cwt_adjoint, rows_ptr
+from ._stft import stft_adjoint
+from . import _variants as F
+from ._variants import (FORM_CWT, FORM_STFT, check_gamma, check_x, finish_outputs,
+                        stft_setup)
 from .algos import make_reassign_desc
 from .ssqueezing import _get_center_frequency
-from .utils.cwt_utils import _process_fs_and_t
-from .wavelets import Wavelet
 
 __all__ = ['mssq_stft', 'mssq_cwt']
 
-FORM_STFT, FORM_CWT = 0, 1
 MAX_ITER = 64
 
 
@@ -48,9 +45,9 @@ def _check_n_iter(n_iter):
     return int(n_iter)
 
 
-def _check_x(x):
-    if not hasattr(x, 'ndim') or x.ndim not in (1, 2):
-        raise ValueError("`x` must be a 1D or 2D array or tensor")
+def _check_order0(wavelet):
+    if getattr(wavelet, 'config', None) and wavelet.config.get('order', 0):
+        raise ValueError("`mssq_cwt` takes order-0 wavelets (got %s)" % wavelet.name)
 
 
 def row_of_bin_cwt(scales, ssq_freqs, c):
@@ -126,11 +123,7 @@ class _MssqStftFn(torch.autograd.Function):
         if gT is not None:
             gS = _backward(call.dtype, FORM_STFT, Sx, dSx, call.Sfs_tensor(), ctx.desc, None,
                            ctx.n_iter, gT, gS)
-        gS = gS.to(Bk.cplx_dtype(call.dtype)).contiguous()
-        gx = torch.empty((Sx.shape[0], call.N), dtype=Bk.real_dtype(call.dtype), device='cuda')
-        _lib.check(Bk.require_cuda().ssqb_stft_backward(
-            C.byref(call.desc), gS.data_ptr(), None, Sx.shape[0], gx.data_ptr(), Bk.stream_ptr()))
-        return gx, None, None, None, None
+        return stft_adjoint(call, gS, None, Sx.shape[0]), None, None, None, None
 
 
 def mssq_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=None,
@@ -149,17 +142,9 @@ def mssq_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=No
     `Tx` and `Sx` are differentiable; the gradient holds the targets where the forward put
     them.  Other arguments as `ssq_stft`."""
     n_iter = _check_n_iter(n_iter)
-    hop_len = check_hop_len(hop_len)
-    gamma = _check_gamma(gamma)
-    _check_x(x)
-    N = x.shape[-1]
-    _, fs, _ = _process_fs_and_t(fs, t, N)
-    call = _get_call(N, window, n_fft, win_len, hop_len, fs, padtype, modulated, dtype)
-    gamma = _default_gamma(gamma, call.dtype)
-    Bk.require_cuda()
+    call, x2, gamma, fs = stft_setup(x, window, n_fft, win_len, hop_len, fs, t, padtype,
+                                     modulated, gamma, dtype)
     desc = call.reassign_desc(flipud, gamma, make_reassign_desc)
-    xd = Bk.to_device(x, call.dtype)
-    x2 = xd if xd.ndim == 2 else xd.unsqueeze(0)
     tgt = (torch.empty((x2.shape[0], call.n_rows, call.n_hops), dtype=torch.int32, device='cuda')
            if get_tgt else None)
     if torch.is_tensor(x) and x.requires_grad:
@@ -168,68 +153,50 @@ def mssq_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=No
         dSx = dSx if get_dWx else None
     else:
         Tx, Sx, dSx = stft_exec(call, x2, desc, n_iter, get_Sx=get_Sx, get_dSx=get_dWx, tgt=tgt)
-    if x.ndim == 1:
-        Tx, Sx, dSx, tgt = [None if v is None else v[0] for v in (Tx, Sx, dSx, tgt)]
     ssq_freqs = call.Sfs[::-1].copy() if flipud else call.Sfs.copy()
     Sfs = call.Sfs_tensor() if astensor else call.Sfs.copy()
-    Tx, Sx, dSx, tgt = _finish((Tx, Sx, dSx, tgt), astensor)
+    Tx, Sx, dSx, tgt = finish_outputs(x, (Tx, Sx, dSx, tgt), astensor)
     return (Tx, Sx, ssq_freqs, Sfs) + ((dSx,) if get_dWx else ()) + ((tgt,) if get_tgt else ())
 
 
 # ---- CWT -------------------------------------------------------------------------------------
-class _MssqCwt:
-    """The group scratch of one base plan, kept in the base plan's `derived` dict.  A batch runs
-    in groups of signals whose W and dW planes fit the scratch, so only `Tx` (and the planes
-    asked for) cover the whole batch."""
-
-    def __init__(self, plan):
-        self.dtype, self.na, self.N = plan.dtype, plan.na, plan.N
-        per_signal = 2 * self.na * self.N * torch.empty(
-            (), dtype=Bk.cplx_dtype(self.dtype)).element_size()
-        self.group = max(1, SCRATCH_BYTES // per_signal)
-        self.rob = {}                     # row_of_bin per ssq_freqs grid
-        self._scratch = None
-        self._done = None                 # event after the last call that used the scratch
-
-    def _get_scratch(self, g, ncol):
-        size = 2 * g * self.na * ncol
-        if self._scratch is None or self._scratch.numel() < size:
-            self._scratch = None
-            self._scratch = torch.empty(size, dtype=Bk.cplx_dtype(self.dtype), device='cuda')
-        return self._scratch[:size].view(2, g, self.na, ncol)
+class _MssqCwt(GroupRunner):
+    """The W, dW group runner of one base plan, kept in the base plan's `derived` dict."""
+    N_PLANES = 2
 
     def run(self, plan, xd, desc, rob, n_iter, Tx, Wx=None, dWx=None, tgt=None, hop=1):
-        """Tx [B, na, ncol] of the [B, N] device signals `xd`; `Wx`, `dWx` and `tgt`
-        (full-batch planes), when given, receive the planes."""
+        """Tx [B, na, ncol] of the [B, N] device signals `xd`; `Wx`, `dWx` (full-batch planes),
+        when given, receive W and dW instead of the scratch; `tgt` the final rows."""
         lib = Bk.require_cuda()
-        B = xd.shape[0]
-        full = Wx is not None and dWx is not None
-        g = B if full else min(self.group, B)
-        ncol = plan.n_cols(hop)
-        with plan._lock:
-            if self._done is not None:    # the scratch of a call on another stream
-                torch.cuda.current_stream().wait_event(self._done)
-            S = None if full else self._get_scratch(g, ncol)
-            for b0 in range(0, B, g):
-                b1 = min(B, b0 + g)
-                W_ = S[0, :b1 - b0] if Wx is None else Wx[b0:b1]
-                dW_ = S[1, :b1 - b0] if dWx is None else dWx[b0:b1]
-                plan.cwt_into(xd[b0:b1], W_, dW_, hop_len=hop)
-                _lib.check(lib.ssqb_mssq_cwt_reassign(
-                    Bk.dtype_code(self.dtype), W_.data_ptr(), dW_.data_ptr(), C.byref(desc),
-                    rob.ctypes.data, n_iter, b1 - b0, self.na, ncol, Tx[b0:b1].data_ptr(),
-                    None if tgt is None else tgt[b0:b1].data_ptr(), Bk.stream_ptr()))
-            self._done = torch.cuda.Event()
-            self._done.record()
+
+        def step(b0, b1, P):
+            W, dW = P
+            plan.cwt_into(xd[b0:b1], W, dW, hop_len=hop)
+            _lib.check(lib.ssqb_mssq_cwt_reassign(
+                Bk.dtype_code(plan.dtype), W.data_ptr(), dW.data_ptr(), C.byref(desc),
+                rob.ctypes.data, n_iter, b1 - b0, plan.na, W.shape[-1], Tx[b0:b1].data_ptr(),
+                rows_ptr(tgt, b0, b1), Bk.stream_ptr()))
+        self.run_groups(plan, xd, hop, [Wx, dWx], step)
 
 
 def mssq_of(plan):
     """The MSST companion of `plan`, built once and cached with it."""
-    with plan._lock:
-        derived = plan.__dict__.setdefault('derived', {})
-        if 'mssq' not in derived:
-            derived['mssq'] = _MssqCwt(plan)
-        return derived['mssq']
+    return plan.companion('mssq', lambda: _MssqCwt(plan))
+
+
+def cwt_setup(x, wavelet, scales, nv, fs, t, ssq_freqs, padtype, maprange, flipud, gamma):
+    """(wavelet, plan, desc, rob, ssq_freqs) of a `mssq_cwt` call: the plan, the reassignment
+    descriptor and the returned `ssq_freqs` of the fused first-order `ssq_cwt` with the same
+    arguments (`_variants.cwt_setup`), and the int32 row_of_bin of its grid, cached with the
+    plan per grid."""
+    c = F.cwt_setup(x, wavelet, scales, nv, fs, t, padtype, gamma, _check_order0,
+                    first_order=True, maprange=maprange, flipud=flipud, ssq_freqs=ssq_freqs)
+    f = c.hp['ssq_freqs']
+    f64 = np.asarray(Bk.finish(f, False) if Bk.is_tensor(f) else f, dtype=np.float64)
+    sc = c.hp['scales']
+    rob = c.plan.companion(('row_of_bin', f64.tobytes(), c.was_padded), lambda: row_of_bin_cwt(
+        sc, f64, peak_constant(c.wavelet, c.N, c.dt, sc[0], c.was_padded)))
+    return c.wavelet, c.plan, c.desc, rob, c.ssq_freqs
 
 
 class _MssqCwtFn(torch.autograd.Function):
@@ -258,62 +225,7 @@ class _MssqCwtFn(torch.autograd.Function):
         if gT is not None:
             gW = _backward(plan.dtype, FORM_CWT, W, dW, None, ctx.desc, ctx.rob, ctx.n_iter, gT,
                            gW)
-        gW = gW.to(Bk.cplx_dtype(plan.dtype)).contiguous()
-        gx = torch.empty((W.shape[0], plan.N), dtype=Bk.real_dtype(plan.dtype), device='cuda')
-        with plan._lock:
-            _lib.check(plan.lib.ssqb_cwt_backward_hop(plan.handle, gW.data_ptr(), None,
-                                                      W.shape[0], None, 0, ctx.hop,
-                                                      gx.data_ptr(), Bk.stream_ptr()))
-        return (gx,) + (None,) * 7
-
-
-def _freqs_arg(ssq_freqs, na):
-    """`ssq_freqs` of a `mssq_cwt` call: None, a grid name, or a float64 array of `na` values."""
-    if ssq_freqs is None or isinstance(ssq_freqs, str):
-        return ssq_freqs
-    f = np.asarray(Bk.finish(ssq_freqs, False) if Bk.is_tensor(ssq_freqs) else ssq_freqs,
-                   dtype=np.float64).reshape(-1)
-    if f.size != na:
-        raise ValueError("`ssq_freqs` must hold len(scales) = %d values (got %d)" % (na, f.size))
-    return f
-
-
-def cwt_setup(x, wavelet, scales, nv, fs, t, ssq_freqs, padtype, maprange, flipud, gamma):
-    """(wavelet, plan, desc, rob, ssq_freqs) of a `mssq_cwt` call: the plan, the reassignment
-    descriptor and the returned `ssq_freqs` of the fused first-order `ssq_cwt` with the same
-    arguments, and the int32 row_of_bin of its grid."""
-    if nv is None and not isinstance(scales, np.ndarray):
-        nv = 32
-    N = x.shape[-1]
-    dt, fs, _ = _process_fs_and_t(fs, t, N)
-    wavelet = Wavelet._init_if_not_isinstance(wavelet, N=N)
-    if getattr(wavelet, 'config', None) and wavelet.config.get('order', 0):
-        raise ValueError("`mssq_cwt` takes order-0 wavelets (got %s)" % wavelet.name)
-    gamma = _default_gamma(gamma, wavelet.dtype)
-    scales, cwt_scaletype, *_ = cached_process_scales(scales, N, wavelet, nv)
-    ssq_freqs = _freqs_arg(ssq_freqs, len(scales))
-    if ssq_freqs is None:
-        ssq_freqs = cwt_scaletype
-    was_padded = padtype is not None
-    n_up, n1, pad_kind = _pad_geometry_for(N, padtype)
-    hp = ssq_cwt_host_params(N, wavelet, scales, ssq_freqs, maprange, was_padded, dt)
-    plan = CwtPlan.get(wavelet, hp['scales'], N, n_up, n1, pad_kind, dt)
-    desc = make_reassign_desc(hp['ssq_freqs'], hp['const'], plan.na, hp['logscale'], flipud,
-                              gamma, wavelet.dtype)
-    f = hp['ssq_freqs']
-    f64 = np.asarray(Bk.finish(f, False) if Bk.is_tensor(f) else f, dtype=np.float64)
-    o = mssq_of(plan)
-    key = (f64.tobytes(), was_padded)
-    with plan._lock:
-        rob = o.rob.get(key)
-    if rob is None:
-        c = peak_constant(wavelet, N, dt, hp['scales'][0], was_padded)
-        rob = row_of_bin_cwt(hp['scales'], f64, c)
-        with plan._lock:
-            o.rob[key] = rob
-    # `scales` go high -> low, so the returned frequencies are reversed (as `ssq_cwt`)
-    ssq_freqs = f.flip(0) if Bk.is_tensor(f) else np.asarray(f)[::-1].copy()
-    return wavelet, plan, desc, rob, ssq_freqs
+        return (cwt_adjoint(plan, gW, None, W.shape[0], ctx.hop),) + (None,) * 7
 
 
 def mssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
@@ -337,8 +249,8 @@ def mssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
     differentiable (targets held).  Other arguments as `ssq_cwt`."""
     n_iter = _check_n_iter(n_iter)
     hop_len = check_hop_len(hop_len)
-    gamma = _check_gamma(gamma)
-    _check_x(x)
+    gamma = check_gamma(gamma)
+    check_x(x)
     wavelet, plan, desc, rob, ssq_freqs = cwt_setup(x, wavelet, scales, nv, fs, t, ssq_freqs,
                                                     padtype, maprange, flipud, gamma)
     x = _clean_input(x, nan_checks)
@@ -355,10 +267,7 @@ def mssq_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
     else:
         Tx, Wx, dWx = new(cdt), new(cdt, get_Wx), new(cdt, get_dWx)
         o.run(plan, xd, desc, rob, n_iter, Tx, Wx=Wx, dWx=dWx, tgt=tgt, hop=hop_len)
-    if x.ndim == 1:
-        Tx, Wx, dWx, tgt = [None if v is None else v[0] for v in (Tx, Wx, dWx, tgt)]
-    sc = plan.scales_tensor().clone()
-    Tx, Wx, dWx, tgt, sc = _finish((Tx, Wx, dWx, tgt, sc), astensor)
-    if not astensor and Bk.is_tensor(ssq_freqs):
-        ssq_freqs = ssq_freqs.cpu().numpy()
+    Tx, Wx, dWx, tgt = finish_outputs(x, (Tx, Wx, dWx, tgt), astensor)
+    sc = Bk.finish(plan.scales_tensor().clone(), astensor)
+    ssq_freqs = Bk.finish(ssq_freqs, astensor)
     return (Tx, Wx, ssq_freqs, sc) + ((dWx,) if get_dWx else ()) + ((tgt,) if get_tgt else ())

@@ -14,22 +14,20 @@ Points with |V| <= gamma, a non-finite delay or a target outside [0, n_cols) are
 kept set of `tssq_*`).  `Rx` is a real plane of the data dtype with the shape of `Tx`; its sum is
 the kept energy.  The STFT runs as one fused kernel (the `ssq_stft` packing of g and g', plus a
 transform of tau g per frame); the CWT takes W and dW from the call's plan and A from the
-`tssq_cwt` table plan, then one reassignment kernel.  DESIGN.md section 12 has the details.
+plan's A-table plan (`_ssq_cwt2.a_plan`), then one reassignment kernel.  DESIGN.md section 12
+has the details.
 """
 import ctypes as C
-import numpy as np
 import torch
 
 from . import _lib, backend as Bk
-from ._cwt import CwtPlan, _clean_input, _pad_geometry_for, cached_process_scales, check_hop_len
-from ._ssq_cwt import ssq_cwt_host_params
-from ._ssq_cwt2 import psih_pair, SCRATCH_BYTES
-from ._stft import _get_call
-from ._tssq import (_check_gamma, _default_gamma, _finish, _tau_out, tau_window, tssq_of,
-                    FORM_STFT, FORM_CWT)
+from ._cwt import GroupRunner, _clean_input, check_hop_len, cwt_adjoint, rows_ptr
+from ._ssq_cwt2 import a_plan
+from ._stft import stft_adjoint
+from . import _variants as F
+from ._variants import (FORM_CWT, FORM_STFT, check_gamma, check_x, finish_outputs, seconds,
+                        stft_setup)
 from .algos import make_reassign_desc
-from .utils.cwt_utils import _process_fs_and_t
-from .wavelets import Wavelet
 
 __all__ = ['reassigned_stft', 'reassigned_cwt']
 
@@ -48,7 +46,7 @@ def _backward(dtype, form, V, P1, P2, Sfs, desc, gR, gV, nrows, ncols, hop, gamm
 
 def _tf_out(o, fs):
     """(w, tau) in Hz and seconds from the kernel's planes (w is already in Hz)."""
-    return o['w'], _tau_out(o['tau'], fs)
+    return o['w'], seconds(o['tau'], fs)
 
 
 # ---- STFT ------------------------------------------------------------------------------------
@@ -66,8 +64,8 @@ def stft_exec(call, x2, desc, gamma, get_Sx=True, get_dSx=False, get_Vt=False, g
                kk=new(tgt, torch.int32), jt=new(tgt, torch.int32), w=new(get_tf, rdt),
                tau=new(get_tf, rdt))
     _lib.check(Bk.require_cuda().ssqb_rs_stft_exec(
-        C.byref(call.desc), tau_window(call).ctypes.data, C.byref(desc), gamma, x2.data_ptr(), B,
-        Bk.ptr(out['Sx']), out['Rx'].data_ptr(), Bk.ptr(out['dSx']), Bk.ptr(out['Vt']),
+        C.byref(call.desc), call.tau_window().ctypes.data, C.byref(desc), gamma, x2.data_ptr(),
+        B, Bk.ptr(out['Sx']), out['Rx'].data_ptr(), Bk.ptr(out['dSx']), Bk.ptr(out['Vt']),
         Bk.ptr(out['kk']), Bk.ptr(out['jt']), Bk.ptr(out['w']), Bk.ptr(out['tau']),
         Bk.stream_ptr()))
     return out
@@ -96,11 +94,7 @@ class _RsStftFn(torch.autograd.Function):
         if gR is not None:
             gS = _backward(call.dtype, FORM_STFT, Sx, dSx, Vt, call.Sfs_tensor(), ctx.desc, gR,
                            gS, call.n_rows, call.n_hops, call.hop, ctx.gamma)
-        gS = gS.to(Bk.cplx_dtype(call.dtype)).contiguous()
-        gx = torch.empty((Sx.shape[0], call.N), dtype=Bk.real_dtype(call.dtype), device='cuda')
-        _lib.check(Bk.require_cuda().ssqb_stft_backward(
-            C.byref(call.desc), gS.data_ptr(), None, Sx.shape[0], gx.data_ptr(), Bk.stream_ptr()))
-        return gx, None, None, None
+        return stft_adjoint(call, gS, None, Sx.shape[0]), None, None, None
 
 
 def reassigned_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=None,
@@ -119,18 +113,9 @@ def reassigned_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None
     seconds, both inf where a point is dropped.  With `x.requires_grad`, `Rx` and `Sx` are
     differentiable; the gradient holds the targets where the forward put them.  Other
     arguments as `ssq_stft`."""
-    hop_len = check_hop_len(hop_len)
-    gamma = _check_gamma(gamma)
-    if not hasattr(x, 'ndim') or x.ndim not in (1, 2):
-        raise ValueError("`x` must be a 1D or 2D array or tensor")
-    N = x.shape[-1]
-    _, fs, _ = _process_fs_and_t(fs, t, N)
-    call = _get_call(N, window, n_fft, win_len, hop_len, fs, padtype, modulated, dtype)
-    gamma = _default_gamma(gamma, call.dtype)
-    Bk.require_cuda()
+    call, x2, gamma, fs = stft_setup(x, window, n_fft, win_len, hop_len, fs, t, padtype,
+                                     modulated, gamma, dtype)
     desc = call.reassign_desc(flipud, gamma, make_reassign_desc)
-    xd = Bk.to_device(x, call.dtype)
-    x2 = xd if xd.ndim == 2 else xd.unsqueeze(0)
     w = tau = None
     if torch.is_tensor(x) and x.requires_grad:
         Rx, Sx = _RsStftFn.apply(x2, call, desc, gamma)
@@ -143,76 +128,45 @@ def reassigned_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None
         Rx, Sx = o['Rx'], o['Sx']
         if get_tf:
             w, tau = _tf_out(o, fs)
-    if x.ndim == 1:
-        Rx, Sx, w, tau = [None if v is None else v[0] for v in (Rx, Sx, w, tau)]
     ssq_freqs = call.Sfs[::-1].copy() if flipud else call.Sfs.copy()
     Sfs = call.Sfs_tensor() if astensor else call.Sfs.copy()
-    Rx, Sx, w, tau = _finish((Rx, Sx, w, tau), astensor)
+    Rx, Sx, w, tau = finish_outputs(x, (Rx, Sx, w, tau), astensor)
     return (Rx, Sx, ssq_freqs, Sfs, w, tau) if get_tf else (Rx, Sx, ssq_freqs, Sfs)
 
 
 # ---- CWT -------------------------------------------------------------------------------------
-class _RsCwt:
-    """The A-plane table plan (shared with `tssq_cwt`) and the group scratch of one base plan,
-    kept in the base plan's `derived` dict.  A batch runs in groups of signals whose W, dW and A
-    planes fit the scratch, so only `Rx` (and `Wx` when asked for) cover the whole batch."""
+class _RsCwt(GroupRunner):
+    """The W, dW, A group runner of one base plan (`pA` its shared A-table plan), kept in the
+    base plan's `derived` dict."""
+    N_PLANES = 3
 
     def __init__(self, plan, wavelet):
-        self.dtype, self.na, self.N = plan.dtype, plan.na, plan.N
-        self.pA = tssq_of(plan, wavelet).pA
-        per_signal = 3 * self.na * self.N * torch.empty(
-            (), dtype=Bk.cplx_dtype(self.dtype)).element_size()
-        self.group = max(1, SCRATCH_BYTES // per_signal)
-        self._scratch = None
-        self._done = None                 # event after the last call that used the scratch
-
-    def _get_scratch(self, g, ncol):
-        size = 3 * g * self.na * ncol
-        if self._scratch is None or self._scratch.numel() < size:
-            self._scratch = None
-            self._scratch = torch.empty(size, dtype=Bk.cplx_dtype(self.dtype), device='cuda')
-        return self._scratch[:size].view(3, g, self.na, ncol)
+        super().__init__(plan)
+        self.pA = a_plan(plan, wavelet)
 
     def run(self, plan, xd, desc, gamma, Rx, Wx=None, dWx=None, A=None, tp=None, hop=1):
         """Rx [B, na, ncol] of the [B, N] device signals `xd`; `Wx`, `dWx`, `A` (full-batch
-        planes), when given, receive the planes instead of the scratch; `tp` the dict of
-        target planes 'kk', 'jt', 'w', 'tau' (each may be None)."""
+        planes), when given, receive the planes instead of the scratch; `tp` the dict of target
+        planes 'kk', 'jt', 'w', 'tau' (each may be None)."""
         lib = Bk.require_cuda()
-        B = xd.shape[0]
-        full = Wx is not None and dWx is not None and A is not None
-        g = B if full else min(self.group, B)
-        ncol = plan.n_cols(hop)
         tp = tp or {}
-        sub = lambda v, b0, b1: None if v is None else v[b0:b1].data_ptr()
-        with plan._lock:
-            if self._done is not None:    # the scratch of a call on another stream
-                torch.cuda.current_stream().wait_event(self._done)
-            S = None if full else self._get_scratch(g, ncol)
-            for b0 in range(0, B, g):
-                b1 = min(B, b0 + g)
-                n = b1 - b0
-                W_ = S[0, :n] if Wx is None else Wx[b0:b1]
-                dW_ = S[1, :n] if dWx is None else dWx[b0:b1]
-                A_ = S[2, :n] if A is None else A[b0:b1]
-                xg = xd[b0:b1]
-                plan.cwt_into(xg, W_, dW_, hop_len=hop)
-                self.pA.cwt_into(xg, A_, hop_len=hop)
-                _lib.check(lib.ssqb_rs_cwt_reassign(
-                    Bk.dtype_code(self.dtype), W_.data_ptr(), dW_.data_ptr(), A_.data_ptr(),
-                    C.byref(desc), n, self.na, ncol, hop, gamma, Rx[b0:b1].data_ptr(),
-                    sub(tp.get('kk'), b0, b1), sub(tp.get('jt'), b0, b1),
-                    sub(tp.get('w'), b0, b1), sub(tp.get('tau'), b0, b1), Bk.stream_ptr()))
-            self._done = torch.cuda.Event()
-            self._done.record()
+
+        def step(b0, b1, P):
+            W, dW, A_ = P
+            xg = xd[b0:b1]
+            plan.cwt_into(xg, W, dW, hop_len=hop)
+            self.pA.cwt_into(xg, A_, hop_len=hop)
+            _lib.check(lib.ssqb_rs_cwt_reassign(
+                Bk.dtype_code(plan.dtype), W.data_ptr(), dW.data_ptr(), A_.data_ptr(),
+                C.byref(desc), b1 - b0, plan.na, W.shape[-1], hop, gamma, Rx[b0:b1].data_ptr(),
+                *[rows_ptr(tp.get(k), b0, b1) for k in ('kk', 'jt', 'w', 'tau')],
+                Bk.stream_ptr()))
+        self.run_groups(plan, xd, hop, [Wx, dWx, A], step)
 
 
 def rs_of(plan, wavelet):
     """The reassignment companion of `plan`, built once and cached with it."""
-    with plan._lock:
-        derived = plan.__dict__.setdefault('derived', {})
-        if 'rs' not in derived:
-            derived['rs'] = _RsCwt(plan, wavelet)
-        return derived['rs']
+    return plan.companion('rs', lambda: _RsCwt(plan, wavelet))
 
 
 class _RsCwtFn(torch.autograd.Function):
@@ -241,40 +195,16 @@ class _RsCwtFn(torch.autograd.Function):
         if gR is not None:
             gW = _backward(plan.dtype, FORM_CWT, W, dW, A, None, ctx.desc, gR, gW, plan.na,
                            W.shape[-1], ctx.hop, ctx.gamma)
-        gW = gW.to(Bk.cplx_dtype(plan.dtype)).contiguous()
-        gx = torch.empty((W.shape[0], plan.N), dtype=Bk.real_dtype(plan.dtype), device='cuda')
-        with plan._lock:
-            _lib.check(plan.lib.ssqb_cwt_backward_hop(plan.handle, gW.data_ptr(), None,
-                                                      W.shape[0], None, 0, ctx.hop,
-                                                      gx.data_ptr(), Bk.stream_ptr()))
-        return gx, None, None, None, None, None
+        return cwt_adjoint(plan, gW, None, W.shape[0], ctx.hop), None, None, None, None, None
 
 
 def cwt_setup(x, wavelet, scales, nv, fs, t, padtype, maprange, flipud, gamma):
     """(fs, wavelet, plan, desc, ssq_freqs, gamma) of a `reassigned_cwt` call: the plan, the
-    reassignment descriptor and the returned `ssq_freqs` of the fused first-order `ssq_cwt` with
-    the same arguments.  Raises before any device work for an unsupported wavelet."""
-    if nv is None and not isinstance(scales, np.ndarray):
-        nv = 32
-    N = x.shape[-1]
-    dt, fs, _ = _process_fs_and_t(fs, t, N)
-    wavelet = Wavelet._init_if_not_isinstance(wavelet, N=N)
-    try:
-        psih_pair(wavelet)
-    except NotImplementedError:
-        raise NotImplementedError("`reassigned_cwt` supports the Morlet and the order-0 GMW "
-                                  "(L1 or L2) wavelets (got %s)" % wavelet.name)
-    gamma = _default_gamma(gamma, wavelet.dtype)
-    scales, cwt_scaletype, *_ = cached_process_scales(scales, N, wavelet, nv)
-    n_up, n1, pad_kind = _pad_geometry_for(N, padtype)
-    hp = ssq_cwt_host_params(N, wavelet, scales, cwt_scaletype, maprange, padtype is not None, dt)
-    plan = CwtPlan.get(wavelet, hp['scales'], N, n_up, n1, pad_kind, dt)
-    desc = make_reassign_desc(hp['ssq_freqs'], hp['const'], plan.na, hp['logscale'], flipud,
-                              gamma, wavelet.dtype)
-    f = hp['ssq_freqs']
-    # `scales` go high -> low, so the returned frequencies are reversed (as `ssq_cwt`)
-    ssq_freqs = f.flip(0) if Bk.is_tensor(f) else np.asarray(f)[::-1].copy()
-    return fs, wavelet, plan, desc, ssq_freqs, gamma
+    reassignment descriptor and the returned `ssq_freqs` of the fused first-order `ssq_cwt`
+    with the same arguments (`_variants.cwt_setup`)."""
+    c = F.cwt_setup(x, wavelet, scales, nv, fs, t, padtype, gamma, F.needs_psih('reassigned_cwt'),
+                    first_order=True, maprange=maprange, flipud=flipud)
+    return c.fs, c.wavelet, c.plan, c.desc, c.ssq_freqs, c.gamma
 
 
 def reassigned_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t=None,
@@ -294,9 +224,8 @@ def reassigned_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t
     groups of signals, so only `Rx` and `Wx` cover the whole batch.  With `x.requires_grad`,
     `Rx` and `Wx` are differentiable (targets held)."""
     hop_len = check_hop_len(hop_len)
-    gamma = _check_gamma(gamma)
-    if not hasattr(x, 'ndim') or x.ndim not in (1, 2):
-        raise ValueError("`x` must be a 1D or 2D array or tensor")
+    gamma = check_gamma(gamma)
+    check_x(x)
     fs, wavelet, plan, desc, ssq_freqs, gamma = cwt_setup(x, wavelet, scales, nv, fs, t, padtype,
                                                           maprange, flipud, gamma)
     x = _clean_input(x, nan_checks)
@@ -317,10 +246,7 @@ def reassigned_cwt(x, wavelet='gmw', scales='log-piecewise', nv=None, fs=None, t
         Rx, Wx = new(rdt), new(cdt, get_Wx)
         o.run(plan, xd, desc, gamma, Rx, Wx=Wx, tp=tp, hop=hop_len)
     w, tau = _tf_out(tp, fs) if get_tf else (None, None)
-    if x.ndim == 1:
-        Rx, Wx, w, tau = [None if v is None else v[0] for v in (Rx, Wx, w, tau)]
-    sc = plan.scales_tensor().clone()
-    Rx, Wx, w, tau, sc = _finish((Rx, Wx, w, tau, sc), astensor)
-    if not astensor and Bk.is_tensor(ssq_freqs):
-        ssq_freqs = ssq_freqs.cpu().numpy()
+    Rx, Wx, w, tau = finish_outputs(x, (Rx, Wx, w, tau), astensor)
+    sc = Bk.finish(plan.scales_tensor().clone(), astensor)
+    ssq_freqs = Bk.finish(ssq_freqs, astensor)
     return (Rx, Wx, ssq_freqs, sc, w, tau) if get_tf else (Rx, Wx, ssq_freqs, sc)

@@ -10,8 +10,8 @@ for (`get_dWx`, `get_w`).
 import numpy as np
 import torch
 
-from . import _lib, backend as Bk
-from ._cwt import (cwt, CwtPlan, _CwtFn, _clean_input, _pad_geometry_for,
+from . import backend as Bk
+from ._cwt import (cwt, cwt_adjoint, CwtPlan, _CwtFn, _clean_input, _pad_geometry_for,
                    cached_process_scales, wavelet_key, check_hop_len, _CACHE_LOCK)
 from ._ssq_cwt2 import psih_pair, order2_of
 from .algos import (phase_cwt_gpu, make_reassign_desc, colsum_real, invert_components,
@@ -240,18 +240,7 @@ class _SsqCwtFn(torch.autograd.Function):
         Wx, dWx = ctx.saved_tensors
         if gT is not None:
             gW = reassign_backward(ctx.desc, gT, plan.dtype, Wx=Wx, dWx=dWx, gWx=gW)
-        cdt = Bk.cplx_dtype(plan.dtype)
-        gW = None if gW is None else gW.to(cdt).contiguous()
-        gdW = None if gdW is None else gdW.to(cdt).contiguous()
-        if gW is None and gdW is None:
-            return None, None, None, None, None
-        B = Wx.shape[0]
-        gx = torch.empty((B, plan.N), dtype=Bk.real_dtype(plan.dtype), device='cuda')
-        with plan._lock:
-            _lib.check(plan.lib.ssqb_cwt_backward_hop(plan.handle, Bk.ptr(gW), Bk.ptr(gdW), B,
-                                                      None, 0, ctx.hop, gx.data_ptr(),
-                                                      Bk.stream_ptr()))
-        return gx, None, None, None, None
+        return cwt_adjoint(plan, gW, gdW, Wx.shape[0], ctx.hop), None, None, None, None
 
 
 _HP_CACHE = {}

@@ -6,21 +6,20 @@ chirp.  The second order corrects it by the local frequency modulation (DESIGN.m
 which needs three more transforms of every row:
     A  = ifft(a psih'(a xi) xh),   dA = ifft(i Om a psih'(a xi) xh),   D2 = ifft(-Om^2 psih_a xh)
 with Om = xi / dt.  They come from two more `CwtPlan`s of the same geometry, on host tables
-evaluated in float64 (`order2_tables`); `ssqb_ssq_cwt2_reassign` then reads the five planes and
-either reassigns into Tx or writes the second-order w.  A batch runs in groups of signals whose
-five planes fit a scratch of bounded size owned by the plan.
+evaluated in float64: the A plan (`a_table`, shared with `tssq_cwt` and `reassigned_cwt`) and the
+D2 plan (`d2_table`); `ssqb_ssq_cwt2_reassign` then reads the five planes and either
+reassigns into Tx or writes the second-order w.  A batch runs in groups of signals
+(`_cwt.GroupRunner`).
 """
 import ctypes as C
 import numpy as np
-import torch
 
 from . import _lib, backend as Bk
+from ._cwt import CwtPlan, GroupRunner, rows_ptr
 from .wavelets import Wavelet, xi_grid
 
-__all__ = ['psih_pair', 'order2_tables', 'order2_of']
+__all__ = ['psih_pair', 'a_table', 'd2_table', 'order2_tables', 'a_plan', 'order2_of']
 
-# bound of the scratch that holds one group's transforms (at least one signal's)
-SCRATCH_BYTES = 1 << 30
 _ROWS_PER_CHUNK = 16                  # host table rows evaluated at a time
 
 
@@ -64,96 +63,87 @@ def psih_pair(wavelet):
     return psih, dpsih
 
 
+def a_table(wavelet, scales, n, dtype=None):
+    """`a psih'(a xi)`, [na, n]: the table of the A plane (the CWT with psih' in place of psih),
+    evaluated in float64 and cast to `dtype` (default the wavelet's).  `scales` are taken in the
+    wavelet dtype, as the transform takes them; the Nyquist bin of an even `n` is halved, as in
+    the psih table (reference wavelets.py:86-95)."""
+    return _table(wavelet, scales, n, dtype, lambda a, w, psih, dpsih: a * dpsih(w))
+
+
+def d2_table(wavelet, scales, n, dt, dtype=None):
+    """`-psih(a xi) (xi / dt)^2`, [na, n]: the table of the D2 plane, as `a_table`."""
+    om2 = (xi_grid(n) / dt) ** 2
+    return _table(wavelet, scales, n, dtype, lambda a, w, psih, dpsih: -psih(w) * om2)
+
+
 def order2_tables(wavelet, scales, n, dt, dtype=None):
-    """`(a psih'(a xi), -psih(a xi) (xi / dt)^2)`, [na, n] each: the tables of the two extra
-    plans, evaluated in float64 and cast to `dtype` (default the wavelet's).  `scales` are
-    taken in the wavelet dtype, as the transform takes them; the Nyquist bin of an even `n` is
-    halved, as in the psih table (reference wavelets.py:86-95)."""
+    """`(a_table, d2_table)`: the tables of the second order's two extra plans."""
+    return a_table(wavelet, scales, n, dtype), d2_table(wavelet, scales, n, dt, dtype)
+
+
+def _table(wavelet, scales, n, dtype, row):
     psih, dpsih = psih_pair(wavelet)
     dtype = wavelet.dtype if dtype is None else dtype
     a = np.asarray(scales, dtype=wavelet.dtype).astype(np.float64).reshape(-1, 1)
     xi = xi_grid(n)
-    om2 = (xi / dt) ** 2
-    ta = np.empty((len(a), n), dtype=dtype)
-    tb = np.empty((len(a), n), dtype=dtype)
+    t = np.empty((len(a), n), dtype=dtype)
     for r0 in range(0, len(a), _ROWS_PER_CHUNK):
         ar = a[r0:r0 + _ROWS_PER_CHUNK]
-        w = ar * xi
-        va, vb = ar * dpsih(w), -psih(w) * om2
+        v = row(ar, ar * xi, psih, dpsih)
         if n % 2 == 0:
-            va[:, n // 2] /= 2
-            vb[:, n // 2] /= 2
-        ta[r0:r0 + len(ar)] = va
-        tb[r0:r0 + len(ar)] = vb
-    return ta, tb
+            v[:, n // 2] /= 2
+        t[r0:r0 + len(ar)] = v
+    return t
 
 
-class _Order2:
-    """The two table plans and the scratch of one base plan (see the module docstring).  It is
-    kept in the base plan's `derived` dict and holds no reference back to it (the base plan is
-    passed to `run`), so a plan evicted from the plan cache is freed with everything it owns."""
+def _table_plan(plan, wavelet, table):
+    """A plan of `plan`'s geometry on the host `table`."""
+    sc = plan.scales_np.reshape(-1)
+    return CwtPlan(wavelet, sc, plan.N, plan.n_up, plan.n1, plan.padtype, plan.dt,
+                   table=Bk.to_device(table(wavelet, sc, plan.n_up), plan.dtype))
+
+
+def a_plan(plan, wavelet):
+    """The `a_table` plan of `plan`: one per base plan, shared by the second-order, the
+    time-reassigned and the reassigned CWT."""
+    return plan.companion('a_table', lambda: _table_plan(plan, wavelet, a_table))
+
+
+class _Order2(GroupRunner):
+    """The D2 table plan of one base plan and its five-plane group runner (`pA` is the shared
+    A-table plan), kept in the base plan's `derived` dict under ('ssq_order', 2)."""
+    N_PLANES = 5
 
     def __init__(self, plan, wavelet, dt):
-        from ._cwt import CwtPlan
+        super().__init__(plan)
         self.dt = float(dt)
-        self.dtype, self.na, self.N = plan.dtype, plan.na, plan.N
-        ta, tb = order2_tables(wavelet, plan.scales_np.reshape(-1), plan.n_up, dt)
-        geo = (plan.scales_np.reshape(-1), plan.N, plan.n_up, plan.n1, plan.padtype, dt)
-        self.pA = CwtPlan(wavelet, *geo, table=Bk.to_device(ta, self.dtype))
-        self.pB = CwtPlan(wavelet, *geo, table=Bk.to_device(tb, self.dtype))
-        per_signal = 5 * self.na * self.N * torch.empty((), dtype=Bk.cplx_dtype(self.dtype)).element_size()
-        self.group = max(1, SCRATCH_BYTES // per_signal)
-        self._scratch = None
-        self._done = None                 # event after the last call that used the scratch
-
-    def _get_scratch(self, g, ncol):
-        """[5, g, na, ncol] view of the scratch (ncol <= N)."""
-        size = 5 * g * self.na * ncol
-        if self._scratch is None or self._scratch.numel() < size:
-            self._scratch = None
-            self._scratch = torch.empty(5 * g * self.na * self.N, dtype=Bk.cplx_dtype(self.dtype),
-                                        device='cuda')
-        return self._scratch[:size].view(5, g, self.na, ncol)
+        self.pA = a_plan(plan, wavelet)
+        self.pB = _table_plan(plan, wavelet, lambda wav, sc, n: d2_table(wav, sc, n, self.dt))
 
     def run(self, plan, xd, desc, Tx=None, w=None, Wx=None, dWx=None, W_given=False, hop=1):
         """`plan`: the base plan this companion belongs to; `xd` [B, N] device signals of its
         dtype.  Exactly one of `Tx` (complex) and `w` (real), [B, na, Nh], receives the result;
-        `Wx` / `dWx` [B, na, Nh], when given, receive W / dW (otherwise they stay in the scratch).
-        `W_given`: `Wx` and `dWx` already hold this plan's transform of `xd`, which is then not
-        computed again.  Every plane holds the columns j * hop, Nh = (N - 1) // hop + 1."""
+        `Wx` / `dWx` [B, na, Nh], when given, receive W / dW (otherwise they stay in the
+        scratch).  `W_given`: `Wx` and `dWx` already hold this plan's transform of `xd`, which
+        is then not computed again.  Every plane holds the columns j * hop,
+        Nh = (N - 1) // hop + 1."""
         lib = Bk.require_cuda()
-        B = xd.shape[0]
-        g = min(self.group, B)
-        ncol = plan.n_cols(hop)
-        with plan._lock:
-            if self._done is not None:    # the scratch of a call on another stream
-                torch.cuda.current_stream().wait_event(self._done)
-            S = self._get_scratch(g, ncol)
-            for b0 in range(0, B, g):
-                b1 = min(B, b0 + g)
-                n = b1 - b0
-                W = S[0, :n] if Wx is None else Wx[b0:b1]
-                dW = S[1, :n] if dWx is None else dWx[b0:b1]
-                A, dA, D2 = S[2, :n], S[3, :n], S[4, :n]
-                xg = xd[b0:b1]
-                if not W_given:
-                    plan.cwt_into(xg, W, dW, hop_len=hop)
-                self.pA.cwt_into(xg, A, dA, hop_len=hop)
-                self.pB.cwt_into(xg, D2, hop_len=hop)
-                _lib.check(lib.ssqb_ssq_cwt2_reassign(
-                    Bk.dtype_code(self.dtype), W.data_ptr(), dW.data_ptr(), A.data_ptr(),
-                    dA.data_ptr(), D2.data_ptr(), self.dt, n, self.na, ncol, C.byref(desc),
-                    None if Tx is None else Tx[b0:b1].data_ptr(),
-                    None if w is None else w[b0:b1].data_ptr(), Bk.stream_ptr()))
-            self._done = torch.cuda.Event()
-            self._done.record()
+
+        def step(b0, b1, P):
+            W, dW, A, dA, D2 = P
+            xg = xd[b0:b1]
+            if not W_given:
+                plan.cwt_into(xg, W, dW, hop_len=hop)
+            self.pA.cwt_into(xg, A, dA, hop_len=hop)
+            self.pB.cwt_into(xg, D2, hop_len=hop)
+            _lib.check(lib.ssqb_ssq_cwt2_reassign(
+                Bk.dtype_code(plan.dtype), W.data_ptr(), dW.data_ptr(), A.data_ptr(),
+                dA.data_ptr(), D2.data_ptr(), self.dt, b1 - b0, plan.na, W.shape[-1],
+                C.byref(desc), rows_ptr(Tx, b0, b1), rows_ptr(w, b0, b1), Bk.stream_ptr()))
+        self.run_groups(plan, xd, hop, [Wx, dWx, None, None, None], step)
 
 
 def order2_of(plan, wavelet, dt, ssq_order=2):
     """The order-2 companion of `plan`, built once and cached with it."""
-    with plan._lock:
-        derived = plan.__dict__.setdefault('derived', {})
-        key = ('ssq_order', int(ssq_order))
-        if key not in derived:
-            derived[key] = _Order2(plan, wavelet, dt)
-        return derived[key]
+    return plan.companion(('ssq_order', int(ssq_order)), lambda: _Order2(plan, wavelet, dt))

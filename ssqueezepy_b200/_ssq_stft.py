@@ -8,7 +8,7 @@ import numpy as np
 import torch
 
 from . import _lib, backend as Bk
-from ._stft import stft, _StftCall, _get_call, get_window, _check_NOLA
+from ._stft import stft, stft_adjoint, _StftCall, _get_call, get_window, _check_NOLA
 from .algos import phase_stft_gpu, make_reassign_desc, reassign_backward
 from .ssqueezing import ssqueeze, _check_ssqueezing_args
 from .utils.common import EPS32, EPS64, WARN
@@ -44,16 +44,7 @@ class _SsqStftFn(torch.autograd.Function):
         if gT is not None:
             gS = reassign_backward(ctx.desc, gT, call.dtype, Wx=Sx, dWx=dSx, gWx=gS,
                                    Sfs=call.Sfs_tensor())
-        cdt = Bk.cplx_dtype(call.dtype)
-        gS = None if gS is None else gS.to(cdt).contiguous()
-        gdS = None if gdS is None else gdS.to(cdt).contiguous()
-        if gS is None and gdS is None:
-            return None, None, None
-        B = Sx.shape[0]
-        gx = torch.empty((B, call.N), dtype=Bk.real_dtype(call.dtype), device='cuda')
-        _lib.check(Bk.require_cuda().ssqb_stft_backward(
-            C.byref(call.desc), Bk.ptr(gS), Bk.ptr(gdS), B, gx.data_ptr(), Bk.stream_ptr()))
-        return gx, None, None
+        return stft_adjoint(call, gS, gdS, Sx.shape[0]), None, None
 
 
 def ssq_stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=None,

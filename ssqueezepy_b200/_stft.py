@@ -138,7 +138,7 @@ class _StftCall:
         self._Sfs_dev = None
         self._rdesc = {}
         self._window_spec, self._win_len, self.fs = window, win_len, fs
-        self._tables2 = None
+        self._tables2 = self._twin = None
 
     def order2_tables(self):
         """`ssqb_stft2_tables` of second-order synchrosqueezing, built on first use: g'' (the
@@ -162,6 +162,19 @@ class _StftCall:
             t._keep = arrs          # the host arrays live as long as the struct
             self._tables2 = t
         return self._tables2
+
+    def tau_window(self):
+        """`tau g` of time reassignment, built on first use: (l - n_fft//2) g[l] on the
+        unshifted float64 window, cast to the data dtype and laid out like `_win` (ifftshifted
+        when modulated)."""
+        if self._twin is None:
+            g = np.asarray(get_window(self._window_spec, self._win_len, self.n_fft,
+                                      dtype='float64'), dtype=np.float64)
+            tg = (np.arange(len(g)) - len(g) // 2) * g
+            if self.desc.modulated:
+                tg = np.fft.ifftshift(tg)
+            self._twin = np.ascontiguousarray(tg, dtype=self.dtype)
+        return self._twin
 
     def Sfs_tensor(self):
         """`Sfs` on the device (uploaded once per call object; callers get a copy)."""
@@ -231,15 +244,20 @@ class _StftFn(torch.autograd.Function):
     def backward(ctx, gS, gdS=None):
         if gS is None and gdS is None:
             return None, None, None
-        call = ctx.call
-        cdt = Bk.cplx_dtype(call.dtype)
-        gS = None if gS is None else gS.to(cdt).contiguous()
-        gdS = None if gdS is None else gdS.to(cdt).contiguous()
         B = (gS if gS is not None else gdS).shape[0]
-        gx = torch.empty((B, call.N), dtype=Bk.real_dtype(call.dtype), device='cuda')
-        _lib.check(Bk.require_cuda().ssqb_stft_backward(
-            C.byref(call.desc), Bk.ptr(gS), Bk.ptr(gdS), B, gx.data_ptr(), Bk.stream_ptr()))
-        return gx, None, None
+        return stft_adjoint(ctx.call, gS, gdS, B), None, None
+
+
+def stft_adjoint(call, gS, gdS, B):
+    """`ssqb_stft_backward`: the gradient [B, N] of the signals from the gradients of the
+    [B, rows, n_hops] Sx and dSx of `call` (either may be None; not both)."""
+    cdt = Bk.cplx_dtype(call.dtype)
+    gS = None if gS is None else gS.to(cdt).contiguous()
+    gdS = None if gdS is None else gdS.to(cdt).contiguous()
+    gx = torch.empty((B, call.N), dtype=Bk.real_dtype(call.dtype), device='cuda')
+    _lib.check(Bk.require_cuda().ssqb_stft_backward(
+        C.byref(call.desc), Bk.ptr(gS), Bk.ptr(gdS), B, gx.data_ptr(), Bk.stream_ptr()))
+    return gx
 
 
 def stft(x, window=None, n_fft=None, win_len=None, hop_len=1, fs=None, t=None,

@@ -180,6 +180,14 @@ CwtPlanBase* make_cwt_plan_f64(const ssqb_cwt_desc* d, int* err);
 // fills the float32 fast-path helpers of a device-side grid from the descriptor
 struct ReassignGrid;
 int fill_grid(const ssqb_reassign_desc* r, int n_rows, ReassignGrid* g);
+// fill_grid for planes of the given form: SSQB_GRID_STFT for FORM_STFT; any other grid for FORM_CWT
+static inline int fill_form_grid(const ssqb_reassign_desc* r, int n_rows, int form, ReassignGrid* g) {
+  int rc = fill_grid(r, n_rows, g); if (rc) return rc;
+  if (form == FORM_STFT) g->kind = SSQB_GRID_STFT;
+  else if (g->kind == SSQB_GRID_STFT)
+    return set_error(SSQB_E_ARG, "the CWT takes a log, log-piecewise or linear grid");
+  return 0;
+}
 
 // dtype-dispatched stand-alone operators (reassign_ops.cu / stft_ops.cu)
 int run_ssqueeze(int dtype, const void* Wx, const void* dWx, void* Tx, long long B, int na,

@@ -21,7 +21,6 @@
 
 namespace ssqb {
 
-enum { MSSQ_FORM_STFT = 0, MSSQ_FORM_CWT = 1 };
 #define SSQB_MSSQ_MAX_ITER 64
 #define SSQB_MSSQ_MAX_ROWS 32767   // bins and final rows are int16 in shared memory
 
@@ -31,7 +30,7 @@ __device__ __forceinline__ int mssq_bin(int form, cx<T> V, cx<T> dV, double sfs,
                                         const ReassignGrid& g) {
   if (!is_active_exact(V.x, V.y, g.gamma)) return -1;
   const double r = phase_ratio_exact<T>(dV.x, dV.y, V.x, V.y);
-  return bin_from_w_exact(form == MSSQ_FORM_STFT ? fabs(sfs - r) : fabs(r), g);
+  return bin_from_w_exact(form == FORM_STFT ? fabs(sfs - r) : fabs(r), g);
 }
 
 // Final row of a point whose own bin is beta >= 0.  bins[r * stride] is b(r, j) of the point's
@@ -78,7 +77,7 @@ __device__ __forceinline__ short mssq_stft_bin(const StftArgs<T>& A, int k, long
   mssq_split<T>(A, Ck, Cmk, S, dS);
   if (EPI & MSSQ_EPI_SX) A.Sx[o] = S;
   if (A.write_dSx) A.dSx[o] = dS;
-  return (short)mssq_bin<T>(MSSQ_FORM_STFT, S, dS, (double)A.Sfs[k], A.grid);
+  return (short)mssq_bin<T>(FORM_STFT, S, dS, (double)A.Sfs[k], A.grid);
 }
 
 // second pass: the chain from the frame's bins, then red.add of S const[k] into Tx
@@ -100,12 +99,12 @@ __device__ __forceinline__ void mssq_stft_add(const MssqStftArgs<T>& P, int b, i
   if (EPI & MSSQ_EPI_TGT) P.tgt[o] = t;
 }
 
-// the ssq_stft tile (R = ELEMS / M frames) plus the bins of its frames, [M/2 + 1][R] int16
+// the ssq_stft tile (F = ELEMS / M frames) plus the bins of its frames, [M/2 + 1][F] int16
 template <typename T, int LOG_M> struct MssqTile {
   static constexpr int M = 1 << LOG_M;
-  static constexpr int R = Tile<T>::ELEMS / M;
-  static constexpr size_t FFT_BYTES = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);
-  static constexpr size_t SMEM = FFT_BYTES + sizeof(short) * (size_t)(M / 2 + 1) * R;
+  static constexpr int F = Tile<T>::ELEMS / M;
+  static constexpr size_t FFT_BYTES = ((size_t)M * (F + 1) + M) * sizeof(cx<T>);
+  static constexpr size_t SMEM = FFT_BYTES + sizeof(short) * (size_t)(M / 2 + 1) * F;
 };
 
 template <typename T, int LOG_M, int EPI>
@@ -113,7 +112,7 @@ __global__ void __launch_bounds__(Tile<T>::NT)
 mssq_stft_pow2_kernel(const MssqStftArgs<T> P) {
   constexpr int NT = Tile<T>::NT;
   constexpr int M = 1 << LOG_M;
-  constexpr int R = MssqTile<T, LOG_M>::R;
+  constexpr int R = MssqTile<T, LOG_M>::F;
   constexpr int STRIDE = R + 1;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   cx<T>* s = reinterpret_cast<cx<T>*>(smem_raw);          // [M][STRIDE]
@@ -231,7 +230,7 @@ mssq_cwt_kernel(const cx<T>* __restrict__ W, const cx<T>* __restrict__ dW, cx<T>
     short bb = -1;
     if (j < ncols) {
       const long long o = plane + (long long)k * ncols + j;
-      bb = (short)mssq_bin<T>(MSSQ_FORM_CWT, W[o], dW[o], 0.0, g);
+      bb = (short)mssq_bin<T>(FORM_CWT, W[o], dW[o], 0.0, g);
     }
     bins[lin] = bb;
     acc[lin] = mkc<T>((T)0, (T)0);
@@ -295,7 +294,7 @@ mssq_bwd_kernel(int form, const cx<T>* __restrict__ V, const cx<T>* __restrict__
     short bb = -1;
     if (j < ncols) {
       const long long o = plane + (long long)k * ncols + j;
-      bb = (short)mssq_bin<T>(form, V[o], dV[o], form == MSSQ_FORM_STFT ? (double)Sfs[k] : 0.0, g);
+      bb = (short)mssq_bin<T>(form, V[o], dV[o], form == FORM_STFT ? (double)Sfs[k] : 0.0, g);
     }
     bins[lin] = bb;
   }

@@ -70,8 +70,7 @@ int run_mssq_cwt(int dtype, const void* W, const void* dW, const ssqb_reassign_d
   if (!(r->gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
   int rc = mssq_check_rob(rob_host, na); if (rc) return rc;
   ReassignGrid g;
-  rc = fill_grid(r, na, &g); if (rc) return rc;
-  if (g.kind == 3) return set_error(SSQB_E_ARG, "the CWT takes a log, log-piecewise or linear grid");
+  rc = fill_form_grid(r, na, FORM_CWT, &g); if (rc) return rc;
   const int flipud = g.flipud; g.flipud = 0;                   // the chain works on unflipped bins
   return dtype == SSQB_F32
              ? mssq_cwt_t<float>(W, dW, g, flipud, r, rob_host, n_iter, B, na, ncols, Tx, tgt, st)
@@ -102,9 +101,9 @@ int run_mssq_backward(int dtype, int form, const void* V, const void* dV, const 
                       const void* gTx, const void* gV, void* gVout, long long B, int nrows,
                       long long ncols, cudaStream_t st) {
   if (!V || !dV || !r || !r->cst_host || !gTx || !gVout) return set_error(SSQB_E_ARG, "null pointer");
-  if (form != MSSQ_FORM_STFT && form != MSSQ_FORM_CWT) return set_error(SSQB_E_ARG, "bad form %d", form);
-  if (form == MSSQ_FORM_STFT && !Sfs) return set_error(SSQB_E_ARG, "the STFT form needs Sfs");
-  if (form == MSSQ_FORM_CWT && !rob_host) return set_error(SSQB_E_ARG, "the CWT form needs row_of_bin");
+  if (form != FORM_STFT && form != FORM_CWT) return set_error(SSQB_E_ARG, "bad form %d", form);
+  if (form == FORM_STFT && !Sfs) return set_error(SSQB_E_ARG, "the STFT form needs Sfs");
+  if (form == FORM_CWT && !rob_host) return set_error(SSQB_E_ARG, "the CWT form needs row_of_bin");
   if (B < 1 || nrows < 1 || ncols < 1) return set_error(SSQB_E_ARG, "bad shape");
   if (nrows > SSQB_MSSQ_MAX_ROWS) return set_error(SSQB_E_UNSUPP, "rows must be <= %d", SSQB_MSSQ_MAX_ROWS);
   if (n_iter < 1 || n_iter > SSQB_MSSQ_MAX_ITER) return set_error(SSQB_E_ARG, "n_iter must be in [1, 64]");
@@ -112,9 +111,7 @@ int run_mssq_backward(int dtype, int form, const void* V, const void* dV, const 
   int rc = 0;
   if (rob_host) { rc = mssq_check_rob(rob_host, nrows); if (rc) return rc; }
   ReassignGrid g;
-  rc = fill_grid(r, nrows, &g); if (rc) return rc;
-  if (form == MSSQ_FORM_STFT) g.kind = 3;
-  else if (g.kind == 3) return set_error(SSQB_E_ARG, "the CWT takes a log, log-piecewise or linear grid");
+  rc = fill_form_grid(r, nrows, form, &g); if (rc) return rc;
   const int flipud = g.flipud; g.flipud = 0;
   return dtype == SSQB_F32
              ? mssq_bwd_t<float>(form, V, dV, Sfs, g, flipud, r, rob_host, n_iter, gTx, gV, gVout,

@@ -40,7 +40,7 @@ static int ssqueeze_t(const void* Wx, const void* dWx, void* Tx, long long B, in
                       cudaStream_t st) {
   ReassignGrid g;
   int rc = fill_grid(r, na, &g); if (rc) return rc;
-  if (g.kind == 3 && !Sfs) return set_error(SSQB_E_ARG, "SSQB_GRID_STFT needs Sfs_dev");
+  if (g.kind == SSQB_GRID_STFT && !Sfs) return set_error(SSQB_E_ARG, "SSQB_GRID_STFT needs Sfs_dev");
   double* cst = nullptr;
   SSQB_CUDA(cudaMallocAsync((void**)&cst, sizeof(double) * na, st));
   SSQB_CUDA(cudaMemcpyAsync(cst, r->cst_host, sizeof(double) * na, cudaMemcpyHostToDevice, st));
@@ -66,7 +66,7 @@ static int indexed_sum_t(const void* Wx, const void* w, void* Tx, long long B, i
                          long long N, const ssqb_reassign_desc* r, cudaStream_t st) {
   ReassignGrid g;
   int rc = fill_grid(r, na, &g); if (rc) return rc;
-  if (g.kind == 3) g.kind = 2;
+  if (g.kind == SSQB_GRID_STFT) g.kind = SSQB_GRID_LIN;
   double* cst = nullptr;
   SSQB_CUDA(cudaMallocAsync((void**)&cst, sizeof(double) * na, st));
   SSQB_CUDA(cudaMemcpyAsync(cst, r->cst_host, sizeof(double) * na, cudaMemcpyHostToDevice, st));
@@ -96,8 +96,8 @@ static int reassign_bwd_t(const void* Wx, const void* dWx, const void* w, const 
   ReassignGrid g;
   int rc = fill_grid(r, na, &g); if (rc) return rc;
   if (w) {
-    if (g.kind == 3) g.kind = 2;
-  } else if (g.kind == 3 && !Sfs) {
+    if (g.kind == SSQB_GRID_STFT) g.kind = SSQB_GRID_LIN;
+  } else if (g.kind == SSQB_GRID_STFT && !Sfs) {
     return set_error(SSQB_E_ARG, "SSQB_GRID_STFT needs Sfs_dev");
   }
   if (B > 65535) return set_error(SSQB_E_UNSUPP, "batch of %lld > 65535", B);
@@ -134,8 +134,7 @@ template <typename T>
 static int ssq2_cwt_t(const void* const* planes, double dt, long long B, int na, long long N,
                       const ssqb_reassign_desc* r, void* Tx, void* w, cudaStream_t st) {
   ReassignGrid g;
-  int rc = fill_grid(r, na, &g); if (rc) return rc;
-  if (g.kind == 3) return set_error(SSQB_E_ARG, "SSQB_GRID_STFT is not a CWT grid");
+  int rc = fill_form_grid(r, na, FORM_CWT, &g); if (rc) return rc;
   if (B > 65535) return set_error(SSQB_E_UNSUPP, "batch of %lld > 65535", B);
   double* cst = nullptr;
   if (Tx) {

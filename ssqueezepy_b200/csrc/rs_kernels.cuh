@@ -19,8 +19,6 @@
 
 namespace ssqb {
 
-enum { RS_FORM_STFT = TSSQ_FORM_STFT, RS_FORM_CWT = TSSQ_FORM_CWT };
-
 // Targets of one point: false (kk = jt = -1) when the point is dropped.  dV is the frequency
 // derivative plane (dSx / dW), P the time plane (V^{tau g} / A), sfs = Sfs[k] (STFT only).
 template <typename T>
@@ -34,7 +32,7 @@ __device__ __forceinline__ bool rs_target(int form, cx<T> V, cx<T> dV, cx<T> P, 
   jt = tssq_column(delay, j, hop, ncols);
   if (jt < 0) return false;
   const double r = phase_ratio_exact<T>(dV.x, dV.y, V.x, V.y);
-  w = form == RS_FORM_STFT ? fabs(sfs - r) : fabs(r);
+  w = form == FORM_STFT ? fabs(sfs - r) : fabs(r);
   kk = bin_from_w_exact(w, g);
   return true;
 }
@@ -95,7 +93,7 @@ __device__ __forceinline__ void rs_stft_emit(const RsStftArgs<T>& P, int b, int 
   if (EPI & RS_EPI_SX) A.Sx[o] = S;
   if (A.write_dSx) A.dSx[o] = dS;
   if (P.Vt) P.Vt[o] = Vt;
-  rs_point<T, (EPI & RS_EPI_TGT) != 0>(RS_FORM_STFT, S, dS, Vt, (double)A.Sfs[k], frame, A.hop,
+  rs_point<T, (EPI & RS_EPI_TGT) != 0>(FORM_STFT, S, dS, Vt, (double)A.Sfs[k], frame, A.hop,
                                        A.n_hops, A.grid, P.Rx + plane, P.tp, o);
 }
 
@@ -196,7 +194,7 @@ rs_cwt_kernel(const cx<T>* __restrict__ W, const cx<T>* __restrict__ dW,
   if (o >= total) return;
   const long long j = o % ncols;
   const long long plane = (o / ((long long)na * ncols)) * na * ncols;
-  rs_point<T, TGT>(RS_FORM_CWT, W[o], dW[o], Ap[o], 0.0, j, hop, ncols, g, Rx + plane, tp, o);
+  rs_point<T, TGT>(FORM_CWT, W[o], dW[o], Ap[o], 0.0, j, hop, ncols, g, Rx + plane, tp, o);
 }
 
 // ---- backward --------------------------------------------------------------------------------
@@ -217,7 +215,7 @@ rs_bwd_kernel(int form, const cx<T>* __restrict__ V, const cx<T>* __restrict__ d
   cx<T> out = gV ? gV[o] : mkc<T>((T)0, (T)0);
   const cx<T> v = V[o];
   int kk; long long jt; double w = 0.0, delay = 0.0;
-  if (rs_target<T>(form, v, dV[o], P[o], form == RS_FORM_STFT ? (double)Sfs[k] : 0.0, j, hop,
+  if (rs_target<T>(form, v, dV[o], P[o], form == FORM_STFT ? (double)Sfs[k] : 0.0, j, hop,
                    ncols, g, kk, jt, w, delay)) {
     const T s = (T)2 * gRx[plane + (long long)kk * ncols + jt];
     out = mkc<T>(out.x + s * v.x, out.y + s * v.y);

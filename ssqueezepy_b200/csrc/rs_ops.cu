@@ -31,8 +31,7 @@ int run_rs_cwt(int dtype, const void* W, const void* dW, const void* Ap,
   if (B < 1 || na < 1 || ncols < 1 || hop < 1) return set_error(SSQB_E_ARG, "bad shape");
   if (!(gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
   ReassignGrid g;
-  int rc = fill_grid(r, na, &g); if (rc) return rc;
-  if (g.kind == 3) return set_error(SSQB_E_ARG, "the CWT takes a log, log-piecewise or linear grid");
+  int rc = fill_form_grid(r, na, FORM_CWT, &g); if (rc) return rc;
   g.gamma = gamma;
   const long long total = B * na * ncols;
   if (dtype == SSQB_F32) {
@@ -59,14 +58,12 @@ int run_rs_backward(int dtype, int form, const void* V, const void* P1, const vo
                     const void* gV, void* gVout, long long B, int nrows, long long ncols,
                     long long hop, double gamma, cudaStream_t st) {
   if (!V || !P1 || !P2 || !gRx || !gVout) return set_error(SSQB_E_ARG, "null pointer");
-  if (form != RS_FORM_STFT && form != RS_FORM_CWT) return set_error(SSQB_E_ARG, "bad form %d", form);
-  if (form == RS_FORM_STFT && !Sfs) return set_error(SSQB_E_ARG, "the STFT form needs Sfs");
+  if (form != FORM_STFT && form != FORM_CWT) return set_error(SSQB_E_ARG, "bad form %d", form);
+  if (form == FORM_STFT && !Sfs) return set_error(SSQB_E_ARG, "the STFT form needs Sfs");
   if (B < 1 || nrows < 1 || ncols < 1 || hop < 1) return set_error(SSQB_E_ARG, "bad shape");
   if (!(gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
   ReassignGrid g;
-  int rc = fill_grid(r, nrows, &g); if (rc) return rc;
-  if (form == RS_FORM_STFT) g.kind = 3;
-  else if (g.kind == 3) return set_error(SSQB_E_ARG, "the CWT takes a log, log-piecewise or linear grid");
+  int rc = fill_form_grid(r, nrows, form, &g); if (rc) return rc;
   g.gamma = gamma;
   const long long total = B * nrows * ncols;
   return dtype == SSQB_F32

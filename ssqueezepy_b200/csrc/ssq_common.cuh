@@ -133,6 +133,10 @@ struct ReassignGrid {
                       //    (log-piecewise on float32 data, see DESIGN.md)
 };
 
+// Layout of the planes a time-frequency reassignment reads (tssq, rs and mssq kernels, and the
+// `form` argument of their backward ABI): STFT rows are the frequencies Sfs, CWT rows the scales.
+enum { FORM_STFT = 0, FORM_CWT = 1 };
+
 // |z| > gamma exactly as numba types it (algos.py:915): complex64 -> float32
 // magnitude (correctly rounded hypot), compared in float64.
 __device__ __forceinline__ bool is_active_exact(float C, float D, double gamma) {

@@ -7,6 +7,7 @@
 #include "inverse_kernels.cuh"   // IstftArgs, istft_bwd_norm_kernel
 #include "cwt_generic.cuh"      // Gfft<T>: generic-length FFT
 #include <algorithm>
+#include <initializer_list>
 #include <map>
 #include <memory>
 #include <vector>
@@ -128,39 +129,61 @@ static double pack_kappa(const T* win, const T* dwin, int M) {
   return kap;
 }
 
+// The StftArgs fields every forward route fills alike: the framing of d, the [B, N] signal x,
+// the planes (dSx, which may be null, is stored when given) and the packing constant kappa of
+// the two windows transformed together, win (g) and win2 (A.dwin).
 template <typename T>
-static int stft_t(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const void* x,
-                  long long B, void* Sx, void* Tx, void* dSx, bool ssq, cudaStream_t st) {
-  const int M = d->n_fft, nrows = M / 2 + 1;
-  StftArgs<T> A;
-  memset(&A, 0, sizeof(A));
-  A.N = d->N; A.n_fft = M; A.hop = d->hop; A.n1 = d->n1; A.padtype = d->padtype;
+static void stft_args(StftArgs<T>& A, const ssqb_stft_desc* d, const void* x, long long B,
+                      void* Sx, void* dSx, void* Tx, const void* win, const void* win2) {
+  A.N = d->N; A.n_fft = d->n_fft; A.hop = d->hop; A.n1 = d->n1; A.padtype = d->padtype;
   A.modulated = d->modulated; A.B = (int)B;
   A.n_hops = (d->N - 1) / d->hop + 1;
   A.x = (const T*)x; A.Sx = (cx<T>*)Sx; A.dSx = (cx<T>*)dSx; A.Tx = (cx<T>*)Tx;
   A.write_dSx = dSx ? 1 : 0;
-  const T* win = (const T*)d->win_host; const T* dwin = (const T*)d->dwin_host;
-  const double kap = pack_kappa(win, dwin, M);
+  const double kap = pack_kappa((const T*)win, (const T*)win2, d->n_fft);
   A.kappa = (T)kap; A.inv_kappa = (T)(1.0 / kap);
-  // device copies of the small tables: built on the host, cached on the device by content
-  // (a streaming caller repeats the same window / grid thousands of times; without the
-  // cache every call pays an allocation, a copy and a stream synchronisation)
-  std::vector<double> cst((size_t)nrows, 0.0);
-  if (ssq) for (int i = 0; i < nrows; ++i) cst[i] = r->cst_host[i];
+}
+
+// Device copies of a forward route's small tables, built on the host and cached on the device
+// by content (a streaming caller repeats the same window / grid thousands of times; without the
+// cache every call pays an allocation, a copy and a stream synchronisation): the roots, g and
+// win2 (A.dwin), cst and Sfs when asked for, then `extra` windows of n_fft values, whose device
+// pointers go to extra_dev in order.
+template <typename T>
+static int stft_tables(StftArgs<T>& A, const ssqb_stft_desc* d, const void* win2,
+                       const double* cst, bool sfs, cudaStream_t st,
+                       std::initializer_list<const void*> extra = {},
+                       const T** extra_dev = nullptr) {
+  const int M = d->n_fft, nrows = M / 2 + 1;
   BlobBuilder bb;
   const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
-  const size_t o_cst = bb.put(cst.data(), sizeof(double) * nrows);
-  const size_t o_win = bb.put(win, sizeof(T) * M);
-  const size_t o_dwin = bb.put(dwin, sizeof(T) * M);
-  const size_t o_sfs = bb.put(d->Sfs_host, sizeof(T) * nrows);
+  const size_t o_win = bb.put(d->win_host, sizeof(T) * M);
+  const size_t o_win2 = bb.put(win2, sizeof(T) * M);
+  const size_t o_cst = cst ? bb.put(cst, sizeof(double) * nrows) : 0;
+  const size_t o_sfs = sfs ? bb.put(d->Sfs_host, sizeof(T) * nrows) : 0;
+  std::vector<size_t> o_extra;
+  for (const void* e : extra) o_extra.push_back(bb.put(e, sizeof(T) * M));
   unsigned char* blob = nullptr;
   int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
-  A.tw = (const cx<T>*)(blob + o_tw); A.cst = (const double*)(blob + o_cst);
-  A.win = (const T*)(blob + o_win); A.dwin = (const T*)(blob + o_dwin);
-  A.Sfs = (const T*)(blob + o_sfs);
+  A.tw = (const cx<T>*)(blob + o_tw);
+  A.win = (const T*)(blob + o_win); A.dwin = (const T*)(blob + o_win2);
+  if (cst) A.cst = (const double*)(blob + o_cst);
+  if (sfs) A.Sfs = (const T*)(blob + o_sfs);
+  for (size_t i = 0; i < o_extra.size(); ++i) extra_dev[i] = (const T*)(blob + o_extra[i]);
+  return 0;
+}
+
+template <typename T>
+static int stft_t(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const void* x,
+                  long long B, void* Sx, void* Tx, void* dSx, bool ssq, cudaStream_t st) {
+  const int nrows = d->n_fft / 2 + 1;
+  StftArgs<T> A;
+  memset(&A, 0, sizeof(A));
+  stft_args(A, d, x, B, Sx, dSx, Tx, d->win_host, d->dwin_host);
+  int rc = stft_tables(A, d, d->dwin_host, ssq ? r->cst_host : nullptr, true, st);
+  if (rc) return rc;
   if (ssq) {
-    rc = fill_grid(r, nrows, &A.grid); if (rc) return rc;
-    A.grid.kind = 3;
+    rc = fill_form_grid(r, nrows, FORM_STFT, &A.grid); if (rc) return rc;
     SSQB_CUDA(cudaMemsetAsync(Tx, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(cx<T>), st));
   }
   if (ssq && !Sx) return launch_stft<T, STFT_EPI_SSQ_TX>(A, st);      // Tx only
@@ -323,27 +346,38 @@ int run_istft_backward(const ssqb_istft_desc* d, const void* gx, long long B, vo
 // batched Gfft of 3 transforms per frame -> emit, in chunks that keep each buffer at ~128 MB.
 static constexpr size_t kMaxBlockSmem = 227u << 10;    // sm_90 opt-in limit per block
 
-template <typename T>
-static bool stft2_pow2_fits(int logm) {
+// The power-of-two tile routes whose tile does not fit one CTA at every n_fft (second order,
+// reassignment, MSST): TL<T, L> has the tile's shared memory, SMEM bytes, and its F frames per CTA.
+template <typename T, template <typename, int> class TL>
+static bool pow2_tile_fits(int logm) {
   return logm >= 1 && logm <= 12 &&
-         dispatch_log2<1, 12>(logm, [](auto L) { return Stft2Tile<T, L>::SMEM <= kMaxBlockSmem ? 1 : 0; });
+         dispatch_log2<1, 12>(logm, [](auto L) { return TL<T, L>::SMEM <= kMaxBlockSmem ? 1 : 0; });
 }
 
-template <typename T, int EPI>
-static int launch_stft2_pow2(const Stft2Args<T>& P, int logm, cudaStream_t st) {
+// One launch of kernel_of(L), the route's instance for n_fft = 2^logm, over the route's frames
+// (A.B * A.n_hops) in tiles of TL<T, L>::F.  Only instances whose tile fits are instantiated.
+template <typename T, template <typename, int> class TL, typename P, typename KernelOf>
+static int launch_pow2_tile(const P& args, int logm, KernelOf kernel_of, cudaStream_t st) {
   return dispatch_log2<1, 12>(logm, [&](auto L) {
-    using TL = Stft2Tile<T, L>;
-    if constexpr (TL::SMEM > kMaxBlockSmem) {
+    using Tl = TL<T, L>;
+    if constexpr (Tl::SMEM > kMaxBlockSmem) {
       return set_error(SSQB_E_UNSUPP, "n_fft = 2^%d does not fit one CTA", (int)L);
     } else {
-      const long long total = (long long)P.A.B * P.A.n_hops;
-      auto kern = stft2_pow2_kernel<T, L, EPI>;
-      SSQB_CUDA(opt_in_smem(kern, TL::SMEM));
-      kern<<<(unsigned)((total + TL::F - 1) / TL::F), Tile<T>::NT, TL::SMEM, st>>>(P);
+      const long long total = (long long)args.A.B * args.A.n_hops;
+      auto kern = kernel_of(L);
+      SSQB_CUDA(opt_in_smem(kern, Tl::SMEM));
+      kern<<<(unsigned)((total + Tl::F - 1) / Tl::F), Tile<T>::NT, Tl::SMEM, st>>>(args);
       SSQB_LAUNCH_CHECK();
       return 0;
     }
   });
+}
+
+// launch(E) with the epilogue E = (store Sx ? SX : 0) | (write the target planes ? TGT : 0)
+template <int SX, int TGT, typename Launch>
+static int dispatch_sx_tgt(bool sx, bool tgt, Launch launch) {
+  if (sx) return tgt ? launch(std::integral_constant<int, SX | TGT>{}) : launch(std::integral_constant<int, SX>{});
+  return tgt ? launch(std::integral_constant<int, TGT>{}) : launch(std::integral_constant<int, 0>{});
 }
 
 template <typename T, int EPI>
@@ -365,49 +399,31 @@ static int launch_stft2_generic(const Stft2Args<T>& P, cudaStream_t st) {
 template <typename T, int EPI>
 static int launch_stft2(const Stft2Args<T>& P, cudaStream_t st) {
   const int logm = ilog2_exact(P.A.n_fft);
-  return stft2_pow2_fits<T>(logm) ? launch_stft2_pow2<T, EPI>(P, logm, st)
-                                  : launch_stft2_generic<T, EPI>(P, st);
+  if (pow2_tile_fits<T, Stft2Tile>(logm))
+    return launch_pow2_tile<T, Stft2Tile>(P, logm, [](auto L) { return stft2_pow2_kernel<T, L, EPI>; }, st);
+  return launch_stft2_generic<T, EPI>(P, st);
 }
 
 template <typename T>
 static int stft2_t(const ssqb_stft_desc* d, const ssqb_stft2_tables* t2, const ssqb_reassign_desc* r,
                    const void* x, long long B, void* Sx, void* Tx, void* dSx, void* w,
                    cudaStream_t st) {
-  const int M = d->n_fft, nrows = M / 2 + 1;
+  const int nrows = d->n_fft / 2 + 1;
   Stft2Args<T> P;
   memset(&P, 0, sizeof(P));
   StftArgs<T>& A = P.A;
-  A.N = d->N; A.n_fft = M; A.hop = d->hop; A.n1 = d->n1; A.padtype = d->padtype;
-  A.modulated = d->modulated; A.B = (int)B;
-  A.n_hops = (d->N - 1) / d->hop + 1;
-  A.x = (const T*)x; A.Sx = (cx<T>*)Sx; A.dSx = (cx<T>*)dSx; A.Tx = (cx<T>*)Tx;
-  A.write_dSx = dSx ? 1 : 0;
+  stft_args(A, d, x, B, Sx, dSx, Tx, d->win_host, d->dwin_host);
   P.w = (T*)w;
   P.gamma_t = (T)r->gamma;
-  const T* win = (const T*)d->win_host; const T* dwin = (const T*)d->dwin_host;
-  const T* twin = (const T*)t2->twin_host; const T* tdwin = (const T*)t2->tdwin_host;
-  const double kap = pack_kappa(win, dwin, M), kap2 = pack_kappa(twin, tdwin, M);
-  A.kappa = (T)kap; A.inv_kappa = (T)(1.0 / kap);
+  const double kap2 = pack_kappa((const T*)t2->twin_host, (const T*)t2->tdwin_host, d->n_fft);
   P.kappa2 = (T)kap2; P.inv_kappa2 = (T)(1.0 / kap2);
-  BlobBuilder bb;
-  const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
-  const size_t o_cst = bb.put(r->cst_host, sizeof(double) * nrows);
-  const size_t o_win = bb.put(win, sizeof(T) * M);
-  const size_t o_dwin = bb.put(dwin, sizeof(T) * M);
-  const size_t o_sfs = bb.put(d->Sfs_host, sizeof(T) * nrows);
-  const size_t o_ddwin = bb.put(t2->ddwin_host, sizeof(T) * M);
-  const size_t o_twin = bb.put(twin, sizeof(T) * M);
-  const size_t o_tdwin = bb.put(tdwin, sizeof(T) * M);
-  unsigned char* blob = nullptr;
-  int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
-  A.tw = (const cx<T>*)(blob + o_tw); A.cst = (const double*)(blob + o_cst);
-  A.win = (const T*)(blob + o_win); A.dwin = (const T*)(blob + o_dwin);
-  A.Sfs = (const T*)(blob + o_sfs);
-  P.ddwin = (const T*)(blob + o_ddwin);
-  P.twin = (const T*)(blob + o_twin); P.tdwin = (const T*)(blob + o_tdwin);
+  const T* extra[3];
+  int rc = stft_tables(A, d, d->dwin_host, r->cst_host, true, st,
+                       {t2->ddwin_host, t2->twin_host, t2->tdwin_host}, extra);
+  if (rc) return rc;
+  P.ddwin = extra[0]; P.twin = extra[1]; P.tdwin = extra[2];
   if (!Tx) return launch_stft2<T, STFT2_EPI_W>(P, st);
-  rc = fill_grid(r, nrows, &A.grid); if (rc) return rc;
-  A.grid.kind = 3;
+  rc = fill_form_grid(r, nrows, FORM_STFT, &A.grid); if (rc) return rc;
   SSQB_CUDA(cudaMemsetAsync(Tx, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(cx<T>), st));
   return Sx ? launch_stft2<T, STFT2_EPI_SSQ>(P, st) : launch_stft2<T, STFT2_EPI_SSQ_TX>(P, st);
 }
@@ -461,35 +477,18 @@ template <typename T>
 static int tssq_stft_t(const ssqb_stft_desc* d, const void* twin_host, double gamma, const void* x,
                        long long B, void* Sx, void* Ts, void* Vt, int* tgt, void* tau,
                        cudaStream_t st) {
-  const int M = d->n_fft, nrows = M / 2 + 1;
+  const int nrows = d->n_fft / 2 + 1;
   TssqStftArgs<T> P;
   memset(&P, 0, sizeof(P));
   StftArgs<T>& A = P.A;
-  A.N = d->N; A.n_fft = M; A.hop = d->hop; A.n1 = d->n1; A.padtype = d->padtype;
-  A.modulated = d->modulated; A.B = (int)B;
-  A.n_hops = (d->N - 1) / d->hop + 1;
-  A.x = (const T*)x; A.Sx = (cx<T>*)Sx; A.dSx = (cx<T>*)Vt; A.Tx = (cx<T>*)Ts;
-  A.write_dSx = Vt ? 1 : 0;
+  stft_args(A, d, x, B, Sx, Vt, Ts, d->win_host, twin_host);     // g + i kappa tau g
   A.grid.gamma = gamma;
   P.tgt = tgt; P.tau = (T*)tau;
-  const T* win = (const T*)d->win_host; const T* twin = (const T*)twin_host;
-  const double kap = pack_kappa(win, twin, M);
-  A.kappa = (T)kap; A.inv_kappa = (T)(1.0 / kap);
-  BlobBuilder bb;
-  const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
-  const size_t o_win = bb.put(win, sizeof(T) * M);
-  const size_t o_twin = bb.put(twin, sizeof(T) * M);
-  unsigned char* blob = nullptr;
-  int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
-  A.tw = (const cx<T>*)(blob + o_tw);
-  A.win = (const T*)(blob + o_win); A.dwin = (const T*)(blob + o_twin);
+  int rc = stft_tables(A, d, twin_host, nullptr, false, st); if (rc) return rc;
   SSQB_CUDA(cudaMemsetAsync(Ts, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(cx<T>), st));
-  switch ((Sx ? TSSQ_EPI_SX : 0) | (tgt ? TSSQ_EPI_TGT : 0)) {
-    case 0: return launch_tssq_stft<T, 0>(P, st);
-    case TSSQ_EPI_SX: return launch_tssq_stft<T, TSSQ_EPI_SX>(P, st);
-    case TSSQ_EPI_TGT: return launch_tssq_stft<T, TSSQ_EPI_TGT>(P, st);
-    default: return launch_tssq_stft<T, TSSQ_EPI_SX | TSSQ_EPI_TGT>(P, st);
-  }
+  return dispatch_sx_tgt<TSSQ_EPI_SX, TSSQ_EPI_TGT>(Sx, tgt, [&](auto E) {
+    return launch_tssq_stft<T, E>(P, st);
+  });
 }
 
 int run_tssq_stft(const ssqb_stft_desc* d, const void* twin_host, double gamma, const void* x,
@@ -507,31 +506,13 @@ int run_tssq_stft(const ssqb_stft_desc* d, const void* twin_host, double gamma, 
 // Power-of-two n_fft whose 2F transforms per tile fit one CTA (float32 up to 4096, float64 up to
 // 2048): rs_stft_pow2_kernel.  Every other n_fft: stft_frames_kernel (the g / g' sequences) and
 // rs_tau_frames_kernel (tau g) -> one batched Gfft of 2 transforms per frame -> the emit kernel.
-template <typename T>
-static bool rs_pow2_fits(int logm) {
-  return logm >= 1 && logm <= 12 &&
-         dispatch_log2<1, 12>(logm, [](auto L) { return RsTile<T, L>::SMEM <= kMaxBlockSmem ? 1 : 0; });
-}
-
 template <typename T, int EPI>
 static int launch_rs_stft(const RsStftArgs<T>& P, cudaStream_t st) {
   const StftArgs<T>& A = P.A;
   const long long total = (long long)A.B * A.n_hops;
   const int logm = ilog2_exact(A.n_fft);
-  if (rs_pow2_fits<T>(logm)) {
-    return dispatch_log2<1, 12>(logm, [&](auto L) {
-      using TL = RsTile<T, L>;
-      if constexpr (TL::SMEM > kMaxBlockSmem) {
-        return set_error(SSQB_E_UNSUPP, "n_fft = 2^%d does not fit one CTA", (int)L);
-      } else {
-        auto kern = rs_stft_pow2_kernel<T, L, EPI>;
-        SSQB_CUDA(opt_in_smem(kern, TL::SMEM));
-        kern<<<(unsigned)((total + TL::F - 1) / TL::F), Tile<T>::NT, TL::SMEM, st>>>(P);
-        SSQB_LAUNCH_CHECK();
-        return 0;
-      }
-    });
-  }
+  if (pow2_tile_fits<T, RsTile>(logm))
+    return launch_pow2_tile<T, RsTile>(P, logm, [](auto L) { return rs_stft_pow2_kernel<T, L, EPI>; }, st);
   const long long M = A.n_fft, nrows = M / 2 + 1;
   return generic_frames<T>(A.n_fft, total, 2, -1,
       [&](cx<T>* c, long long f0, long long nf) {
@@ -553,42 +534,21 @@ template <typename T>
 static int rs_stft_t(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reassign_desc* r,
                      double gamma, const void* x, long long B, void* Sx, void* Rx, void* dSx,
                      void* Vt, int* kk, int* jt, void* w, void* tau, cudaStream_t st) {
-  const int M = d->n_fft, nrows = M / 2 + 1;
+  const int nrows = d->n_fft / 2 + 1;
   RsStftArgs<T> P;
   memset(&P, 0, sizeof(P));
   StftArgs<T>& A = P.A;
-  A.N = d->N; A.n_fft = M; A.hop = d->hop; A.n1 = d->n1; A.padtype = d->padtype;
-  A.modulated = d->modulated; A.B = (int)B;
-  A.n_hops = (d->N - 1) / d->hop + 1;
-  A.x = (const T*)x; A.Sx = (cx<T>*)Sx; A.dSx = (cx<T>*)dSx;
-  A.write_dSx = dSx ? 1 : 0;
+  stft_args(A, d, x, B, Sx, dSx, nullptr, d->win_host, d->dwin_host);   // the packing of ssq_stft
   P.Rx = (T*)Rx; P.Vt = (cx<T>*)Vt;
   P.tp.kk = kk; P.tp.jt = jt; P.tp.w = (T*)w; P.tp.tau = (T*)tau;
-  const T* win = (const T*)d->win_host; const T* dwin = (const T*)d->dwin_host;
-  const double kap = pack_kappa(win, dwin, M);                 // the packing of ssq_stft
-  A.kappa = (T)kap; A.inv_kappa = (T)(1.0 / kap);
-  BlobBuilder bb;
-  const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
-  const size_t o_win = bb.put(win, sizeof(T) * M);
-  const size_t o_dwin = bb.put(dwin, sizeof(T) * M);
-  const size_t o_twin = bb.put(twin_host, sizeof(T) * M);
-  const size_t o_sfs = bb.put(d->Sfs_host, sizeof(T) * nrows);
-  unsigned char* blob = nullptr;
-  int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
-  A.tw = (const cx<T>*)(blob + o_tw);
-  A.win = (const T*)(blob + o_win); A.dwin = (const T*)(blob + o_dwin);
-  A.Sfs = (const T*)(blob + o_sfs);
-  P.twin = (const T*)(blob + o_twin);
-  rc = fill_grid(r, nrows, &A.grid); if (rc) return rc;
-  A.grid.kind = 3;
+  int rc = stft_tables(A, d, d->dwin_host, nullptr, true, st, {twin_host}, &P.twin);
+  if (rc) return rc;
+  rc = fill_form_grid(r, nrows, FORM_STFT, &A.grid); if (rc) return rc;
   A.grid.gamma = gamma;
   SSQB_CUDA(cudaMemsetAsync(Rx, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(T), st));
-  switch ((Sx ? RS_EPI_SX : 0) | (jt ? RS_EPI_TGT : 0)) {
-    case 0: return launch_rs_stft<T, 0>(P, st);
-    case RS_EPI_SX: return launch_rs_stft<T, RS_EPI_SX>(P, st);
-    case RS_EPI_TGT: return launch_rs_stft<T, RS_EPI_TGT>(P, st);
-    default: return launch_rs_stft<T, RS_EPI_SX | RS_EPI_TGT>(P, st);
-  }
+  return dispatch_sx_tgt<RS_EPI_SX, RS_EPI_TGT>(Sx, jt, [&](auto E) {
+    return launch_rs_stft<T, E>(P, st);
+  });
 }
 
 int run_rs_stft(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reassign_desc* r,
@@ -610,31 +570,13 @@ int run_rs_stft(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reass
 // Power-of-two n_fft whose ssq_stft tile and bins fit one CTA: mssq_stft_pow2_kernel.  Every other
 // n_fft: stft_frames_kernel -> Gfft -> mssq_stft_emit_kernel (one CTA per frame), in
 // generic_frames' chunks.
-template <typename T>
-static bool mssq_pow2_fits(int logm) {
-  return logm >= 1 && logm <= 12 &&
-         dispatch_log2<1, 12>(logm, [](auto L) { return MssqTile<T, L>::SMEM <= kMaxBlockSmem ? 1 : 0; });
-}
-
 template <typename T, int EPI>
 static int launch_mssq_stft(const MssqStftArgs<T>& P, cudaStream_t st) {
   const StftArgs<T>& A = P.A;
   const long long total = (long long)A.B * A.n_hops;
   const int logm = ilog2_exact(A.n_fft);
-  if (mssq_pow2_fits<T>(logm)) {
-    return dispatch_log2<1, 12>(logm, [&](auto L) {
-      using TL = MssqTile<T, L>;
-      if constexpr (TL::SMEM > kMaxBlockSmem) {
-        return set_error(SSQB_E_UNSUPP, "n_fft = 2^%d does not fit one CTA", (int)L);
-      } else {
-        auto kern = mssq_stft_pow2_kernel<T, L, EPI>;
-        SSQB_CUDA(opt_in_smem(kern, TL::SMEM));
-        kern<<<(unsigned)((total + TL::R - 1) / TL::R), Tile<T>::NT, TL::SMEM, st>>>(P);
-        SSQB_LAUNCH_CHECK();
-        return 0;
-      }
-    });
-  }
+  if (pow2_tile_fits<T, MssqTile>(logm))
+    return launch_pow2_tile<T, MssqTile>(P, logm, [](auto L) { return mssq_stft_pow2_kernel<T, L, EPI>; }, st);
   const long long M = A.n_fft;
   const size_t smem = sizeof(short) * (size_t)(M / 2 + 1);
   if (smem > kMaxBlockSmem) return set_error(SSQB_E_UNSUPP, "n_fft = %d: the bins of a frame do not fit one CTA", A.n_fft);
@@ -656,40 +598,19 @@ template <typename T>
 static int mssq_stft_t(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, int n_iter,
                        const void* x, long long B, void* Sx, void* Tx, void* dSx, int* tgt,
                        cudaStream_t st) {
-  const int M = d->n_fft, nrows = M / 2 + 1;
+  const int nrows = d->n_fft / 2 + 1;
   MssqStftArgs<T> P;
   memset(&P, 0, sizeof(P));
   StftArgs<T>& A = P.A;
-  A.N = d->N; A.n_fft = M; A.hop = d->hop; A.n1 = d->n1; A.padtype = d->padtype;
-  A.modulated = d->modulated; A.B = (int)B;
-  A.n_hops = (d->N - 1) / d->hop + 1;
-  A.x = (const T*)x; A.Sx = (cx<T>*)Sx; A.dSx = (cx<T>*)dSx; A.Tx = (cx<T>*)Tx;
-  A.write_dSx = dSx ? 1 : 0;
+  stft_args(A, d, x, B, Sx, dSx, Tx, d->win_host, d->dwin_host);        // the packing of ssq_stft
   P.n_iter = n_iter; P.tgt = tgt;
-  const T* win = (const T*)d->win_host; const T* dwin = (const T*)d->dwin_host;
-  const double kap = pack_kappa(win, dwin, M);                 // the packing of ssq_stft
-  A.kappa = (T)kap; A.inv_kappa = (T)(1.0 / kap);
-  BlobBuilder bb;
-  const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
-  const size_t o_cst = bb.put(r->cst_host, sizeof(double) * nrows);
-  const size_t o_win = bb.put(win, sizeof(T) * M);
-  const size_t o_dwin = bb.put(dwin, sizeof(T) * M);
-  const size_t o_sfs = bb.put(d->Sfs_host, sizeof(T) * nrows);
-  unsigned char* blob = nullptr;
-  int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
-  A.tw = (const cx<T>*)(blob + o_tw); A.cst = (const double*)(blob + o_cst);
-  A.win = (const T*)(blob + o_win); A.dwin = (const T*)(blob + o_dwin);
-  A.Sfs = (const T*)(blob + o_sfs);
-  rc = fill_grid(r, nrows, &A.grid); if (rc) return rc;
-  A.grid.kind = 3;
+  int rc = stft_tables(A, d, d->dwin_host, r->cst_host, true, st); if (rc) return rc;
+  rc = fill_form_grid(r, nrows, FORM_STFT, &A.grid); if (rc) return rc;
   P.flipud = A.grid.flipud; A.grid.flipud = 0;                 // the chain works on unflipped bins
   SSQB_CUDA(cudaMemsetAsync(Tx, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(cx<T>), st));
-  switch ((Sx ? MSSQ_EPI_SX : 0) | (tgt ? MSSQ_EPI_TGT : 0)) {
-    case 0: return launch_mssq_stft<T, 0>(P, st);
-    case MSSQ_EPI_SX: return launch_mssq_stft<T, MSSQ_EPI_SX>(P, st);
-    case MSSQ_EPI_TGT: return launch_mssq_stft<T, MSSQ_EPI_TGT>(P, st);
-    default: return launch_mssq_stft<T, MSSQ_EPI_SX | MSSQ_EPI_TGT>(P, st);
-  }
+  return dispatch_sx_tgt<MSSQ_EPI_SX, MSSQ_EPI_TGT>(Sx, tgt, [&](auto E) {
+    return launch_mssq_stft<T, E>(P, st);
+  });
 }
 
 int run_mssq_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, int n_iter,

@@ -17,13 +17,11 @@
 
 namespace ssqb {
 
-enum { TSSQ_FORM_STFT = 0, TSSQ_FORM_CWT = 1 };
-
 template <typename T>
 __device__ __forceinline__ double tssq_delay(int form, cx<T> V, cx<T> P) {
   const double vr = V.x, vi = V.y, pr = P.x, pi = P.y;
   const double den = __dadd_rn(__dmul_rn(vr, vr), __dmul_rn(vi, vi));
-  const double num = form == TSSQ_FORM_STFT ? __dadd_rn(__dmul_rn(pr, vr), __dmul_rn(pi, vi))
+  const double num = form == FORM_STFT ? __dadd_rn(__dmul_rn(pr, vr), __dmul_rn(pi, vi))
                                             : __dsub_rn(__dmul_rn(pi, vr), __dmul_rn(pr, vi));
   return __ddiv_rn(num, den);
 }
@@ -88,7 +86,7 @@ __device__ __forceinline__ void tssq_stft_emit(const TssqStftArgs<T>& P, int b, 
   const long long row = ((long long)b * nrows + k) * A.n_hops;
   if (EPI & TSSQ_EPI_SX) A.Sx[row + frame] = S;
   if (A.write_dSx) A.dSx[row + frame] = St;
-  tssq_point<T, (EPI & TSSQ_EPI_TGT) != 0>(TSSQ_FORM_STFT, S, St, frame, A.hop, A.n_hops,
+  tssq_point<T, (EPI & TSSQ_EPI_TGT) != 0>(FORM_STFT, S, St, frame, A.hop, A.n_hops,
                                            A.grid.gamma, A.Tx + row, P.tgt, P.tau, row + frame);
 }
 
@@ -161,7 +159,7 @@ tssq_cwt_kernel(const cx<T>* __restrict__ W, const cx<T>* __restrict__ Ap, cx<T>
   const long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (o >= total) return;
   const long long j = o % ncols;
-  tssq_point<T, TGT>(TSSQ_FORM_CWT, W[o], Ap[o], j, hop, ncols, gamma, Ts + (o - j), tgt, tau, o);
+  tssq_point<T, TGT>(FORM_CWT, W[o], Ap[o], j, hop, ncols, gamma, Ts + (o - j), tgt, tau, o);
 }
 
 // ---- backward --------------------------------------------------------------------------------

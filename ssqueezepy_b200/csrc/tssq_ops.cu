@@ -47,7 +47,7 @@ int run_tssq_backward(int dtype, int form, const void* V, const void* P, const v
                       const void* gV, void* gVout, long long B, int nrows, long long ncols,
                       long long hop, double gamma, cudaStream_t st) {
   if (!V || !P || !gTs || !gVout) return set_error(SSQB_E_ARG, "null pointer");
-  if (form != TSSQ_FORM_STFT && form != TSSQ_FORM_CWT) return set_error(SSQB_E_ARG, "bad form %d", form);
+  if (form != FORM_STFT && form != FORM_CWT) return set_error(SSQB_E_ARG, "bad form %d", form);
   if (B < 1 || nrows < 1 || ncols < 1 || hop < 1) return set_error(SSQB_E_ARG, "bad shape");
   const long long total = B * nrows * ncols;
   return dtype == SSQB_F32 ? tssq_bwd_t<float>(form, V, P, gTs, gV, gVout, total, ncols, hop, gamma, st)

@@ -486,6 +486,61 @@ def test_evicted_plan_is_freed_without_gc(S):
     assert not any(alive), alive
 
 
+def _plan_with_companions(N):
+    """(cache key, plan) of the one cached plan of length N that has companions"""
+    from ssqueezepy_b200._cwt import CwtPlan, _CACHE_LOCK
+    with _CACHE_LOCK:
+        keys = [k for k, p in CwtPlan._cache.items() if p.N == N and 'derived' in p.__dict__]
+    assert len(keys) == 1
+    return keys[0], CwtPlan._cache[keys[0]]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('variant,N', [('tssq', 3011), ('rs', 3013), ('mssq', 3017)])
+def test_evicted_variant_plan_is_freed_without_gc(S, variant, N):
+    """As `test_evicted_plan_is_freed_without_gc`, for the companions of `tssq_cwt`,
+    `reassigned_cwt` and `mssq_cwt`: the plan, the A-table plan, the group runner with its
+    scratch and the row_of_bin tables are freed at once with the collector off."""
+    import gc
+    import weakref
+    import torch
+    from ssqueezepy_b200._cwt import CwtPlan, _CACHE_LOCK
+    x = O.chirp(N, 0, 'float32')
+    {'tssq': S.tssq_cwt, 'rs': S.reassigned_cwt, 'mssq': S.mssq_cwt}[variant](x, 'morlet')
+    key, plan = _plan_with_companions(N)
+    held = list(plan.derived.values())
+    o = plan.derived[variant]
+    assert o._scratch is not None
+    assert variant == 'mssq' or isinstance(plan.derived['a_table'], CwtPlan)
+    refs = [weakref.ref(v) for v in [plan, o._scratch] + held]
+    del plan, held, o
+    torch.cuda.synchronize()
+    gc.disable()
+    try:
+        with _CACHE_LOCK:
+            CwtPlan._cache.pop(key)
+        alive = [r() is not None for r in refs]
+    finally:
+        gc.enable()
+    assert not any(alive), alive
+
+
+@pytest.mark.gpu
+def test_one_a_table_plan_per_plan(S):
+    """ssq_cwt(ssq_order=2), tssq_cwt and reassigned_cwt on one plan share a single plan of the
+    a psih'(a xi) table; the second order adds only its D2 plan."""
+    from ssqueezepy_b200._cwt import CwtPlan
+    x = O.chirp(3003, 0, 'float32')
+    S.ssq_cwt(x, 'morlet', ssq_order=2)
+    _, plan = _plan_with_companions(3003)
+    pA = plan.derived['a_table']
+    S.tssq_cwt(x, 'morlet')
+    S.reassigned_cwt(x, 'morlet')
+    o2, ot, ors = plan.derived[('ssq_order', 2)], plan.derived['tssq'], plan.derived['rs']
+    assert o2.pA is pA and ot.pA is pA and ors.pA is pA
+    assert [v for v in plan.derived.values() if isinstance(v, CwtPlan)] == [pA]
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize('wname', ['gmw_centered', 'morlet6'])
 def test_sampling_rate(S, wname):
