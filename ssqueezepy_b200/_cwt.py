@@ -281,13 +281,16 @@ class GroupRunner:
         [B, na, n_cols(hop)] tensor, or None for a plane that lives in the scratch; `views`
         holds each plane's rows of the group.  The group is the whole batch when every plane is
         given.  The scratch only grows, to what the call keeps in it; a call on another stream
-        first waits for the last one that used it."""
+        first waits for the last one that used it, and marks it used on its stream, so that a
+        scratch dropped when it grows is not handed to its allocation stream's next tensor
+        while this call's kernels may still write it."""
         B, na, ncol = xd.shape[0], plan.na, plan.n_cols(hop)
         held = [i for i, p in enumerate(planes) if p is None]
         g = min(self.group, B) if held else B
+        stream = torch.cuda.current_stream()
         with plan._lock:
             if self._done is not None:
-                torch.cuda.current_stream().wait_event(self._done)
+                stream.wait_event(self._done)
             S = None
             if held:
                 size = len(held) * g * na * ncol
@@ -295,6 +298,7 @@ class GroupRunner:
                     self._scratch = None
                     self._scratch = torch.empty(size, dtype=Bk.cplx_dtype(plan.dtype),
                                                 device='cuda')
+                self._scratch.record_stream(stream)
                 S = self._scratch[:size].view(len(held), g, na, ncol)
             for b0 in range(0, B, g):
                 b1 = min(B, b0 + g)

@@ -466,6 +466,8 @@ struct GenericCwtPlan : public CwtPlanBase {
     have_grid = true;
     return 0;
   }
+  // calls share xp_d .. dW_tmp and the adjoint's buffers: ordered as in CwtPlan
+  CallOrder order;
   int exec(const void* xv, long long B, void* Wxv, void* dWxv, void* Txv, bool ssq,
            const double* out_mul_host, bool rpadded, long long hop, cudaStream_t st) override {
     if (B < 1 || !xv || (!Wxv && !ssq)) return set_error(SSQB_E_ARG, "bad arguments");
@@ -473,6 +475,13 @@ struct GenericCwtPlan : public CwtPlanBase {
     if (ssq && rpadded) return set_error(SSQB_E_ARG, "ssq works on the unpadded part");
     { int rc = check_hop(hop, rpadded); if (rc) return rc; }
     if (hop > d.N) hop = d.N;                       // one column either way
+    SSQB_CUDA(order.begin(st));
+    const int rc = exec_body(xv, B, Wxv, dWxv, Txv, ssq, out_mul_host, rpadded, hop, st);
+    order.end(st);
+    return rc;
+  }
+  int exec_body(const void* xv, long long B, void* Wxv, void* dWxv, void* Txv, bool ssq,
+                const double* out_mul_host, bool rpadded, long long hop, cudaStream_t st) {
     const long long n = d.n_up, off = rpadded ? 0 : d.n1;
     const long long Nout = rpadded ? n : (d.N - 1) / hop + 1;
     const long long rows = B * d.na;
@@ -525,19 +534,25 @@ struct GenericCwtPlan : public CwtPlanBase {
   }
   int debug_xh(const void* x, long long B, void* xh, cudaStream_t st) override {
     const long long n = d.n_up;
+    SSQB_CUDA(order.begin(st));
     SSQB_CUDA(xp_d.ensure((size_t)B * (size_t)n));
     gen_pad_kernel<T><<<(unsigned)((B * n + 255) / 256), 256, 0, st>>>((const T*)x, xp_d.p, d.N, n,
                                                                        d.n1, d.padtype, B);
     SSQB_LAUNCH_CHECK();
-    return fft.exec(xp_d.p, (cx<T>*)xh, B, -1, (T)(1.0 / (double)n), st);
+    const int rc = fft.exec(xp_d.p, (cx<T>*)xh, B, -1, (T)(1.0 / (double)n), st);
+    order.end(st);
+    return rc;
   }
   CwtAdjoint<T> adj;
   int backward(const void* gWx, const void* gdWx, long long B, const double* out_mul_host,
                bool rpadded, long long hop, void* gx, cudaStream_t st) override {
     { int rc = check_hop(hop, rpadded); if (rc) return rc; }
+    SSQB_CUDA(order.begin(st));
     CwtArgs<T> A; cwt_common_args(d, scales_d.p, A);
-    return adj.run(d, A, (const cx<T>*)gWx, (const cx<T>*)gdWx, B, out_mul_host, rpadded,
-                   hop < d.N ? hop : d.N, (T*)gx, st);
+    const int rc = adj.run(d, A, (const cx<T>*)gWx, (const cx<T>*)gdWx, B, out_mul_host, rpadded,
+                           hop < d.N ? hop : d.N, (T*)gx, st);
+    order.end(st);
+    return rc;
   }
   int set_profiling(int) override { return 0; }
   int get_profile(double* ms, long long* launches, long long* rows) override {

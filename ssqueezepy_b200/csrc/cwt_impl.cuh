@@ -943,11 +943,14 @@ struct CwtPlan : public CwtPlanBase {
   int set_reassign(const ssqb_reassign_desc* r) override {
     int rc = fill_grid(r, d.na, &grid);
     if (rc) return rc;
-    std::vector<double> c(r->cst_host, r->cst_host + d.na);
-    SSQB_CUDA(cst_d.upload(c));
+    // the next call uploads it on its own stream, behind the calls that may still read cst_d
+    cst_h.assign(r->cst_host, r->cst_host + d.na);
+    cst_dirty = true;
     have_grid = true;
     return 0;
   }
+  std::vector<double> cst_h;
+  bool cst_dirty = false;
 
   // rows of G that fit the scratch budget
   long long rows_per_chunk(int narr, long long total_rows) {
@@ -987,13 +990,11 @@ struct CwtPlan : public CwtPlanBase {
     return 0;
   }
 
-  // Calls on one plan share its scratch, tables and worker streams, so consecutive calls are
-  // ordered on the device whatever streams they arrive on: each call first waits for the
-  // completion event of the previous one (a no-op when both use the same stream).  If a call
+  // Calls on one plan share its scratch, tables and worker streams, so consecutive calls
+  // (forward, backward) are ordered on the device whatever streams they arrive on.  If a call
   // fails half-way, the side / lane streams are still joined into the caller's stream.
-  Event ev_done;
-  bool ev_done_valid = false;
-  long long maps_B = -1;                   // batch size the per-batch row maps were built for
+  CallOrder order;
+  long long maps_B = -1;                  // batch size the per-batch row maps were built for
   // zero-ahead state of the group being launched (see CwtArgs::zero_next)
   int zero_next_ = 0;
   long long zero_off_ = 0;
@@ -1033,8 +1034,11 @@ struct CwtPlan : public CwtPlanBase {
            const double* out_mul_host, bool rpadded, long long hop, cudaStream_t st) override {
     { int rc = check_hop(hop, rpadded); if (rc) return rc; }
     if (hop > d.N) hop = d.N;                       // one column either way
-    if (!ev_done) SSQB_CUDA(ev_done.create());
-    if (ev_done_valid) SSQB_CUDA(cudaStreamWaitEvent(st, ev_done, 0));
+    SSQB_CUDA(order.begin(st));
+    if (cst_dirty) {                         // ordered behind every earlier call on the plan
+      SSQB_CUDA(cst_d.upload_async(cst_h, st));
+      cst_dirty = false;
+    }
     const long long S = (B >= 1) ? group_size(B, ssq, rpadded) : B;
     if (maps_B != S) {
       // the row maps are re-uploaded with blocking copies when the batch size changes:
@@ -1070,8 +1074,7 @@ struct CwtPlan : public CwtPlanBase {
         cudaEventDestroy(e);
       }
     }
-    cudaEventRecord(ev_done, st);
-    ev_done_valid = true;
+    order.end(st);
     return rc;
   }
 
@@ -1238,10 +1241,10 @@ struct CwtPlan : public CwtPlanBase {
       bjobs.clear();
     }
 
-    rc = forward(x, B, xh_d.p, st); if (rc) return rc;
-    const bool use_cut = use_blocks && have_cut && sblk[2].used();
-    if (lanes_on) SSQB_CUDA(cudaEventRecord(ev_lane_fork, st));
-
+    // the two-pass row map: rpadded calls (no blocks) take every routed row two-pass, so the map
+    // changes when rpadded flips at an unchanged B.  The copy is ordered on the caller's stream
+    // (an earlier call on the plan may still read the old map) before ev_lane_fork, which the
+    // lane running the two-pass rows waits for.
     const int* rowmap = nullptr;
     long long two_pass_rows = total_rows;
     if (fast) {
@@ -1254,12 +1257,16 @@ struct CwtPlan : public CwtPlanBase {
           size_t k = 0;
           for (long long b = 0; b < B; ++b)
             for (int a : bs) mp[k++] = (int)(b * d.na + a);
-          SSQB_CUDA(bigmap_d.upload(mp));
+          SSQB_CUDA(bigmap_d.upload_async(mp, st));
           bigmap_B = mkey;
         }
         rowmap = bigmap_d.p;
       }
     }
+
+    rc = forward(x, B, xh_d.p, st); if (rc) return rc;
+    const bool use_cut = use_blocks && have_cut && sblk[2].used();
+    if (lanes_on) SSQB_CUDA(cudaEventRecord(ev_lane_fork, st));
     // (g) gridded narrow-band rows first on the caller's stream: the coarse-grid transforms
     // need only xh; the interpolation kernel (the largest launch of a step) starts as soon
     // as Tx is zeroed
@@ -1364,15 +1371,21 @@ struct CwtPlan : public CwtPlanBase {
   }
 
   int debug_xh(const void* x, long long B, void* xh, cudaStream_t st) override {
-    return forward((const T*)x, B, (cx<T>*)xh, st);
+    SSQB_CUDA(order.begin(st));
+    const int rc = forward((const T*)x, B, (cx<T>*)xh, st);
+    order.end(st);
+    return rc;
   }
   CwtAdjoint<T> adj;
   int backward(const void* gWx, const void* gdWx, long long B, const double* out_mul_host,
                bool rpadded, long long hop, void* gx, cudaStream_t st) override {
     { int rc = check_hop(hop, rpadded); if (rc) return rc; }
+    SSQB_CUDA(order.begin(st));
     CwtArgs<T> A; base_args(A);
-    return adj.run(d, A, (const cx<T>*)gWx, (const cx<T>*)gdWx, B, out_mul_host, rpadded,
-                   hop < d.N ? hop : d.N, (T*)gx, st);
+    const int rc = adj.run(d, A, (const cx<T>*)gWx, (const cx<T>*)gdWx, B, out_mul_host, rpadded,
+                           hop < d.N ? hop : d.N, (T*)gx, st);
+    order.end(st);
+    return rc;
   }
 };
 

@@ -151,10 +151,37 @@ struct DevBuf {
     if (e == cudaSuccess) n = count;
     return e;
   }
+  // blocking copy on the legacy stream: only for tables written before the owner's first call
+  // (plan creation ends in a device synchronise), never for one rewritten between calls
   cudaError_t upload(const std::vector<T>& h) {
     cudaError_t e = ensure(h.size() ? h.size() : 1);
     if (e != cudaSuccess) return e;
     return cudaMemcpy(p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice);
+  }
+  // copy ordered on `st`: kernels queued earlier on `st` still read the old contents, later
+  // ones the new.  A pageable source is staged before the call returns, so `h` may die then.
+  cudaError_t upload_async(const std::vector<T>& h, cudaStream_t st) {
+    cudaError_t e = ensure(h.size() ? h.size() : 1);
+    if (e != cudaSuccess) return e;
+    return cudaMemcpyAsync(p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, st);
+  }
+};
+
+// Orders the calls on one plan on the device, whatever streams they arrive on: each call first
+// waits for the completion event of the previous one (a no-op when both use the same stream).
+// The plan's scratch and the tables it rewrites between calls are then never used by two calls
+// at once.  The host side is not locked: one host thread at a time per plan.
+struct CallOrder {
+  Event done;
+  bool valid = false;
+  cudaError_t begin(cudaStream_t st) {
+    if (!done) { cudaError_t e = done.create(); if (e != cudaSuccess) return e; }
+    return valid ? cudaStreamWaitEvent(st, done, 0) : cudaSuccess;
+  }
+  cudaError_t end(cudaStream_t st) {
+    cudaError_t e = cudaEventRecord(done, st);
+    valid = valid || e == cudaSuccess;
+    return e;
   }
 };
 
