@@ -366,6 +366,39 @@ int ssqb_mssq_backward(int dtype, int form, const void* V_dev, const void* dV_de
                        const void* gV_dev, void* gVout_dev, int64_t B, int nrows, int64_t n_cols,
                        void* stream);
 
+/* ---- synchroextracting / transient-extracting transforms (SET: Yu, Wang & Zhao, IEEE Trans.
+ * Ind. Electron. 64(10), 2017; TET: Yu, IEEE Trans. Instrum. Meas. 69(2), 2020; not in the
+ * reference) -- the transform's own coefficients, kept where the reassignment leaves them:
+ *   mode 0 (SET): kept iff |V| > gamma and row_of_bin[b(k, j)] == k
+ *   mode 1 (TET): kept iff |V| > gamma, the delay is finite and jt == j
+ *   Te[k][j] = V[k][j] where kept, 0 elsewhere;  mask[k][j] = kept (uint8 0 / 1)
+ * b is the bin the fused first-order ssq_* route gives the point before its flip (w = |Sfs[k] - r|
+ * for the STFT, |r| for the CWT, on the grid of r; the gamma of r is replaced by `gamma`), the
+ * bin of ssqb_mssq_* at n_iter = 1; row_of_bin is the identity for the STFT.  jt is the tssq_*
+ * target column.  Every entry of Te is written once (no zero fill, no atomics), so Te is
+ * bit-reproducible and the same batched or one signal at a time.  mask_dev may be NULL.        */
+/* STFT, fused: d as for ssqb_stft_exec.  Mode 0 reads r (as for ssqb_ssq_stft_exec) and
+ * transforms g and g' as ssq_stft does; mode 1 reads twin_host (tau g, as for
+ * ssqb_tssq_stft_exec) and transforms g and tau g as tssq_stft does; the other may be NULL.
+ * Sx_dev may be NULL (not stored); on the power-of-two route it holds the bits of the matching
+ * ssq_stft / tssq_stft.  Planes [B][n_fft/2+1][n_hops].                                        */
+int ssqb_extract_stft_exec(const ssqb_stft_desc* d, const void* twin_host,
+                           const ssqb_reassign_desc* r, int mode, double gamma, const void* x_dev,
+                           int64_t B, void* Sx_dev, void* Te_dev, uint8_t* mask_dev,
+                           void* stream);
+/* CWT: W_dev and P_dev [B][na][n_cols] complex (the columns j * hop of the full planes): P = dW
+ * for mode 0, A = ifft(a psih'(a xi) xh) for mode 1.  Mode 0 reads r (the descriptor of the fused
+ * ssq_cwt) and row_of_bin_host [na], the scale row of each bin; mode 1 neither (may be NULL).
+ * One thread per point.                                                                       */
+int ssqb_extract_cwt(int dtype, int mode, const void* W_dev, const void* P_dev,
+                     const ssqb_reassign_desc* r, const int32_t* row_of_bin_host, int64_t B,
+                     int na, int64_t n_cols, int64_t hop, double gamma, void* Te_dev,
+                     uint8_t* mask_dev, void* stream);
+/* backward of both (torch.autograd), the kept set held: gVout = gV + mask gTe over `total`
+ * points (gV_dev may be NULL = 0 and may alias gVout_dev).  One thread per point, no atomics. */
+int ssqb_extract_backward(int dtype, const uint8_t* mask_dev, const void* gTe_dev,
+                          const void* gV_dev, void* gVout_dev, int64_t total, void* stream);
+
 /* ---- inverse transforms (column reductions / overlap-add) -------------------------- */
 /* Weighted real-part column sum, the core of
  *   issq_cwt  (_ssq_cwt.py:366-377: `Tx.real.sum(axis=0) * (2 / Css)`)

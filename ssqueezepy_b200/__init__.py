@@ -17,6 +17,8 @@ from ._ssq_stft import ssq_stft, issq_stft, phase_stft
 from ._tssq import tssq_stft, tssq_cwt
 from ._reassigned import reassigned_stft, reassigned_cwt
 from ._mssq import mssq_stft, mssq_cwt
+from ._extract import (synchroextract_stft, transient_extract_stft, synchroextract_cwt,
+                       transient_extract_cwt, isynchroextract_stft, isynchroextract_cwt)
 from .ssqueezing import ssqueeze
 from .experimental import phase_ssqueeze, phase_transform
 from .ridge_extraction import extract_ridges

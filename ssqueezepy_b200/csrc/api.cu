@@ -361,6 +361,24 @@ int ssqb_mssq_backward(int dtype, int form, const void* V, const void* dV, const
                            nrows, n_cols, (cudaStream_t)stream);
 }
 
+int ssqb_extract_stft_exec(const ssqb_stft_desc* d, const void* twin_host,
+                           const ssqb_reassign_desc* r, int mode, double gamma, const void* x,
+                           int64_t B, void* Sx, void* Te, uint8_t* mask, void* stream) {
+  return run_extract_stft(d, twin_host, r, mode, gamma, x, B, Sx, Te, mask, (cudaStream_t)stream);
+}
+
+int ssqb_extract_cwt(int dtype, int mode, const void* W, const void* P, const ssqb_reassign_desc* r,
+                     const int32_t* row_of_bin, int64_t B, int na, int64_t n_cols, int64_t hop,
+                     double gamma, void* Te, uint8_t* mask, void* stream) {
+  return run_extract_cwt(dtype, mode, W, P, r, row_of_bin, B, na, n_cols, hop, gamma, Te, mask,
+                         (cudaStream_t)stream);
+}
+
+int ssqb_extract_backward(int dtype, const uint8_t* mask, const void* gTe, const void* gV,
+                          void* gVout, int64_t total, void* stream) {
+  return run_extract_backward(dtype, mask, gTe, gV, gVout, total, (cudaStream_t)stream);
+}
+
 int ssqb_extract_ridges(int dtype, const void* Tf, int64_t B, int na, int64_t N, const double* ls_host,
                         const double* scales_host, double penalty, double eps, int n_ridges, int bw,
                         int64_t* idx_dev, void* f_dev, void* e_dev, void* stream) {

@@ -267,6 +267,15 @@ int run_mssq_backward(int dtype, int form, const void* V, const void* dV, const 
                       const ssqb_reassign_desc* r, const int* rob_host, int n_iter,
                       const void* gTx, const void* gV, void* gVout, long long B, int nrows,
                       long long ncols, cudaStream_t st);
+// synchroextracting / transient-extracting transforms (stft_ops.cu, extract_ops.cu)
+int run_extract_stft(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reassign_desc* r,
+                     int mode, double gamma, const void* x, long long B, void* Sx, void* Te,
+                     unsigned char* mask, cudaStream_t st);
+int run_extract_cwt(int dtype, int mode, const void* W, const void* P, const ssqb_reassign_desc* r,
+                    const int* rob_host, long long B, int na, long long ncols, long long hop,
+                    double gamma, void* Te, unsigned char* mask, cudaStream_t st);
+int run_extract_backward(int dtype, const unsigned char* mask, const void* gTe, const void* gV,
+                         void* gVout, long long total, cudaStream_t st);
 int run_istft_backward(const ssqb_istft_desc* d, const void* gx, long long B, void* gSx,
                        cudaStream_t st);
 // inverse_ops.cu

@@ -4,6 +4,7 @@
 #include "tssq_kernels.cuh"
 #include "rs_kernels.cuh"
 #include "mssq_kernels.cuh"
+#include "extract_kernels.cuh"
 #include "inverse_kernels.cuh"   // IstftArgs, istft_bwd_norm_kernel
 #include "cwt_generic.cuh"      // Gfft<T>: generic-length FFT
 #include <algorithm>
@@ -625,6 +626,80 @@ int run_mssq_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, int n_it
   if (d->n_fft / 2 + 1 > SSQB_MSSQ_MAX_ROWS) return set_error(SSQB_E_UNSUPP, "n_fft must be < 65534");
   return d->dtype == SSQB_F32 ? mssq_stft_t<float>(d, r, n_iter, x, B, Sx, Tx, dSx, tgt, st)
                               : mssq_stft_t<double>(d, r, n_iter, x, B, Sx, Tx, dSx, tgt, st);
+}
+
+// ---- synchroextracting / transient-extracting STFT (extract_kernels.cuh) ----------------------
+// The first order's routes: extract_stft_pow2_kernel for n_fft = 2 .. 4096 (the tile of
+// tssq_stft_pow2_kernel), otherwise stft_frames_kernel -> Gfft -> extract_stft_emit_kernel in
+// generic_frames' chunks.  SET packs g' (ssq_stft's transform), TET packs tau g (tssq_stft's).
+template <typename T, int MODE, int EPI>
+static int launch_extract_stft(const ExtractStftArgs<T>& P, cudaStream_t st) {
+  const StftArgs<T>& A = P.A;
+  const long long total = (long long)A.B * A.n_hops;
+  if (stft_pow2_tile(A.n_fft)) {
+    return dispatch_log2<1, 12>(ilog2_exact(A.n_fft), [&](auto L) {
+      constexpr int M = 1 << L; constexpr int R = Tile<T>::ELEMS / M;
+      const size_t smem = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);
+      auto kern = extract_stft_pow2_kernel<T, L, MODE, EPI>;
+      SSQB_CUDA(opt_in_smem(kern, smem));
+      kern<<<(unsigned)((total + R - 1) / R), Tile<T>::NT, smem, st>>>(P);
+      SSQB_LAUNCH_CHECK();
+      return 0;
+    });
+  }
+  const long long M = A.n_fft, nrows = M / 2 + 1;
+  return generic_frames<T>(A.n_fft, total, 1, -1,
+      [&](cx<T>* c, long long f0, long long nf) {
+        stft_frames_kernel<T, STFT_EPI_PLAIN><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(A, c, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      },
+      [&](const cx<T>* C, long long f0, long long nf) {
+        extract_stft_emit_kernel<T, MODE, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(P, C, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      }, st);
+}
+
+template <typename T>
+static int extract_stft_t(const ssqb_stft_desc* d, const void* twin_host,
+                          const ssqb_reassign_desc* r, int mode, double gamma, const void* x,
+                          long long B, void* Sx, void* Te, unsigned char* mask, cudaStream_t st) {
+  const int nrows = d->n_fft / 2 + 1;
+  const bool set = mode == EXTRACT_SET;
+  const void* win2 = set ? d->dwin_host : twin_host;
+  ExtractStftArgs<T> P;
+  memset(&P, 0, sizeof(P));
+  StftArgs<T>& A = P.A;
+  stft_args(A, d, x, B, Sx, nullptr, Te, d->win_host, win2);      // g + i kappa (g' or tau g)
+  P.mask = mask;
+  int rc = stft_tables(A, d, win2, nullptr, set, st); if (rc) return rc;
+  if (set) {
+    rc = fill_form_grid(r, nrows, FORM_STFT, &A.grid); if (rc) return rc;
+    A.grid.flipud = 0;                                     // the kept test reads unflipped bins
+  }
+  A.grid.gamma = gamma;
+  return dispatch_sx_tgt<EXTRACT_EPI_SX, EXTRACT_EPI_MASK>(Sx, mask, [&](auto E) {
+    return set ? launch_extract_stft<T, EXTRACT_SET, E>(P, st)
+               : launch_extract_stft<T, EXTRACT_TET, E>(P, st);
+  });
+}
+
+int run_extract_stft(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reassign_desc* r,
+                     int mode, double gamma, const void* x, long long B, void* Sx, void* Te,
+                     unsigned char* mask, cudaStream_t st) {
+  if (!d || !x || !Te) return set_error(SSQB_E_ARG, "null pointer");
+  if (mode != EXTRACT_SET && mode != EXTRACT_TET) return set_error(SSQB_E_ARG, "bad mode %d", mode);
+  if (!d->win_host || !d->dwin_host || !d->Sfs_host) return set_error(SSQB_E_ARG, "null table");
+  if (mode == EXTRACT_SET && (!r || !r->cst_host))
+    return set_error(SSQB_E_ARG, "the synchroextracting mode needs the reassignment descriptor");
+  if (mode == EXTRACT_TET && !twin_host)
+    return set_error(SSQB_E_ARG, "the transient-extracting mode needs tau g");
+  if (!(gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
+  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
+  return d->dtype == SSQB_F32
+             ? extract_stft_t<float>(d, twin_host, r, mode, gamma, x, B, Sx, Te, mask, st)
+             : extract_stft_t<double>(d, twin_host, r, mode, gamma, x, B, Sx, Te, mask, st);
 }
 
 }  // namespace ssqb
