@@ -15,7 +15,7 @@
 #pragma once
 #include "stft_kernels.cuh"
 #include "tssq_kernels.cuh"   // tssq_delay, tssq_column
-#include "mssq_kernels.cuh"   // mssq_bin, mssq_split
+#include "mssq_kernels.cuh"   // mssq_bin
 
 namespace ssqb {
 
@@ -35,95 +35,33 @@ __device__ __forceinline__ bool extract_kept(int form, cx<T> V, cx<T> P, double 
   return tssq_column(tssq_delay<T>(form, V, P), j, hop, ncols) == j;
 }
 
-// ---- STFT: one packed transform per frame ------------------------------------------------------
-// SET packs g + i kappa g' (ssq_stft's transform, so Sx has its bits); TET packs g + i kappa tau g
-// (tssq_stft's).  StftArgs carries the framing, Sx (stored with EXTRACT_EPI_SX), Tx = Te, Sfs and
-// the grid (SET: flipud 0; both: gamma).
+// ---- STFT: the first order's route, g + i kappa win2 ----------------------------------------------
+// SET packs win2 = g' (ssq_stft's transform, so Sx has its bits); TET packs win2 = tau g
+// (tssq_stft's).  A carries the framing, Sx (stored with EXTRACT_EPI_SX), Tx = Te, Sfs and the
+// grid (SET: flipud 0; both: gamma).
+// bit 0: store Sx; bit 1: write the mask; bit 2: the transient-extracting test (else SET)
+enum { EXTRACT_EPI_SX = 1, EXTRACT_EPI_MASK = 2, EXTRACT_EPI_TET = 4 };
+
 template <typename T>
-struct ExtractStftArgs {
-  StftArgs<T> A;
+struct ExtractStftArgs : Stft1Args<T> {
   unsigned char* mask;      // [B][n_fft/2+1][n_hops] kept set (EXTRACT_EPI_MASK) or null
+
+  template <int EPI, class Bins>
+  __device__ __forceinline__ void emit(int b, int k, long long frame, const Bins& C, int mk) const {
+    constexpr int MODE = (EPI & EXTRACT_EPI_TET) ? EXTRACT_TET : EXTRACT_SET;
+    const StftArgs<T>& A = this->A;
+    cx<T> S, D;
+    hermitian_split<T>(C(0, k), C(0, mk), A.inv_kappa, S, D);
+    const int nrows = A.n_fft / 2 + 1;
+    const long long o = ((long long)b * nrows + k) * A.n_hops + frame;
+    if (EPI & EXTRACT_EPI_SX) A.Sx[o] = S;
+    const bool keep = extract_kept<T, MODE>(FORM_STFT, S, D,
+                                            MODE == EXTRACT_SET ? (double)A.Sfs[k] : 0.0, A.grid,
+                                            nullptr, k, frame, A.hop, A.n_hops);
+    A.Tx[o] = keep ? S : mkc<T>((T)0, (T)0);
+    if (EPI & EXTRACT_EPI_MASK) mask[o] = keep ? 1 : 0;
+  }
 };
-
-// bit 0: store Sx; bit 1: write the mask
-enum { EXTRACT_EPI_SX = 1, EXTRACT_EPI_MASK = 2 };
-
-template <typename T, int MODE, int EPI>
-__device__ __forceinline__ void extract_stft_emit(const ExtractStftArgs<T>& P, int b, int k,
-                                                  long long frame, cx<T> Ck, cx<T> Cmk) {
-  const StftArgs<T>& A = P.A;
-  cx<T> S, D;
-  mssq_split<T>(A, Ck, Cmk, S, D);          // stft_emit's arithmetic, for both packings
-  const int nrows = A.n_fft / 2 + 1;
-  const long long o = ((long long)b * nrows + k) * A.n_hops + frame;
-  if (EPI & EXTRACT_EPI_SX) A.Sx[o] = S;
-  const bool keep = extract_kept<T, MODE>(FORM_STFT, S, D,
-                                          MODE == EXTRACT_SET ? (double)A.Sfs[k] : 0.0, A.grid,
-                                          nullptr, k, frame, A.hop, A.n_hops);
-  A.Tx[o] = keep ? S : mkc<T>((T)0, (T)0);
-  if (EPI & EXTRACT_EPI_MASK) P.mask[o] = keep ? 1 : 0;
-}
-
-// power-of-two n_fft: the framing and transform of stft_pow2_kernel, the extraction epilogue
-template <typename T, int LOG_M, int MODE, int EPI>
-__global__ void __launch_bounds__(Tile<T>::NT)
-extract_stft_pow2_kernel(const ExtractStftArgs<T> P) {
-  constexpr int NT = Tile<T>::NT;
-  constexpr int M = 1 << LOG_M;
-  constexpr int R = Tile<T>::ELEMS / M;
-  constexpr int STRIDE = R + 1;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  cx<T>* s = reinterpret_cast<cx<T>*>(smem_raw);          // [M][STRIDE]
-  cx<T>* tw = s + (size_t)M * STRIDE;                     // [M]
-  const StftArgs<T>& A = P.A;
-  const int tid = threadIdx.x;
-  const long long total_frames = (long long)A.B * A.n_hops;
-  const long long f0 = (long long)blockIdx.x * R;
-
-  for (int m = tid; m < M; m += NT) tw[m] = A.tw[m];
-#pragma unroll 1
-  for (int lin = tid; lin < M * R; lin += NT) {
-    const int r = lin % R, l = lin / R;
-    const long long fr = f0 + r;
-    cx<T> z = mkc<T>((T)0, (T)0);
-    if (fr < total_frames) {
-      const int b = (int)(fr / A.n_hops);
-      const long long i = fr - (long long)b * A.n_hops;
-      const long long src = pad_src_index(frame_src(l, i, A.hop, M, A.modulated), A.n1, A.N, A.padtype);
-      const T v = (src >= 0) ? A.x[(long long)b * A.N + src] : (T)0;
-      z = mkc<T>(v * A.win[l], -(v * A.dwin[l]) * A.kappa);  // conj(c)
-    }
-    s[l * STRIDE + r] = z;
-  }
-  __syncthreads();
-  block_ifft<T, LOG_M, R, NT, STRIDE>(s, tw);
-#pragma unroll 1
-  for (int lin = tid; lin < (M / 2 + 1) * R; lin += NT) {
-    const int r = lin % R, k = lin / R;
-    const long long fr = f0 + r;
-    if (fr >= total_frames) continue;
-    const int b = (int)(fr / A.n_hops);
-    const long long i = fr - (long long)b * A.n_hops;
-    extract_stft_emit<T, MODE, EPI>(P, b, k, i, cconj<T>(s[k * STRIDE + r]),
-                                    cconj<T>(s[((M - k) & (M - 1)) * STRIDE + r]));
-  }
-}
-
-// any other n_fft: stft_frames_kernel<T, STFT_EPI_PLAIN> (the same packing), one batched Gfft,
-// then this epilogue, one thread per point
-template <typename T, int MODE, int EPI>
-__global__ void __launch_bounds__(256)
-extract_stft_emit_kernel(const ExtractStftArgs<T> P, const cx<T>* __restrict__ C, long long f0,
-                         long long nf) {
-  const int M = P.A.n_fft, nrows = M / 2 + 1;
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= nf * nrows) return;
-  const int k = (int)(idx / nf); const long long fl = idx - (long long)k * nf;   // frames fastest
-  const long long fr = f0 + fl;
-  const int b = (int)(fr / P.A.n_hops);
-  const long long i = fr - (long long)b * P.A.n_hops;
-  extract_stft_emit<T, MODE, EPI>(P, b, k, i, C[fl * M + k], C[fl * M + (k ? M - k : 0)]);
-}
 
 // ---- CWT: one thread per point of the [B][na][ncols] planes W, P -------------------------------
 // A pure streaming kernel: reads W and P, writes Te and (MASK) the mask.

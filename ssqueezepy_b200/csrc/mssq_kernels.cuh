@@ -48,33 +48,33 @@ __device__ __forceinline__ int mssq_chain(int beta, int n_iter, const short* bin
 }
 
 // ---- STFT -------------------------------------------------------------------------------------
-// StftArgs carries the ssq_stft framing, tables, Sx (stored with MSSQ_EPI_SX), dSx (stored when
-// write_dSx), Tx (zeroed by the host), Sfs, cst and the grid (flipud 0, gamma set).
-template <typename T>
-struct MssqStftArgs {
-  StftArgs<T> A;
-  int n_iter, flipud;
-  int* tgt;                 // [B][n_fft/2+1][n_hops] final rows (-1 = dropped), MSSQ_EPI_TGT
-};
-
+// The first order's packing.  A carries the ssq_stft framing, tables, Sx (stored with
+// MSSQ_EPI_SX), dSx (stored when write_dSx), Tx (zeroed by the host), Sfs, cst and the grid
+// (flipud 0, gamma set).
 // bit 0: store Sx; bit 1: write the target plane
 enum { MSSQ_EPI_SX = 1, MSSQ_EPI_TGT = 2 };
 
-// S and dS of bin k from the packed transform (stft_emit's arithmetic, so Sx has its bits)
+// the ssq_stft tile (F = ELEMS / M frames) plus the bins of its frames, [M/2 + 1][F] int16
+template <typename T, int LOG_M> struct MssqTile {
+  static constexpr int M = 1 << LOG_M;
+  static constexpr int F = Tile<T>::ELEMS / M;
+  static constexpr size_t FFT_BYTES = ((size_t)M * (F + 1) + M) * sizeof(cx<T>);
+  static constexpr size_t SMEM = FFT_BYTES + sizeof(short) * (size_t)(M / 2 + 1) * F;
+};
+
 template <typename T>
-__device__ __forceinline__ void mssq_split(const StftArgs<T>& A, cx<T> Ck, cx<T> Cmk, cx<T>& S,
-                                           cx<T>& dS) {
-  const T h = (T)0.5;
-  S  = mkc<T>((Ck.x + Cmk.x) * h, (Ck.y - Cmk.y) * h);
-  dS = mkc<T>((Ck.y + Cmk.y) * h * A.inv_kappa, (Cmk.x - Ck.x) * h * A.inv_kappa);
-}
+struct MssqStftArgs : Stft1Args<T> {
+  int n_iter, flipud;
+  int* tgt;                 // [B][n_fft/2+1][n_hops] final rows (-1 = dropped), MSSQ_EPI_TGT
+  template <int LOG_M> using Tile = MssqTile<T, LOG_M>;
+};
 
 // first pass of a point: the Sx / dSx stores and its bin
 template <typename T, int EPI>
 __device__ __forceinline__ short mssq_stft_bin(const StftArgs<T>& A, int k, long long o,
                                                cx<T> Ck, cx<T> Cmk) {
   cx<T> S, dS;
-  mssq_split<T>(A, Ck, Cmk, S, dS);
+  hermitian_split<T>(Ck, Cmk, A.inv_kappa, S, dS);
   if (EPI & MSSQ_EPI_SX) A.Sx[o] = S;
   if (A.write_dSx) A.dSx[o] = dS;
   return (short)mssq_bin<T>(FORM_STFT, S, dS, (double)A.Sfs[k], A.grid);
@@ -91,7 +91,7 @@ __device__ __forceinline__ void mssq_stft_add(const MssqStftArgs<T>& P, int b, i
   int t = -1;
   if (b0 >= 0) {
     cx<T> S, dS;
-    mssq_split<T>(A, Ck, Cmk, S, dS);
+    hermitian_split<T>(Ck, Cmk, A.inv_kappa, S, dS);
     t = mssq_chain(b0, P.n_iter, bins, stride, nullptr, nrows - 1, P.flipud);
     const T cc = (T)A.cst[k];
     atomic_add_cx<T>(&A.Tx[((long long)b * nrows + t) * A.n_hops + frame], S.x * cc, S.y * cc);
@@ -99,14 +99,8 @@ __device__ __forceinline__ void mssq_stft_add(const MssqStftArgs<T>& P, int b, i
   if (EPI & MSSQ_EPI_TGT) P.tgt[o] = t;
 }
 
-// the ssq_stft tile (F = ELEMS / M frames) plus the bins of its frames, [M/2 + 1][F] int16
-template <typename T, int LOG_M> struct MssqTile {
-  static constexpr int M = 1 << LOG_M;
-  static constexpr int F = Tile<T>::ELEMS / M;
-  static constexpr size_t FFT_BYTES = ((size_t)M * (F + 1) + M) * sizeof(cx<T>);
-  static constexpr size_t SMEM = FFT_BYTES + sizeof(short) * (size_t)(M / 2 + 1) * F;
-};
-
+// power-of-two n_fft: the framed-transform tile of the first order, then two passes over its
+// bins with a barrier between them (every bin of a frame before any chain walks it)
 template <typename T, int LOG_M, int EPI>
 __global__ void __launch_bounds__(Tile<T>::NT)
 mssq_stft_pow2_kernel(const MssqStftArgs<T> P) {
@@ -123,24 +117,7 @@ mssq_stft_pow2_kernel(const MssqStftArgs<T> P) {
   const int nrows = M / 2 + 1;
   const long long total_frames = (long long)A.B * A.n_hops;
   const long long f0 = (long long)blockIdx.x * R;
-
-  for (int m = tid; m < M; m += NT) tw[m] = A.tw[m];
-#pragma unroll 1
-  for (int lin = tid; lin < M * R; lin += NT) {
-    const int r = lin % R, l = lin / R;
-    const long long fr = f0 + r;
-    cx<T> z = mkc<T>((T)0, (T)0);
-    if (fr < total_frames) {
-      const int b = (int)(fr / A.n_hops);
-      const long long i = fr - (long long)b * A.n_hops;
-      const long long src = pad_src_index(frame_src(l, i, A.hop, M, A.modulated), A.n1, A.N, A.padtype);
-      const T v = (src >= 0) ? A.x[(long long)b * A.N + src] : (T)0;
-      z = mkc<T>(v * A.win[l], -(v * A.dwin[l]) * A.kappa);   // conj(c), as stft_pow2_kernel
-    }
-    s[l * STRIDE + r] = z;
-  }
-  __syncthreads();
-  block_ifft<T, LOG_M, R, NT, STRIDE>(s, tw);
+  frame_tile<T, MssqStftArgs<T>, LOG_M, R>(P, s, tw, f0);
 #pragma unroll 1
   for (int lin = tid; lin < nrows * R; lin += NT) {
     const int r = lin % R, k = lin / R;
@@ -170,7 +147,7 @@ mssq_stft_pow2_kernel(const MssqStftArgs<T> P) {
 }
 
 // any other n_fft: C[fl][k] is the transform of the packed sequence of frame f0 + fl
-// (stft_frames_kernel + Gfft); one CTA per frame, the frame's bins in shared memory
+// (the first order's stft_frames_kernel + Gfft); one CTA per frame, the frame's bins in shared memory
 template <typename T, int EPI>
 __global__ void __launch_bounds__(256)
 mssq_stft_emit_kernel(const MssqStftArgs<T> P, const cx<T>* __restrict__ C, long long f0) {

@@ -66,8 +66,19 @@ __device__ __forceinline__ void rs_point(int form, cx<T> V, cx<T> dV, cx<T> P, d
 }
 
 // ---- STFT: (g + i kappa g') as in ssq_stft, plus tau g in a transform of its own --------------
-// StftArgs carries the ssq_stft framing, g / g' tables, kappa, Sx (may be null), dSx (stored when
+// A carries the ssq_stft framing, g / g' tables, kappa, Sx (may be null), dSx (stored when
 // write_dSx), Sfs and grid (grid.gamma = gamma); Tx is unused.
+// bit 0: store Sx; bit 1: write the target planes
+enum { RS_EPI_SX = 1, RS_EPI_TGT = 2 };
+
+// frames per CTA of the power-of-two kernel: F frames, 2F transforms (F packed g / g', F tau g),
+// at least 8 NT elements per transform batch
+template <typename T, int LOG_M> struct RsTile {
+  static constexpr int M = 1 << LOG_M;
+  static constexpr int F = (Tile<T>::ELEMS / 2) / M > 0 ? (Tile<T>::ELEMS / 2) / M : 1;
+  static constexpr size_t SMEM = ((size_t)M * (2 * F + 1) + M) * sizeof(cx<T>);
+};
+
 template <typename T>
 struct RsStftArgs {
   StftArgs<T> A;
@@ -75,114 +86,30 @@ struct RsStftArgs {
   T* Rx;                    // [B][n_fft/2+1][n_hops]
   cx<T>* Vt;                // V^{tau g} store, or null
   RsPlanes<T> tp;           // target planes (RS_EPI_TGT)
-};
+  static constexpr int SEQ = 2;
+  template <int LOG_M> using Tile = RsTile<T, LOG_M>;
+  using Framing = RsStftArgs;
 
-// bit 0: store Sx; bit 1: write the target planes
-enum { RS_EPI_SX = 1, RS_EPI_TGT = 2 };
-
-template <typename T, int EPI>
-__device__ __forceinline__ void rs_stft_emit(const RsStftArgs<T>& P, int b, int k,
-                                             long long frame, cx<T> Ck, cx<T> Cmk, cx<T> Vt) {
-  const StftArgs<T>& A = P.A;
-  const T h = (T)0.5;
-  const cx<T> S  = mkc<T>((Ck.x + Cmk.x) * h, (Ck.y - Cmk.y) * h);
-  const cx<T> dS = mkc<T>((Ck.y + Cmk.y) * h * A.inv_kappa, (Cmk.x - Ck.x) * h * A.inv_kappa);
-  const int nrows = A.n_fft / 2 + 1;
-  const long long plane = (long long)b * nrows * A.n_hops;
-  const long long o = plane + (long long)k * A.n_hops + frame;
-  if (EPI & RS_EPI_SX) A.Sx[o] = S;
-  if (A.write_dSx) A.dSx[o] = dS;
-  if (P.Vt) P.Vt[o] = Vt;
-  rs_point<T, (EPI & RS_EPI_TGT) != 0>(FORM_STFT, S, dS, Vt, (double)A.Sfs[k], frame, A.hop,
-                                       A.n_hops, A.grid, P.Rx + plane, P.tp, o);
-}
-
-// frames per CTA of the power-of-two kernel: F frames, 2F transforms (F packed g / g', F tau g),
-// at least 8 NT elements per transform batch
-template <typename T, int LOG_M> struct RsTile {
-  static constexpr int M = 1 << LOG_M;
-  static constexpr int F = (Tile<T>::ELEMS / 2) / M > 0 ? (Tile<T>::ELEMS / 2) / M : 1;
-  static constexpr int R = 2 * F;
-  static constexpr size_t SMEM = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);
-};
-
-template <typename T, int LOG_M, int EPI>
-__global__ void __launch_bounds__(Tile<T>::NT)
-rs_stft_pow2_kernel(const RsStftArgs<T> P) {
-  constexpr int NT = Tile<T>::NT;
-  constexpr int M = 1 << LOG_M;
-  constexpr int F = RsTile<T, LOG_M>::F;
-  constexpr int R = RsTile<T, LOG_M>::R;
-  constexpr int STRIDE = R + 1;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  cx<T>* s = reinterpret_cast<cx<T>*>(smem_raw);          // [M][STRIDE]: c1 of F frames, tau g
-  cx<T>* tw = s + (size_t)M * STRIDE;                     // [M]
-  const StftArgs<T>& A = P.A;
-  const int tid = threadIdx.x;
-  const long long total_frames = (long long)A.B * A.n_hops;
-  const long long f0 = (long long)blockIdx.x * F;
-
-  for (int m = tid; m < M; m += NT) tw[m] = A.tw[m];
-#pragma unroll 1
-  for (int lin = tid; lin < M * F; lin += NT) {
-    const int r = lin % F, l = lin / F;
-    const long long fr = f0 + r;
-    T v = (T)0;
-    if (fr < total_frames) {
-      const int b = (int)(fr / A.n_hops);
-      const long long i = fr - (long long)b * A.n_hops;
-      const long long src = pad_src_index(frame_src(l, i, A.hop, M, A.modulated), A.n1, A.N, A.padtype);
-      v = (src >= 0) ? A.x[(long long)b * A.N + src] : (T)0;
-    }
-    // conjugated inputs: the forward DFT from the inverse engine
-    s[l * STRIDE + r]     = mkc<T>(v * A.win[l], -(v * A.dwin[l]) * A.kappa);
-    s[l * STRIDE + F + r] = mkc<T>(v * P.twin[l], (T)0);
+  template <bool CONJ>
+  __device__ __forceinline__ cx<T> pack(T v, int l, int j) const {
+    return j == 0 ? pack_pair<T, CONJ>(v, A.win[l], A.dwin[l], A.kappa) : mkc<T>(v * twin[l], (T)0);
   }
-  __syncthreads();
-  block_ifft<T, LOG_M, R, NT, STRIDE>(s, tw);
-#pragma unroll 1
-  for (int lin = tid; lin < (M / 2 + 1) * F; lin += NT) {
-    const int r = lin % F, k = lin / F;
-    const long long fr = f0 + r;
-    if (fr >= total_frames) continue;
-    const int b = (int)(fr / A.n_hops);
-    const long long i = fr - (long long)b * A.n_hops;
-    rs_stft_emit<T, EPI>(P, b, k, i, cconj<T>(s[k * STRIDE + r]),
-                         cconj<T>(s[((M - k) & (M - 1)) * STRIDE + r]),
-                         cconj<T>(s[k * STRIDE + F + r]));
-  }
-}
 
-// any other n_fft (and float64 at 4096): c[fl][l] is the packed g / g' sequence of frame f0 + fl
-// (stft_frames_kernel), c[nf + fl][l] its tau g sequence (this kernel)
-template <typename T>
-__global__ void __launch_bounds__(256)
-rs_tau_frames_kernel(const RsStftArgs<T> P, cx<T>* __restrict__ c, long long f0, long long nf) {
-  const StftArgs<T>& A = P.A;
-  const int M = A.n_fft;
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= nf * M) return;
-  const long long fl = idx / M; const int l = (int)(idx - fl * M);
-  const long long fr = f0 + fl;
-  const int b = (int)(fr / A.n_hops);
-  const long long i = fr - (long long)b * A.n_hops;
-  const long long src = pad_src_index(frame_src(l, i, A.hop, M, A.modulated), A.n1, A.N, A.padtype);
-  const T v = (src >= 0) ? A.x[(long long)b * A.N + src] : (T)0;
-  c[idx] = mkc<T>(v * P.twin[l], (T)0);
-}
-template <typename T, int EPI>
-__global__ void __launch_bounds__(256)
-rs_stft_emit_kernel(const RsStftArgs<T> P, const cx<T>* __restrict__ C, long long f0, long long nf) {
-  const int M = P.A.n_fft, nrows = M / 2 + 1;
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= nf * nrows) return;
-  const int k = (int)(idx / nf); const long long fl = idx - (long long)k * nf;   // frames fastest
-  const long long fr = f0 + fl;
-  const int b = (int)(fr / P.A.n_hops);
-  const long long i = fr - (long long)b * P.A.n_hops;
-  rs_stft_emit<T, EPI>(P, b, k, i, C[fl * M + k], C[fl * M + (k ? M - k : 0)],
-                       C[(nf + fl) * M + k]);
-}
+  template <int EPI, class Bins>
+  __device__ __forceinline__ void emit(int b, int k, long long frame, const Bins& C, int mk) const {
+    const cx<T> Ck = C(0, k), Cmk = C(0, mk), V = C(1, k);
+    cx<T> S, dS;
+    hermitian_split<T>(Ck, Cmk, A.inv_kappa, S, dS);
+    const int nrows = A.n_fft / 2 + 1;
+    const long long plane = (long long)b * nrows * A.n_hops;
+    const long long o = plane + (long long)k * A.n_hops + frame;
+    if (EPI & RS_EPI_SX) A.Sx[o] = S;
+    if (A.write_dSx) A.dSx[o] = dS;
+    if (Vt) Vt[o] = V;
+    rs_point<T, (EPI & RS_EPI_TGT) != 0>(FORM_STFT, S, dS, V, (double)A.Sfs[k], frame, A.hop,
+                                         A.n_hops, A.grid, Rx + plane, tp, o);
+  }
+};
 
 // ---- CWT: one thread per point of the [rows][ncols] planes W, dW, A (rows = B * na) -----------
 template <typename T, bool TGT>

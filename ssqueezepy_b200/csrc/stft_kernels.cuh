@@ -45,117 +45,207 @@ __device__ __forceinline__ long long frame_src(int l, long long i, int hop, int 
   return (l < s20) ? start + s21 + l : start + (l - s20);
 }
 
-// What the transform of a frame feeds: Sx (+ dSx), the same plus the fused reassignment
-// (ssq_stft), or the istft adjoint, which transforms one real sequence (no dSx half) and
-// writes gSx[k] = (c_k / n_fft) C[k]  (c_0 = c_{n_fft/2} = 1, otherwise 2).  STFT_EPI_SSQ_TX is
-// STFT_EPI_SSQ without the Sx store (the caller asked for Tx only).
-enum { STFT_EPI_PLAIN = 0, STFT_EPI_SSQ = 1, STFT_EPI_ISTFT_BWD = 2, STFT_EPI_SSQ_TX = 3 };
+// The padded, framed sample of frame fr of the flattened batch: x_b[pad_src_index(frame_src(l, i))],
+// or 0 where the frame reaches into zero padding
+template <typename T>
+__device__ __forceinline__ T frame_sample(const StftArgs<T>& A, int M, int l, long long fr) {
+  const int b = (int)(fr / A.n_hops);
+  const long long i = fr - (long long)b * A.n_hops;
+  const long long src = pad_src_index(frame_src(l, i, A.hop, M, A.modulated), A.n1, A.N, A.padtype);
+  return (src >= 0) ? A.x[(long long)b * A.N + src] : (T)0;
+}
 
-template <typename T, int EPI>
-__device__ __forceinline__ void stft_emit(const StftArgs<T>& A, int b, int k, long long frame,
-                                          cx<T> Ck, cx<T> Cmk) {
-  // C = FFT(c);  S = (C[k] + conj(C[M-k]))/2 ; kappa*dS = (C[k] - conj(C[M-k]))/(2i)
-  T h = (T)0.5;
-  cx<T> S  = mkc<T>((Ck.x + Cmk.x) * h, (Ck.y - Cmk.y) * h);
-  int nrows = A.n_fft / 2 + 1;
-  long long o = ((long long)b * nrows + k) * A.n_hops + frame;
-  if (EPI == STFT_EPI_ISTFT_BWD) {
+// v g + i kappa v g' packed for one transform.  The power-of-two tile stores it conjugated (CONJ):
+// the forward DFT from the inverse engine.
+template <typename T, bool CONJ>
+__device__ __forceinline__ cx<T> pack_pair(T v, T g, T dg, T kappa) {
+  return mkc<T>(v * g, CONJ ? -(v * dg) * kappa : (v * dg) * kappa);
+}
+
+// S and D / kappa of bin k from C = FFT(c) of c = f g + i kappa f g':
+// S = (C[k] + conj(C[M-k]))/2, kappa D = (C[k] - conj(C[M-k]))/(2i)
+template <typename T>
+__device__ __forceinline__ void hermitian_split(cx<T> Ck, cx<T> Cmk, T inv_kappa, cx<T>& S, cx<T>& D) {
+  const T h = (T)0.5;
+  S = mkc<T>((Ck.x + Cmk.x) * h, (Ck.y - Cmk.y) * h);
+  D = mkc<T>((Ck.y + Cmk.y) * h * inv_kappa, (Cmk.x - Ck.x) * h * inv_kappa);
+}
+
+// ---- routes ---------------------------------------------------------------------------------
+// A route is the argument struct of one STFT variant.  It holds the framing in A and gives the
+// framed-transform tile and the generic-length kernels below two things:
+//   pack<CONJ>(v, l, j)           packed sequence j (of SEQ) at frame sample l, sample value v
+//   emit<EPI>(b, k, frame, C, mk) the outputs of bin k of the frame, where C(j, k) is bin k of
+//                                 the transform of sequence j and mk is the bin M - k (0 at k = 0)
+// Tile<LOG_M> is its power-of-two tile: F frames per CTA, SMEM bytes.  Routes that frame like the
+// first order derive from Stft1Args; Framing is the route whose frame kernel they run.
+
+// the first order's tile: R = F = TILE / n_fft frames, one transform each
+template <typename T, int LOG_M> struct StftTile {
+  static constexpr int M = 1 << LOG_M;
+  static constexpr int F = Tile<T>::ELEMS / M;
+  static constexpr size_t SMEM = ((size_t)M * (F + 1) + M) * sizeof(cx<T>);
+};
+
+// stft and ssq_stft: c = f g + i kappa f g'.  PLAIN stores Sx (+ dSx), SSQ adds the fused
+// reassignment into Tx, SSQ_TX is SSQ without the Sx store (the caller asked for Tx only).
+enum { STFT_EPI_PLAIN = 0, STFT_EPI_SSQ = 1, STFT_EPI_SSQ_TX = 3 };
+
+template <typename T>
+struct Stft1Args {
+  StftArgs<T> A;
+  static constexpr int SEQ = 1;
+  template <int LOG_M> using Tile = StftTile<T, LOG_M>;
+  using Framing = Stft1Args;
+
+  template <bool CONJ>
+  __device__ __forceinline__ cx<T> pack(T v, int l, int) const {
+    return pack_pair<T, CONJ>(v, A.win[l], A.dwin[l], A.kappa);
+  }
+
+  template <int EPI, class Bins>
+  __device__ __forceinline__ void emit(int b, int k, long long frame, const Bins& C, int mk) const {
+    cx<T> S, dS;
+    hermitian_split<T>(C(0, k), C(0, mk), A.inv_kappa, S, dS);
+    const int nrows = A.n_fft / 2 + 1;
+    const long long o = ((long long)b * nrows + k) * A.n_hops + frame;
+    if (EPI != STFT_EPI_SSQ_TX) A.Sx[o] = S;
+    if (A.write_dSx) A.dSx[o] = dS;
+    if ((EPI == STFT_EPI_SSQ || EPI == STFT_EPI_SSQ_TX) && is_active_exact(S.x, S.y, A.grid.gamma)) {
+      double r = phase_ratio_exact<T>(dS.x, dS.y, S.x, S.y);
+      double w = fabs((double)A.Sfs[k] - r);
+      int kk = bin_from_w_exact(w, A.grid);
+      T cc = (T)A.cst[k];
+      atomic_add_cx<T>(&A.Tx[((long long)b * nrows + kk) * A.n_hops + frame], S.x * cc, S.y * cc);
+    }
+  }
+};
+
+// The istft adjoint: transforms one real sequence, c = f g, and writes gSx[k] = (c_k / n_fft) C[k]
+// (c_0 = c_{n_fft/2} = 1, otherwise 2).  The imaginary part is +0, not a negated zero.
+template <typename T>
+struct StftAdjArgs {
+  StftArgs<T> A;
+  static constexpr int SEQ = 1;
+  template <int LOG_M> using Tile = StftTile<T, LOG_M>;
+  using Framing = StftAdjArgs;
+
+  template <bool CONJ>
+  __device__ __forceinline__ cx<T> pack(T v, int l, int) const { return mkc<T>(v * A.win[l], (T)0); }
+
+  template <int EPI, class Bins>
+  __device__ __forceinline__ void emit(int b, int k, long long frame, const Bins& C, int mk) const {
+    const cx<T> Ck = C(0, k), Cmk = C(0, mk);
+    const T h = (T)0.5;
+    const cx<T> S = mkc<T>((Ck.x + Cmk.x) * h, (Ck.y - Cmk.y) * h);
+    const long long o = ((long long)b * (A.n_fft / 2 + 1) + k) * A.n_hops + frame;
     // irfft reads only the real part of the DC and Nyquist bins
     const bool edge = (k == 0 || 2 * k == A.n_fft);
     const T sc = (T)((edge ? 1.0 : 2.0) / (double)A.n_fft);
     A.Sx[o] = mkc<T>(S.x * sc, edge ? (T)0 : S.y * sc);
-    return;
   }
-  cx<T> dS = mkc<T>((Ck.y + Cmk.y) * h * A.inv_kappa, (Cmk.x - Ck.x) * h * A.inv_kappa);
-  if (EPI != STFT_EPI_SSQ_TX) A.Sx[o] = S;
-  if (A.write_dSx) A.dSx[o] = dS;
-  if ((EPI == STFT_EPI_SSQ || EPI == STFT_EPI_SSQ_TX) && is_active_exact(S.x, S.y, A.grid.gamma)) {
-    double r = phase_ratio_exact<T>(dS.x, dS.y, S.x, S.y);
-    double w = fabs((double)A.Sfs[k] - r);
-    int kk = bin_from_w_exact(w, A.grid);
-    T cc = (T)A.cst[k];
-    atomic_add_cx<T>(&A.Tx[((long long)b * nrows + kk) * A.n_hops + frame], S.x * cc, S.y * cc);
-  }
-}
+};
 
-// ---- power-of-two n_fft -------------------------------------------------------
-template <typename T, int LOG_M, int EPI>
-__global__ void __launch_bounds__(Tile<T>::NT)
-stft_pow2_kernel(const StftArgs<T> A) {
+// bin k of sequence j in the power-of-two tile (stored conjugated, frame r) and in the
+// generic route's transform (the SEQ sequences of one frame, consecutive)
+template <typename T, int F, int STRIDE>
+struct TileBins {
+  const cx<T>* s; int r;
+  __device__ __forceinline__ cx<T> operator()(int j, int k) const { return cconj<T>(s[k * STRIDE + j * F + r]); }
+};
+template <typename T>
+struct GfftBins {
+  const cx<T>* C; int M;
+  __device__ __forceinline__ cx<T> operator()(int j, int k) const { return C[j * M + k]; }
+};
+
+// ---- power-of-two n_fft: the framed-transform tile ---------------------------------------------
+// F frames per CTA from f0, the SEQ packed sequences of frame r at s[l][j F + r], transformed in
+// place: s[k][j F + r] = conj(FFT(c)[k]).
+template <typename T, class Route, int LOG_M, int F>
+__device__ __forceinline__ void frame_tile(const Route& P, cx<T>* s, cx<T>* tw, long long f0) {
   constexpr int NT = Tile<T>::NT;
   constexpr int M = 1 << LOG_M;
-  constexpr int R = Tile<T>::ELEMS / M;
+  constexpr int R = Route::SEQ * F;
   constexpr int STRIDE = R + 1;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  cx<T>* s = reinterpret_cast<cx<T>*>(smem_raw);          // [M][STRIDE]
-  cx<T>* tw = s + (size_t)M * STRIDE;                     // [M]
+  const StftArgs<T>& A = P.A;
   const int tid = threadIdx.x;
   const long long total_frames = (long long)A.B * A.n_hops;
-  const long long f0 = (long long)blockIdx.x * R;
-
   for (int m = tid; m < M; m += NT) tw[m] = A.tw[m];
 #pragma unroll 1
-  for (int lin = tid; lin < M * R; lin += NT) {
+  for (int lin = tid; lin < M * F; lin += NT) {
     // frames along r; each lane walks the frame samples l (stride hop between lanes)
-    int r = lin % R, l = lin / R;
-    long long fr = f0 + r;
-    cx<T> z = mkc<T>((T)0, (T)0);
-    if (fr < total_frames) {
-      int b = (int)(fr / A.n_hops);
-      long long i = fr - (long long)b * A.n_hops;
-      long long t = frame_src(l, i, A.hop, M, A.modulated);
-      long long src = pad_src_index(t, A.n1, A.N, A.padtype);
-      T v = (src >= 0) ? A.x[(long long)b * A.N + src] : (T)0;
-      z = mkc<T>(v * A.win[l],                                 // conj(c)
-                 EPI == STFT_EPI_ISTFT_BWD ? (T)0 : -(v * A.dwin[l]) * A.kappa);
+    const int r = lin % F, l = lin / F;
+    const long long fr = f0 + r;
+    // Frames past the batch are never read.  The single-sequence tiles store zeros there, the
+    // others pack v = 0: storing zeros in the two- and three-sequence tiles costs registers and
+    // halves the occupancy of some second-order instances.
+    if constexpr (Route::SEQ == 1) {
+      cx<T> z = mkc<T>((T)0, (T)0);
+      if (fr < total_frames) z = P.template pack<true>(frame_sample<T>(A, M, l, fr), l, 0);
+      s[l * STRIDE + r] = z;
+    } else {
+      T v = (T)0;
+      if (fr < total_frames) v = frame_sample<T>(A, M, l, fr);
+#pragma unroll
+      for (int j = 0; j < Route::SEQ; ++j) s[l * STRIDE + j * F + r] = P.template pack<true>(v, l, j);
     }
-    s[l * STRIDE + r] = z;
   }
   __syncthreads();
   block_ifft<T, LOG_M, R, NT, STRIDE>(s, tw);
-  // FFT(c)[k] = conj(s[k])
+}
+
+template <typename T, class Route, int LOG_M, int EPI>
+__global__ void __launch_bounds__(Tile<T>::NT)
+stft_tile_kernel(const Route P) {
+  constexpr int NT = Tile<T>::NT;
+  constexpr int M = 1 << LOG_M;
+  constexpr int F = Route::template Tile<LOG_M>::F;
+  constexpr int STRIDE = Route::SEQ * F + 1;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  cx<T>* s = reinterpret_cast<cx<T>*>(smem_raw);          // [M][STRIDE]
+  cx<T>* tw = s + (size_t)M * STRIDE;                     // [M]
+  const StftArgs<T>& A = P.A;
+  const int tid = threadIdx.x;
+  const long long total_frames = (long long)A.B * A.n_hops;
+  const long long f0 = (long long)blockIdx.x * F;
+  frame_tile<T, Route, LOG_M, F>(P, s, tw, f0);
 #pragma unroll 1
-  for (int lin = tid; lin < (M / 2 + 1) * R; lin += NT) {
-    int r = lin % R, k = lin / R;
-    long long fr = f0 + r;
+  for (int lin = tid; lin < (M / 2 + 1) * F; lin += NT) {
+    const int r = lin % F, k = lin / F;
+    const long long fr = f0 + r;
     if (fr >= total_frames) continue;
-    int b = (int)(fr / A.n_hops);
-    long long i = fr - (long long)b * A.n_hops;
-    cx<T> Ck = cconj<T>(s[k * STRIDE + r]);
-    cx<T> Cmk = cconj<T>(s[((M - k) & (M - 1)) * STRIDE + r]);
-    stft_emit<T, EPI>(A, b, k, i, Ck, Cmk);
+    const int b = (int)(fr / A.n_hops);
+    const long long i = fr - (long long)b * A.n_hops;
+    P.template emit<EPI>(b, k, i, TileBins<T, F, STRIDE>{s, r}, (M - k) & (M - 1));
   }
 }
 
-// ---- any other n_fft: frames -> generic-length FFT (gfft.cuh) -> Hermitian split ------------
-// c[f][l] = x_f[l] win[l] + i kappa x_f[l] dwin[l]   (frames f0 .. f0 + nf of the flattened batch)
-template <typename T, int EPI>
+// ---- any other n_fft: frames -> generic-length FFT (gfft.cuh) -> the route's epilogue ----------
+// c[SEQ fl + j][l] = packed sequence j of frame f0 + fl of the flattened batch
+template <typename T, class Route>
 __global__ void __launch_bounds__(256)
-stft_frames_kernel(const StftArgs<T> A, cx<T>* __restrict__ c, long long f0, long long nf) {
-  const int M = A.n_fft;
+stft_frames_kernel(const Route P, cx<T>* __restrict__ c, long long f0, long long nf) {
+  const int M = P.A.n_fft;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= nf * M) return;
   const long long fl = idx / M; const int l = (int)(idx - fl * M);
-  const long long fr = f0 + fl;
-  const int b = (int)(fr / A.n_hops);
-  const long long i = fr - (long long)b * A.n_hops;
-  const long long t = frame_src(l, i, A.hop, M, A.modulated);
-  const long long src = pad_src_index(t, A.n1, A.N, A.padtype);
-  const T v = (src >= 0) ? A.x[(long long)b * A.N + src] : (T)0;
-  c[idx] = mkc<T>(v * A.win[l], EPI == STFT_EPI_ISTFT_BWD ? (T)0 : (v * A.dwin[l]) * A.kappa);
+  const T v = frame_sample<T>(P.A, M, l, f0 + fl);
+  cx<T>* cf = c + idx + (Route::SEQ - 1) * fl * M;        // c[SEQ fl][l]
+#pragma unroll
+  for (int j = 0; j < Route::SEQ; ++j) cf[j * M] = P.template pack<false>(v, l, j);
 }
-template <typename T, int EPI>
+template <typename T, class Route, int EPI>
 __global__ void __launch_bounds__(256)
-stft_emit_kernel(const StftArgs<T> A, const cx<T>* __restrict__ C, long long f0, long long nf) {
-  const int M = A.n_fft, nrows = M / 2 + 1;
+stft_emit_kernel(const Route P, const cx<T>* __restrict__ C, long long f0, long long nf) {
+  const int M = P.A.n_fft, nrows = M / 2 + 1;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= nf * nrows) return;
   const int k = (int)(idx / nf); const long long fl = idx - (long long)k * nf;   // frames fastest
   const long long fr = f0 + fl;
-  const int b = (int)(fr / A.n_hops);
-  const long long i = fr - (long long)b * A.n_hops;
-  const cx<T> Ck = C[fl * M + k], Cmk = C[fl * M + (k ? M - k : 0)];
-  stft_emit<T, EPI>(A, b, k, i, Ck, Cmk);
+  const int b = (int)(fr / P.A.n_hops);
+  const long long i = fr - (long long)b * P.A.n_hops;
+  P.template emit<EPI>(b, k, i, GfftBins<T>{C + Route::SEQ * fl * M, M}, k ? M - k : 0);
 }
 
 // ---- stft backward (adjoint of x -> (Sx, dSx)) ------------------------------------------
@@ -314,17 +404,6 @@ stft_bwd_fold_kernel(const StftBwdArgs<T> A) {
 //   c1 = f g + i kappa  f g'       (the first-order packing)
 //   c2 = f tau g + i kappa2 f tau g'
 //   c3 = f g''                     (real; the spectrum is C3[k] itself)
-// The first-order kernels above are untouched; Stft2Args carries their arguments unchanged.
-template <typename T>
-struct Stft2Args {
-  StftArgs<T> A;            // framing, g / g' tables, kappa, Sx / dSx / Tx, Sfs, cst, grid
-  const T* ddwin;           // [n_fft] g'' * fs^2, ifftshifted like win
-  const T* twin;            // [n_fft] tau * g
-  const T* tdwin;           // [n_fft] tau * g' (g' already times fs)
-  T kappa2, inv_kappa2;     // power of two balancing ||tau g|| and ||tau g'||
-  T* w;                     // [B][n_fft/2+1][n_hops] (STFT2_EPI_W) or nullptr
-  T gamma_t;                // gamma in the data type: w = inf where |Sx| < gamma (phase_stft)
-};
 
 // SSQ2 stores Sx and scatters into Tx; SSQ2_TX does not store Sx; W writes the real w plane
 // (and Sx when A.Sx is set).  All three store dSx when A.write_dSx.
@@ -365,129 +444,62 @@ __device__ __forceinline__ double ssq2_w(double eta, cx<T> S, cx<T> dS, cx<T> S2
   return isfinite(re2) ? fabs(re2) : w1;
 }
 
-// spectra of frame `frame` at bin k from the three packed transforms -> outputs
-template <typename T, int EPI>
-__device__ __forceinline__ void stft2_emit(const Stft2Args<T>& P, int b, int k, long long frame,
-                                           cx<T> C1k, cx<T> C1mk, cx<T> C2k, cx<T> C2mk, cx<T> S2) {
-  const StftArgs<T>& A = P.A;
-  const T h = (T)0.5;
-  const cx<T> S   = mkc<T>((C1k.x + C1mk.x) * h, (C1k.y - C1mk.y) * h);
-  const cx<T> dS  = mkc<T>((C1k.y + C1mk.y) * h * A.inv_kappa, (C1mk.x - C1k.x) * h * A.inv_kappa);
-  const cx<T> St  = mkc<T>((C2k.x + C2mk.x) * h, (C2k.y - C2mk.y) * h);
-  const cx<T> Std = mkc<T>((C2k.y + C2mk.y) * h * P.inv_kappa2, (C2mk.x - C2k.x) * h * P.inv_kappa2);
-  const int nrows = A.n_fft / 2 + 1;
-  const long long o = ((long long)b * nrows + k) * A.n_hops + frame;
-  if (EPI == STFT2_EPI_SSQ || (EPI == STFT2_EPI_W && A.Sx)) A.Sx[o] = S;
-  if (A.write_dSx) A.dSx[o] = dS;
-  if (EPI == STFT2_EPI_W) {
-    double w = __longlong_as_double(0x7ff0000000000000ll);          // inf: below gamma
-    if (!is_below_exact(S.x, S.y, P.gamma_t)) {
-      const double w1 = fabs((double)A.Sfs[k] - phase_ratio_exact<T>(dS.x, dS.y, S.x, S.y));
-      w = ssq2_w<T>((double)A.Sfs[k], S, dS, S2, St, Std, w1);
-    }
-    P.w[o] = (T)w;
-    return;
-  }
-  if (is_active_exact(S.x, S.y, A.grid.gamma)) {
-    const double w1 = fabs((double)A.Sfs[k] - phase_ratio_exact<T>(dS.x, dS.y, S.x, S.y));
-    const double w = ssq2_w<T>((double)A.Sfs[k], S, dS, S2, St, Std, w1);
-    const int kk = bin_from_w_exact(w, A.grid);
-    const T cc = (T)A.cst[k];
-    atomic_add_cx<T>(&A.Tx[((long long)b * nrows + kk) * A.n_hops + frame], S.x * cc, S.y * cc);
-  }
-}
-
 // frames per CTA of the power-of-two kernel: three transforms per frame, and at least 8 NT
 // elements per transform batch so every Stockham stage divides over the threads
 template <typename T, int LOG_M> struct Stft2Tile {
   static constexpr int M = 1 << LOG_M;
   static constexpr int F = (Tile<T>::ELEMS / 2) / M > 0 ? (Tile<T>::ELEMS / 2) / M : 1;
-  static constexpr int R = 3 * F;
-  static constexpr size_t SMEM = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);
+  static constexpr size_t SMEM = ((size_t)M * (3 * F + 1) + M) * sizeof(cx<T>);
 };
 
-template <typename T, int LOG_M, int EPI>
-__global__ void __launch_bounds__(Tile<T>::NT)
-stft2_pow2_kernel(const Stft2Args<T> P) {
-  constexpr int NT = Tile<T>::NT;
-  constexpr int M = 1 << LOG_M;
-  constexpr int F = Stft2Tile<T, LOG_M>::F;
-  constexpr int R = Stft2Tile<T, LOG_M>::R;
-  constexpr int STRIDE = R + 1;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  cx<T>* s = reinterpret_cast<cx<T>*>(smem_raw);          // [M][STRIDE]: c1 of F frames, c2, c3
-  cx<T>* tw = s + (size_t)M * STRIDE;                     // [M]
-  const StftArgs<T>& A = P.A;
-  const int tid = threadIdx.x;
-  const long long total_frames = (long long)A.B * A.n_hops;
-  const long long f0 = (long long)blockIdx.x * F;
-
-  for (int m = tid; m < M; m += NT) tw[m] = A.tw[m];
-#pragma unroll 1
-  for (int lin = tid; lin < M * F; lin += NT) {
-    const int r = lin % F, l = lin / F;
-    const long long fr = f0 + r;
-    T v = (T)0;
-    if (fr < total_frames) {
-      const int b = (int)(fr / A.n_hops);
-      const long long i = fr - (long long)b * A.n_hops;
-      const long long src = pad_src_index(frame_src(l, i, A.hop, M, A.modulated), A.n1, A.N, A.padtype);
-      v = (src >= 0) ? A.x[(long long)b * A.N + src] : (T)0;
-    }
-    // conjugated inputs: the forward DFT from the inverse engine
-    s[l * STRIDE + r]         = mkc<T>(v * A.win[l], -(v * A.dwin[l]) * A.kappa);
-    s[l * STRIDE + F + r]     = mkc<T>(v * P.twin[l], -(v * P.tdwin[l]) * P.kappa2);
-    s[l * STRIDE + 2 * F + r] = mkc<T>(v * P.ddwin[l], (T)0);
-  }
-  __syncthreads();
-  block_ifft<T, LOG_M, R, NT, STRIDE>(s, tw);
-#pragma unroll 1
-  for (int lin = tid; lin < (M / 2 + 1) * F; lin += NT) {
-    const int r = lin % F, k = lin / F;
-    const long long fr = f0 + r;
-    if (fr >= total_frames) continue;
-    const int b = (int)(fr / A.n_hops);
-    const long long i = fr - (long long)b * A.n_hops;
-    const int mk = (M - k) & (M - 1);
-    stft2_emit<T, EPI>(P, b, k, i,
-                       cconj<T>(s[k * STRIDE + r]), cconj<T>(s[mk * STRIDE + r]),
-                       cconj<T>(s[k * STRIDE + F + r]), cconj<T>(s[mk * STRIDE + F + r]),
-                       cconj<T>(s[k * STRIDE + 2 * F + r]));
-  }
-}
-
-// any other n_fft (and float64 at 4096): c[3 fl + j][l] = packed sequence j of frame f0 + fl
 template <typename T>
-__global__ void __launch_bounds__(256)
-stft2_frames_kernel(const Stft2Args<T> P, cx<T>* __restrict__ c, long long f0, long long nf) {
-  const StftArgs<T>& A = P.A;
-  const int M = A.n_fft;
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= nf * M) return;
-  const long long fl = idx / M; const int l = (int)(idx - fl * M);
-  const long long fr = f0 + fl;
-  const int b = (int)(fr / A.n_hops);
-  const long long i = fr - (long long)b * A.n_hops;
-  const long long src = pad_src_index(frame_src(l, i, A.hop, M, A.modulated), A.n1, A.N, A.padtype);
-  const T v = (src >= 0) ? A.x[(long long)b * A.N + src] : (T)0;
-  cx<T>* cf = c + 3 * fl * M;
-  cf[l]         = mkc<T>(v * A.win[l], (v * A.dwin[l]) * A.kappa);
-  cf[M + l]     = mkc<T>(v * P.twin[l], (v * P.tdwin[l]) * P.kappa2);
-  cf[2 * M + l] = mkc<T>(v * P.ddwin[l], (T)0);
-}
-template <typename T, int EPI>
-__global__ void __launch_bounds__(256)
-stft2_emit_kernel(const Stft2Args<T> P, const cx<T>* __restrict__ C, long long f0, long long nf) {
-  const int M = P.A.n_fft, nrows = M / 2 + 1;
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= nf * nrows) return;
-  const int k = (int)(idx / nf); const long long fl = idx - (long long)k * nf;   // frames fastest
-  const long long fr = f0 + fl;
-  const int b = (int)(fr / P.A.n_hops);
-  const long long i = fr - (long long)b * P.A.n_hops;
-  const cx<T>* Cf = C + 3 * fl * M;
-  const int mk = k ? M - k : 0;
-  stft2_emit<T, EPI>(P, b, k, i, Cf[k], Cf[mk], Cf[M + k], Cf[M + mk], Cf[2 * M + k]);
-}
+struct Stft2Args {
+  StftArgs<T> A;            // framing, g / g' tables, kappa, Sx / dSx / Tx, Sfs, cst, grid
+  const T* ddwin;           // [n_fft] g'' * fs^2, ifftshifted like win
+  const T* twin;            // [n_fft] tau * g
+  const T* tdwin;           // [n_fft] tau * g' (g' already times fs)
+  T kappa2, inv_kappa2;     // power of two balancing ||tau g|| and ||tau g'||
+  T* w;                     // [B][n_fft/2+1][n_hops] (STFT2_EPI_W) or nullptr
+  T gamma_t;                // gamma in the data type: w = inf where |Sx| < gamma (phase_stft)
+  static constexpr int SEQ = 3;
+  template <int LOG_M> using Tile = Stft2Tile<T, LOG_M>;
+  using Framing = Stft2Args;
+
+  template <bool CONJ>
+  __device__ __forceinline__ cx<T> pack(T v, int l, int j) const {
+    if (j == 0) return pack_pair<T, CONJ>(v, A.win[l], A.dwin[l], A.kappa);
+    if (j == 1) return pack_pair<T, CONJ>(v, twin[l], tdwin[l], kappa2);
+    return mkc<T>(v * ddwin[l], (T)0);
+  }
+
+  // the five spectra of bin k from the three transforms -> outputs
+  template <int EPI, class Bins>
+  __device__ __forceinline__ void emit(int b, int k, long long frame, const Bins& C, int mk) const {
+    const cx<T> C1k = C(0, k), C1mk = C(0, mk), C2k = C(1, k), C2mk = C(1, mk), S2 = C(2, k);
+    cx<T> S, dS, St, Std;
+    hermitian_split<T>(C1k, C1mk, A.inv_kappa, S, dS);
+    hermitian_split<T>(C2k, C2mk, inv_kappa2, St, Std);
+    const int nrows = A.n_fft / 2 + 1;
+    const long long o = ((long long)b * nrows + k) * A.n_hops + frame;
+    if (EPI == STFT2_EPI_SSQ || (EPI == STFT2_EPI_W && A.Sx)) A.Sx[o] = S;
+    if (A.write_dSx) A.dSx[o] = dS;
+    if (EPI == STFT2_EPI_W) {
+      double w = __longlong_as_double(0x7ff0000000000000ll);          // inf: below gamma
+      if (!is_below_exact(S.x, S.y, gamma_t)) {
+        const double w1 = fabs((double)A.Sfs[k] - phase_ratio_exact<T>(dS.x, dS.y, S.x, S.y));
+        w = ssq2_w<T>((double)A.Sfs[k], S, dS, S2, St, Std, w1);
+      }
+      this->w[o] = (T)w;
+      return;
+    }
+    if (is_active_exact(S.x, S.y, A.grid.gamma)) {
+      const double w1 = fabs((double)A.Sfs[k] - phase_ratio_exact<T>(dS.x, dS.y, S.x, S.y));
+      const double w = ssq2_w<T>((double)A.Sfs[k], S, dS, S2, St, Std, w1);
+      const int kk = bin_from_w_exact(w, A.grid);
+      const T cc = (T)A.cst[k];
+      atomic_add_cx<T>(&A.Tx[((long long)b * nrows + kk) * A.n_hops + frame], S.x * cc, S.y * cc);
+    }
+  }
+};
 
 }  // namespace ssqb

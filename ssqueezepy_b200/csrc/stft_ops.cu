@@ -45,20 +45,6 @@ int table_blob(const std::vector<unsigned char>& h, cudaStream_t st, unsigned ch
   return 0;
 }
 
-template <typename T, int EPI>
-static int launch_stft_pow2(const StftArgs<T>& A, cudaStream_t st) {
-  const long long total = (long long)A.B * A.n_hops;
-  return dispatch_log2<1, 12>(ilog2_exact(A.n_fft), [&](auto L) {
-    constexpr int M = 1 << L; constexpr int R = Tile<T>::ELEMS / M;
-    const size_t smem = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);
-    auto kern = stft_pow2_kernel<T, L, EPI>;
-    SSQB_CUDA(opt_in_smem(kern, smem));
-    kern<<<(unsigned)((total + R - 1) / R), Tile<T>::NT, smem, st>>>(A);
-    SSQB_LAUNCH_CHECK();
-    return 0;
-  });
-}
-
 // n_fft that is not a power of two (e.g. 598 = 2 * 13 * 23, the reference's own benchmark
 // size): frames -> batched mixed-radix / Bluestein FFT -> Hermitian split + epilogue.
 template <typename T> struct StftGeneric {
@@ -98,25 +84,86 @@ static int generic_frames(int n_fft, long long total, int seqs, int sign, Pre pr
   return 0;
 }
 
-template <typename T, int EPI>
-static int launch_stft_generic(const StftArgs<T>& A, cudaStream_t st) {
-  const long long M = A.n_fft, nrows = M / 2 + 1;
-  return generic_frames<T>(A.n_fft, (long long)A.B * A.n_hops, 1, -1,
+static constexpr size_t kMaxBlockSmem = 227u << 10;    // sm_90 opt-in limit per block
+
+// Does the power-of-two tile of Route (Route::Tile<L>: its shared memory, SMEM bytes, and its F
+// frames per CTA) fit one CTA at n_fft = 2^logm?
+template <class Route>
+static bool pow2_tile_fits(int logm) {
+  return logm >= 1 && logm <= 12 && dispatch_log2<1, 12>(logm, [](auto L) {
+    return Route::template Tile<L>::SMEM <= kMaxBlockSmem ? 1 : 0;
+  });
+}
+
+// One launch of kernel_of(L), the route's instance for n_fft = 2^logm, over the route's frames
+// (A.B * A.n_hops) in tiles of F.  Only instances whose tile fits are instantiated.
+template <typename T, class Route, typename KernelOf>
+static int launch_pow2_tile(const Route& P, int logm, KernelOf kernel_of, cudaStream_t st) {
+  return dispatch_log2<1, 12>(logm, [&](auto L) {
+    using Tl = typename Route::template Tile<L>;
+    if constexpr (Tl::SMEM > kMaxBlockSmem) {
+      return set_error(SSQB_E_UNSUPP, "n_fft = 2^%d does not fit one CTA", (int)L);
+    } else {
+      const long long total = (long long)P.A.B * P.A.n_hops;
+      auto kern = kernel_of(L);
+      SSQB_CUDA(opt_in_smem(kern, Tl::SMEM));
+      kern<<<(unsigned)((total + Tl::F - 1) / Tl::F), Tile<T>::NT, Tl::SMEM, st>>>(P);
+      SSQB_LAUNCH_CHECK();
+      return 0;
+    }
+  });
+}
+
+// Every forward STFT route (stft_kernels.cuh): one launch of the power-of-two tile when it fits
+// one CTA (the first order, tssq, SET / TET and the istft adjoint up to n_fft = 4096 in both
+// dtypes; the second order and rs up to 4096 in float32, 2048 in float64), otherwise the
+// route's packed frames -> one batched Gfft of SEQ transforms per frame -> its epilogue.  The
+// MSST walks its chains in two passes over the tile's bins: its own tile kernel, and one CTA per
+// frame with the frame's bins in shared memory on the generic route.
+template <typename T, class Route, int EPI>
+static int launch_route(const Route& P, cudaStream_t st) {
+  constexpr bool mssq = std::is_same<Route, MssqStftArgs<T>>::value;
+  const int logm = ilog2_exact(P.A.n_fft);
+  if (pow2_tile_fits<Route>(logm))
+    return launch_pow2_tile<T>(P, logm, [](auto L) {
+      if constexpr (mssq) return mssq_stft_pow2_kernel<T, L, EPI>;
+      else return stft_tile_kernel<T, Route, L, EPI>;
+    }, st);
+  const long long M = P.A.n_fft, nrows = M / 2 + 1;
+  const size_t smem = mssq ? sizeof(short) * (size_t)nrows : 0;
+  if constexpr (mssq) {
+    if (smem > kMaxBlockSmem) return set_error(SSQB_E_UNSUPP, "n_fft = %d: the bins of a frame do not fit one CTA", P.A.n_fft);
+    SSQB_CUDA(opt_in_smem(mssq_stft_emit_kernel<T, EPI>, smem));
+  }
+  return generic_frames<T>(P.A.n_fft, (long long)P.A.B * P.A.n_hops, Route::SEQ, -1,
       [&](cx<T>* c, long long f0, long long nf) {
-        stft_frames_kernel<T, EPI><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(A, c, f0, nf);
+        using Framing = typename Route::Framing;      // the route whose packing P uses
+        stft_frames_kernel<T, Framing><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(
+            static_cast<const Framing&>(P), c, f0, nf);
         SSQB_LAUNCH_CHECK();
         return 0;
       },
       [&](const cx<T>* C, long long f0, long long nf) {
-        stft_emit_kernel<T, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(A, C, f0, nf);
+        if constexpr (mssq) mssq_stft_emit_kernel<T, EPI><<<(unsigned)nf, 256, smem, st>>>(P, C, f0);
+        else stft_emit_kernel<T, Route, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(P, C, f0, nf);
         SSQB_LAUNCH_CHECK();
         return 0;
       }, st);
 }
 
-template <typename T, int EPI>
-static int launch_stft(const StftArgs<T>& A, cudaStream_t st) {
-  return stft_pow2_tile(A.n_fft) ? launch_stft_pow2<T, EPI>(A, st) : launch_stft_generic<T, EPI>(A, st);
+// launch(E) with the epilogue E = (store Sx ? SX : 0) | (write the target planes ? TGT : 0)
+template <int SX, int TGT, typename Launch>
+static int dispatch_sx_tgt(bool sx, bool tgt, Launch launch) {
+  if (sx) return tgt ? launch(std::integral_constant<int, SX | TGT>{}) : launch(std::integral_constant<int, SX>{});
+  return tgt ? launch(std::integral_constant<int, TGT>{}) : launch(std::integral_constant<int, 0>{});
+}
+
+// The shape check every STFT entry with an ssqb_stft_desc makes after its own checks (the forward
+// routes and the stft backward), then run(T()) in the descriptor's dtype
+template <typename Run>
+static int stft_dispatch(const ssqb_stft_desc* d, long long B, Run run) {
+  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
+  return d->dtype == SSQB_F32 ? run(float()) : run(double());
 }
 
 // kappa = power of two that balances ||win|| and ||dwin||
@@ -178,8 +225,9 @@ template <typename T>
 static int stft_t(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const void* x,
                   long long B, void* Sx, void* Tx, void* dSx, bool ssq, cudaStream_t st) {
   const int nrows = d->n_fft / 2 + 1;
-  StftArgs<T> A;
-  memset(&A, 0, sizeof(A));
+  Stft1Args<T> P;
+  memset(&P, 0, sizeof(P));
+  StftArgs<T>& A = P.A;
   stft_args(A, d, x, B, Sx, dSx, Tx, d->win_host, d->dwin_host);
   int rc = stft_tables(A, d, d->dwin_host, ssq ? r->cst_host : nullptr, true, st);
   if (rc) return rc;
@@ -187,8 +235,9 @@ static int stft_t(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const vo
     rc = fill_form_grid(r, nrows, FORM_STFT, &A.grid); if (rc) return rc;
     SSQB_CUDA(cudaMemsetAsync(Tx, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(cx<T>), st));
   }
-  if (ssq && !Sx) return launch_stft<T, STFT_EPI_SSQ_TX>(A, st);      // Tx only
-  return ssq ? launch_stft<T, STFT_EPI_SSQ>(A, st) : launch_stft<T, STFT_EPI_PLAIN>(A, st);
+  if (ssq && !Sx) return launch_route<T, Stft1Args<T>, STFT_EPI_SSQ_TX>(P, st);      // Tx only
+  return ssq ? launch_route<T, Stft1Args<T>, STFT_EPI_SSQ>(P, st)
+             : launch_route<T, Stft1Args<T>, STFT_EPI_PLAIN>(P, st);
 }
 
 int run_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const void* x, long long B,
@@ -196,9 +245,9 @@ int run_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const void* x
   if (!d || !x || (!Sx && !ssq)) return set_error(SSQB_E_ARG, "null pointer");   // ssq: Sx may be NULL
   if (!d->win_host || !d->dwin_host || !d->Sfs_host) return set_error(SSQB_E_ARG, "null table");
   if (ssq && (!r || !r->cst_host || !Tx)) return set_error(SSQB_E_ARG, "ssq needs Tx + reassign");
-  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
-  return d->dtype == SSQB_F32 ? stft_t<float>(d, r, x, B, Sx, Tx, dSx, ssq, st)
-                              : stft_t<double>(d, r, x, B, Sx, Tx, dSx, ssq, st);
+  return stft_dispatch(d, B, [&](auto t) {
+    return stft_t<decltype(t)>(d, r, x, B, Sx, Tx, dSx, ssq, st);
+  });
 }
 
 // ---- backward passes (torch.autograd) --------------------------------------------------------
@@ -283,14 +332,12 @@ int run_stft_backward(const ssqb_stft_desc* d, const void* gSx, const void* gdSx
                       void* gx, cudaStream_t st) {
   if (!d || !gx || (!gSx && !gdSx)) return set_error(SSQB_E_ARG, "null pointer");
   if (!d->win_host || !d->dwin_host) return set_error(SSQB_E_ARG, "null table");
-  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
-  return d->dtype == SSQB_F32 ? stft_bwd_t<float>(d, gSx, gdSx, B, gx, st)
-                              : stft_bwd_t<double>(d, gSx, gdSx, B, gx, st);
+  return stft_dispatch(d, B, [&](auto t) { return stft_bwd_t<decltype(t)>(d, gSx, gdSx, B, gx, st); });
 }
 
 // istft backward: gp = gx / wn (istft_bwd_norm_kernel), then the stft framing and transform of
 // gp -- zero padding by n_fft/2, window = window**win_exp, ifftshifted when modulated -- with
-// the STFT_EPI_ISTFT_BWD epilogue, which writes (c_k / n_fft) C[k] into gSx.
+// the adjoint route (StftAdjArgs), which writes (c_k / n_fft) C[k] into gSx.
 template <typename T>
 static int istft_bwd_t(const ssqb_istft_desc* d, const void* gx, long long B, void* gS,
                        cudaStream_t st) {
@@ -318,14 +365,15 @@ static int istft_bwd_t(const ssqb_istft_desc* d, const void* gx, long long B, vo
   SSQB_CUDA(cudaMallocAsync((void**)&gp, sizeof(T) * (size_t)B * (size_t)d->N, st));
   istft_bwd_norm_kernel<T><<<(unsigned)((d->N + 255) / 256), 256, 0, st>>>(I, (const T*)gx, gp);
   SSQB_LAUNCH_CHECK();
-  StftArgs<T> A;
-  memset(&A, 0, sizeof(A));
+  StftAdjArgs<T> P;
+  memset(&P, 0, sizeof(P));
+  StftArgs<T>& A = P.A;
   A.N = d->N; A.n_hops = d->n_hops; A.n_fft = M; A.hop = d->hop;
   A.n1 = M / 2; A.padtype = SSQB_PAD_ZERO; A.modulated = d->modulated; A.B = (int)B;
   A.x = gp; A.win = (const T*)(blob + o_win); A.dwin = nullptr;
   A.kappa = (T)1; A.inv_kappa = (T)1;
   A.Sx = (cx<T>*)gS; A.tw = (const cx<T>*)(blob + o_tw);
-  rc = launch_stft<T, STFT_EPI_ISTFT_BWD>(A, st);
+  rc = launch_route<T, StftAdjArgs<T>, 0>(P, st);
   cudaFreeAsync(gp, st);
   return rc;
 }
@@ -342,69 +390,6 @@ int run_istft_backward(const ssqb_istft_desc* d, const void* gx, long long B, vo
 }
 
 // ---- second-order ssq_stft -------------------------------------------------------------------
-// Power-of-two n_fft whose three transforms per frame fit one CTA's shared memory: one launch of
-// stft2_pow2_kernel (float32 up to 4096, float64 up to 2048).  Every other n_fft: frames -> one
-// batched Gfft of 3 transforms per frame -> emit, in chunks that keep each buffer at ~128 MB.
-static constexpr size_t kMaxBlockSmem = 227u << 10;    // sm_90 opt-in limit per block
-
-// The power-of-two tile routes whose tile does not fit one CTA at every n_fft (second order,
-// reassignment, MSST): TL<T, L> has the tile's shared memory, SMEM bytes, and its F frames per CTA.
-template <typename T, template <typename, int> class TL>
-static bool pow2_tile_fits(int logm) {
-  return logm >= 1 && logm <= 12 &&
-         dispatch_log2<1, 12>(logm, [](auto L) { return TL<T, L>::SMEM <= kMaxBlockSmem ? 1 : 0; });
-}
-
-// One launch of kernel_of(L), the route's instance for n_fft = 2^logm, over the route's frames
-// (A.B * A.n_hops) in tiles of TL<T, L>::F.  Only instances whose tile fits are instantiated.
-template <typename T, template <typename, int> class TL, typename P, typename KernelOf>
-static int launch_pow2_tile(const P& args, int logm, KernelOf kernel_of, cudaStream_t st) {
-  return dispatch_log2<1, 12>(logm, [&](auto L) {
-    using Tl = TL<T, L>;
-    if constexpr (Tl::SMEM > kMaxBlockSmem) {
-      return set_error(SSQB_E_UNSUPP, "n_fft = 2^%d does not fit one CTA", (int)L);
-    } else {
-      const long long total = (long long)args.A.B * args.A.n_hops;
-      auto kern = kernel_of(L);
-      SSQB_CUDA(opt_in_smem(kern, Tl::SMEM));
-      kern<<<(unsigned)((total + Tl::F - 1) / Tl::F), Tile<T>::NT, Tl::SMEM, st>>>(args);
-      SSQB_LAUNCH_CHECK();
-      return 0;
-    }
-  });
-}
-
-// launch(E) with the epilogue E = (store Sx ? SX : 0) | (write the target planes ? TGT : 0)
-template <int SX, int TGT, typename Launch>
-static int dispatch_sx_tgt(bool sx, bool tgt, Launch launch) {
-  if (sx) return tgt ? launch(std::integral_constant<int, SX | TGT>{}) : launch(std::integral_constant<int, SX>{});
-  return tgt ? launch(std::integral_constant<int, TGT>{}) : launch(std::integral_constant<int, 0>{});
-}
-
-template <typename T, int EPI>
-static int launch_stft2_generic(const Stft2Args<T>& P, cudaStream_t st) {
-  const long long M = P.A.n_fft, nrows = M / 2 + 1;
-  return generic_frames<T>(P.A.n_fft, (long long)P.A.B * P.A.n_hops, 3, -1,
-      [&](cx<T>* c, long long f0, long long nf) {
-        stft2_frames_kernel<T><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(P, c, f0, nf);
-        SSQB_LAUNCH_CHECK();
-        return 0;
-      },
-      [&](const cx<T>* C, long long f0, long long nf) {
-        stft2_emit_kernel<T, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(P, C, f0, nf);
-        SSQB_LAUNCH_CHECK();
-        return 0;
-      }, st);
-}
-
-template <typename T, int EPI>
-static int launch_stft2(const Stft2Args<T>& P, cudaStream_t st) {
-  const int logm = ilog2_exact(P.A.n_fft);
-  if (pow2_tile_fits<T, Stft2Tile>(logm))
-    return launch_pow2_tile<T, Stft2Tile>(P, logm, [](auto L) { return stft2_pow2_kernel<T, L, EPI>; }, st);
-  return launch_stft2_generic<T, EPI>(P, st);
-}
-
 template <typename T>
 static int stft2_t(const ssqb_stft_desc* d, const ssqb_stft2_tables* t2, const ssqb_reassign_desc* r,
                    const void* x, long long B, void* Sx, void* Tx, void* dSx, void* w,
@@ -423,10 +408,11 @@ static int stft2_t(const ssqb_stft_desc* d, const ssqb_stft2_tables* t2, const s
                        {t2->ddwin_host, t2->twin_host, t2->tdwin_host}, extra);
   if (rc) return rc;
   P.ddwin = extra[0]; P.twin = extra[1]; P.tdwin = extra[2];
-  if (!Tx) return launch_stft2<T, STFT2_EPI_W>(P, st);
+  if (!Tx) return launch_route<T, Stft2Args<T>, STFT2_EPI_W>(P, st);
   rc = fill_form_grid(r, nrows, FORM_STFT, &A.grid); if (rc) return rc;
   SSQB_CUDA(cudaMemsetAsync(Tx, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(cx<T>), st));
-  return Sx ? launch_stft2<T, STFT2_EPI_SSQ>(P, st) : launch_stft2<T, STFT2_EPI_SSQ_TX>(P, st);
+  return Sx ? launch_route<T, Stft2Args<T>, STFT2_EPI_SSQ>(P, st)
+            : launch_route<T, Stft2Args<T>, STFT2_EPI_SSQ_TX>(P, st);
 }
 
 int run_stft2(const ssqb_stft_desc* d, const ssqb_stft2_tables* t2, const ssqb_reassign_desc* r,
@@ -437,43 +423,12 @@ int run_stft2(const ssqb_stft_desc* d, const ssqb_stft2_tables* t2, const ssqb_r
     return set_error(SSQB_E_ARG, "null table");
   if (!Tx == !w) return set_error(SSQB_E_ARG, "exactly one of Tx and w must be given");
   if (!d->modulated) return set_error(SSQB_E_UNSUPP, "second-order ssq_stft needs modulated frames");
-  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
-  return d->dtype == SSQB_F32 ? stft2_t<float>(d, t2, r, x, B, Sx, Tx, dSx, w, st)
-                              : stft2_t<double>(d, t2, r, x, B, Sx, Tx, dSx, w, st);
+  return stft_dispatch(d, B, [&](auto t) {
+    return stft2_t<decltype(t)>(d, t2, r, x, B, Sx, Tx, dSx, w, st);
+  });
 }
 
 // ---- time-reassigned ssq_stft (tssq_kernels.cuh) ---------------------------------------------
-// The first order's routes with tau g in place of g': tssq_stft_pow2_kernel for n_fft = 2 .. 4096,
-// otherwise stft_frames_kernel -> Gfft -> tssq_stft_emit_kernel in generic_frames' chunks.
-template <typename T, int EPI>
-static int launch_tssq_stft(const TssqStftArgs<T>& P, cudaStream_t st) {
-  const StftArgs<T>& A = P.A;
-  const long long total = (long long)A.B * A.n_hops;
-  if (stft_pow2_tile(A.n_fft)) {
-    return dispatch_log2<1, 12>(ilog2_exact(A.n_fft), [&](auto L) {
-      constexpr int M = 1 << L; constexpr int R = Tile<T>::ELEMS / M;
-      const size_t smem = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);
-      auto kern = tssq_stft_pow2_kernel<T, L, EPI>;
-      SSQB_CUDA(opt_in_smem(kern, smem));
-      kern<<<(unsigned)((total + R - 1) / R), Tile<T>::NT, smem, st>>>(P);
-      SSQB_LAUNCH_CHECK();
-      return 0;
-    });
-  }
-  const long long M = A.n_fft, nrows = M / 2 + 1;
-  return generic_frames<T>(A.n_fft, total, 1, -1,
-      [&](cx<T>* c, long long f0, long long nf) {
-        stft_frames_kernel<T, STFT_EPI_PLAIN><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(A, c, f0, nf);
-        SSQB_LAUNCH_CHECK();
-        return 0;
-      },
-      [&](const cx<T>* C, long long f0, long long nf) {
-        tssq_stft_emit_kernel<T, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(P, C, f0, nf);
-        SSQB_LAUNCH_CHECK();
-        return 0;
-      }, st);
-}
-
 template <typename T>
 static int tssq_stft_t(const ssqb_stft_desc* d, const void* twin_host, double gamma, const void* x,
                        long long B, void* Sx, void* Ts, void* Vt, int* tgt, void* tau,
@@ -488,7 +443,7 @@ static int tssq_stft_t(const ssqb_stft_desc* d, const void* twin_host, double ga
   int rc = stft_tables(A, d, twin_host, nullptr, false, st); if (rc) return rc;
   SSQB_CUDA(cudaMemsetAsync(Ts, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(cx<T>), st));
   return dispatch_sx_tgt<TSSQ_EPI_SX, TSSQ_EPI_TGT>(Sx, tgt, [&](auto E) {
-    return launch_tssq_stft<T, E>(P, st);
+    return launch_route<T, TssqStftArgs<T>, E>(P, st);
   });
 }
 
@@ -498,39 +453,12 @@ int run_tssq_stft(const ssqb_stft_desc* d, const void* twin_host, double gamma, 
   if (!d->win_host || !twin_host) return set_error(SSQB_E_ARG, "null table");
   if (tau && !tgt) return set_error(SSQB_E_ARG, "tau needs the target plane");
   if (!(gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
-  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
-  return d->dtype == SSQB_F32 ? tssq_stft_t<float>(d, twin_host, gamma, x, B, Sx, Ts, Vt, tgt, tau, st)
-                              : tssq_stft_t<double>(d, twin_host, gamma, x, B, Sx, Ts, Vt, tgt, tau, st);
+  return stft_dispatch(d, B, [&](auto t) {
+    return tssq_stft_t<decltype(t)>(d, twin_host, gamma, x, B, Sx, Ts, Vt, tgt, tau, st);
+  });
 }
 
 // ---- reassigned spectrogram (rs_kernels.cuh) -------------------------------------------------
-// Power-of-two n_fft whose 2F transforms per tile fit one CTA (float32 up to 4096, float64 up to
-// 2048): rs_stft_pow2_kernel.  Every other n_fft: stft_frames_kernel (the g / g' sequences) and
-// rs_tau_frames_kernel (tau g) -> one batched Gfft of 2 transforms per frame -> the emit kernel.
-template <typename T, int EPI>
-static int launch_rs_stft(const RsStftArgs<T>& P, cudaStream_t st) {
-  const StftArgs<T>& A = P.A;
-  const long long total = (long long)A.B * A.n_hops;
-  const int logm = ilog2_exact(A.n_fft);
-  if (pow2_tile_fits<T, RsTile>(logm))
-    return launch_pow2_tile<T, RsTile>(P, logm, [](auto L) { return rs_stft_pow2_kernel<T, L, EPI>; }, st);
-  const long long M = A.n_fft, nrows = M / 2 + 1;
-  return generic_frames<T>(A.n_fft, total, 2, -1,
-      [&](cx<T>* c, long long f0, long long nf) {
-        const unsigned nb = (unsigned)((nf * M + 255) / 256);
-        stft_frames_kernel<T, STFT_EPI_PLAIN><<<nb, 256, 0, st>>>(A, c, f0, nf);
-        SSQB_LAUNCH_CHECK();
-        rs_tau_frames_kernel<T><<<nb, 256, 0, st>>>(P, c + nf * M, f0, nf);
-        SSQB_LAUNCH_CHECK();
-        return 0;
-      },
-      [&](const cx<T>* C, long long f0, long long nf) {
-        rs_stft_emit_kernel<T, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(P, C, f0, nf);
-        SSQB_LAUNCH_CHECK();
-        return 0;
-      }, st);
-}
-
 template <typename T>
 static int rs_stft_t(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reassign_desc* r,
                      double gamma, const void* x, long long B, void* Sx, void* Rx, void* dSx,
@@ -548,7 +476,7 @@ static int rs_stft_t(const ssqb_stft_desc* d, const void* twin_host, const ssqb_
   A.grid.gamma = gamma;
   SSQB_CUDA(cudaMemsetAsync(Rx, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(T), st));
   return dispatch_sx_tgt<RS_EPI_SX, RS_EPI_TGT>(Sx, jt, [&](auto E) {
-    return launch_rs_stft<T, E>(P, st);
+    return launch_route<T, RsStftArgs<T>, E>(P, st);
   });
 }
 
@@ -561,40 +489,12 @@ int run_rs_stft(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reass
   if (!kk != !jt) return set_error(SSQB_E_ARG, "kk and jt go together");
   if ((w || tau) && !jt) return set_error(SSQB_E_ARG, "w and tau need the target planes");
   if (!(gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
-  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
-  return d->dtype == SSQB_F32
-             ? rs_stft_t<float>(d, twin_host, r, gamma, x, B, Sx, Rx, dSx, Vt, kk, jt, w, tau, st)
-             : rs_stft_t<double>(d, twin_host, r, gamma, x, B, Sx, Rx, dSx, Vt, kk, jt, w, tau, st);
+  return stft_dispatch(d, B, [&](auto t) {
+    return rs_stft_t<decltype(t)>(d, twin_host, r, gamma, x, B, Sx, Rx, dSx, Vt, kk, jt, w, tau, st);
+  });
 }
 
 // ---- multisynchrosqueezed STFT (mssq_kernels.cuh) --------------------------------------------
-// Power-of-two n_fft whose ssq_stft tile and bins fit one CTA: mssq_stft_pow2_kernel.  Every other
-// n_fft: stft_frames_kernel -> Gfft -> mssq_stft_emit_kernel (one CTA per frame), in
-// generic_frames' chunks.
-template <typename T, int EPI>
-static int launch_mssq_stft(const MssqStftArgs<T>& P, cudaStream_t st) {
-  const StftArgs<T>& A = P.A;
-  const long long total = (long long)A.B * A.n_hops;
-  const int logm = ilog2_exact(A.n_fft);
-  if (pow2_tile_fits<T, MssqTile>(logm))
-    return launch_pow2_tile<T, MssqTile>(P, logm, [](auto L) { return mssq_stft_pow2_kernel<T, L, EPI>; }, st);
-  const long long M = A.n_fft;
-  const size_t smem = sizeof(short) * (size_t)(M / 2 + 1);
-  if (smem > kMaxBlockSmem) return set_error(SSQB_E_UNSUPP, "n_fft = %d: the bins of a frame do not fit one CTA", A.n_fft);
-  SSQB_CUDA(opt_in_smem(mssq_stft_emit_kernel<T, EPI>, smem));
-  return generic_frames<T>(A.n_fft, total, 1, -1,
-      [&](cx<T>* c, long long f0, long long nf) {
-        stft_frames_kernel<T, STFT_EPI_PLAIN><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(A, c, f0, nf);
-        SSQB_LAUNCH_CHECK();
-        return 0;
-      },
-      [&](const cx<T>* C, long long f0, long long nf) {
-        mssq_stft_emit_kernel<T, EPI><<<(unsigned)nf, 256, smem, st>>>(P, C, f0);
-        SSQB_LAUNCH_CHECK();
-        return 0;
-      }, st);
-}
-
 template <typename T>
 static int mssq_stft_t(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, int n_iter,
                        const void* x, long long B, void* Sx, void* Tx, void* dSx, int* tgt,
@@ -610,7 +510,7 @@ static int mssq_stft_t(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, int
   P.flipud = A.grid.flipud; A.grid.flipud = 0;                 // the chain works on unflipped bins
   SSQB_CUDA(cudaMemsetAsync(Tx, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(cx<T>), st));
   return dispatch_sx_tgt<MSSQ_EPI_SX, MSSQ_EPI_TGT>(Sx, tgt, [&](auto E) {
-    return launch_mssq_stft<T, E>(P, st);
+    return launch_route<T, MssqStftArgs<T>, E>(P, st);
   });
 }
 
@@ -622,45 +522,13 @@ int run_mssq_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, int n_it
     return set_error(SSQB_E_ARG, "null table");
   if (n_iter < 1 || n_iter > SSQB_MSSQ_MAX_ITER) return set_error(SSQB_E_ARG, "n_iter must be in [1, 64]");
   if (!(r->gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
-  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
-  if (d->n_fft / 2 + 1 > SSQB_MSSQ_MAX_ROWS) return set_error(SSQB_E_UNSUPP, "n_fft must be < 65534");
-  return d->dtype == SSQB_F32 ? mssq_stft_t<float>(d, r, n_iter, x, B, Sx, Tx, dSx, tgt, st)
-                              : mssq_stft_t<double>(d, r, n_iter, x, B, Sx, Tx, dSx, tgt, st);
+  return stft_dispatch(d, B, [&](auto t) {
+    if (d->n_fft / 2 + 1 > SSQB_MSSQ_MAX_ROWS) return set_error(SSQB_E_UNSUPP, "n_fft must be < 65534");
+    return mssq_stft_t<decltype(t)>(d, r, n_iter, x, B, Sx, Tx, dSx, tgt, st);
+  });
 }
 
 // ---- synchroextracting / transient-extracting STFT (extract_kernels.cuh) ----------------------
-// The first order's routes: extract_stft_pow2_kernel for n_fft = 2 .. 4096 (the tile of
-// tssq_stft_pow2_kernel), otherwise stft_frames_kernel -> Gfft -> extract_stft_emit_kernel in
-// generic_frames' chunks.  SET packs g' (ssq_stft's transform), TET packs tau g (tssq_stft's).
-template <typename T, int MODE, int EPI>
-static int launch_extract_stft(const ExtractStftArgs<T>& P, cudaStream_t st) {
-  const StftArgs<T>& A = P.A;
-  const long long total = (long long)A.B * A.n_hops;
-  if (stft_pow2_tile(A.n_fft)) {
-    return dispatch_log2<1, 12>(ilog2_exact(A.n_fft), [&](auto L) {
-      constexpr int M = 1 << L; constexpr int R = Tile<T>::ELEMS / M;
-      const size_t smem = ((size_t)M * (R + 1) + M) * sizeof(cx<T>);
-      auto kern = extract_stft_pow2_kernel<T, L, MODE, EPI>;
-      SSQB_CUDA(opt_in_smem(kern, smem));
-      kern<<<(unsigned)((total + R - 1) / R), Tile<T>::NT, smem, st>>>(P);
-      SSQB_LAUNCH_CHECK();
-      return 0;
-    });
-  }
-  const long long M = A.n_fft, nrows = M / 2 + 1;
-  return generic_frames<T>(A.n_fft, total, 1, -1,
-      [&](cx<T>* c, long long f0, long long nf) {
-        stft_frames_kernel<T, STFT_EPI_PLAIN><<<(unsigned)((nf * M + 255) / 256), 256, 0, st>>>(A, c, f0, nf);
-        SSQB_LAUNCH_CHECK();
-        return 0;
-      },
-      [&](const cx<T>* C, long long f0, long long nf) {
-        extract_stft_emit_kernel<T, MODE, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(P, C, f0, nf);
-        SSQB_LAUNCH_CHECK();
-        return 0;
-      }, st);
-}
-
 template <typename T>
 static int extract_stft_t(const ssqb_stft_desc* d, const void* twin_host,
                           const ssqb_reassign_desc* r, int mode, double gamma, const void* x,
@@ -680,8 +548,8 @@ static int extract_stft_t(const ssqb_stft_desc* d, const void* twin_host,
   }
   A.grid.gamma = gamma;
   return dispatch_sx_tgt<EXTRACT_EPI_SX, EXTRACT_EPI_MASK>(Sx, mask, [&](auto E) {
-    return set ? launch_extract_stft<T, EXTRACT_SET, E>(P, st)
-               : launch_extract_stft<T, EXTRACT_TET, E>(P, st);
+    return set ? launch_route<T, ExtractStftArgs<T>, E>(P, st)
+               : launch_route<T, ExtractStftArgs<T>, E | EXTRACT_EPI_TET>(P, st);
   });
 }
 
@@ -696,10 +564,9 @@ int run_extract_stft(const ssqb_stft_desc* d, const void* twin_host, const ssqb_
   if (mode == EXTRACT_TET && !twin_host)
     return set_error(SSQB_E_ARG, "the transient-extracting mode needs tau g");
   if (!(gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
-  if (d->N < 1 || d->n_fft < 2 || d->hop < 1 || B < 1) return set_error(SSQB_E_ARG, "bad shape");
-  return d->dtype == SSQB_F32
-             ? extract_stft_t<float>(d, twin_host, r, mode, gamma, x, B, Sx, Te, mask, st)
-             : extract_stft_t<double>(d, twin_host, r, mode, gamma, x, B, Sx, Te, mask, st);
+  return stft_dispatch(d, B, [&](auto t) {
+    return extract_stft_t<decltype(t)>(d, twin_host, r, mode, gamma, x, B, Sx, Te, mask, st);
+  });
 }
 
 }  // namespace ssqb

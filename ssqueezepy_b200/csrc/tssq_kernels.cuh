@@ -62,93 +62,30 @@ __device__ __forceinline__ void tssq_point(int form, cx<T> V, cx<T> P, long long
   }
 }
 
-// ---- STFT: one packed transform per frame, c = f g + i kappa f (tau g) --------------------------
-// StftArgs carries the framing with dwin = tau g (unscaled by fs), Sx (may be null), dSx = the
-// V^{tau g} store (when write_dSx), Tx = Ts, grid.gamma = gamma.
-template <typename T>
-struct TssqStftArgs {
-  StftArgs<T> A;
-  int* tgt;                 // [B][n_fft/2+1][n_hops] target columns (TSSQ_EPI_TGT) or null
-  T* tau;                   // same, reassigned time in samples (TSSQ_EPI_TGT) or null
-};
-
+// ---- STFT: the first order's route with tau g in place of g', c = f g + i kappa f (tau g) -------
+// A carries the framing with dwin = tau g (unscaled by fs), Sx (may be null), dSx = the V^{tau g}
+// store (when write_dSx), Tx = Ts, grid.gamma = gamma.
 // bit 0: store Sx; bit 1: write the target planes
 enum { TSSQ_EPI_SX = 1, TSSQ_EPI_TGT = 2 };
 
-template <typename T, int EPI>
-__device__ __forceinline__ void tssq_stft_emit(const TssqStftArgs<T>& P, int b, int k,
-                                               long long frame, cx<T> Ck, cx<T> Cmk) {
-  const StftArgs<T>& A = P.A;
-  const T h = (T)0.5;
-  const cx<T> S  = mkc<T>((Ck.x + Cmk.x) * h, (Ck.y - Cmk.y) * h);
-  const cx<T> St = mkc<T>((Ck.y + Cmk.y) * h * A.inv_kappa, (Cmk.x - Ck.x) * h * A.inv_kappa);
-  const int nrows = A.n_fft / 2 + 1;
-  const long long row = ((long long)b * nrows + k) * A.n_hops;
-  if (EPI & TSSQ_EPI_SX) A.Sx[row + frame] = S;
-  if (A.write_dSx) A.dSx[row + frame] = St;
-  tssq_point<T, (EPI & TSSQ_EPI_TGT) != 0>(FORM_STFT, S, St, frame, A.hop, A.n_hops,
-                                           A.grid.gamma, A.Tx + row, P.tgt, P.tau, row + frame);
-}
+template <typename T>
+struct TssqStftArgs : Stft1Args<T> {
+  int* tgt;                 // [B][n_fft/2+1][n_hops] target columns (TSSQ_EPI_TGT) or null
+  T* tau;                   // same, reassigned time in samples (TSSQ_EPI_TGT) or null
 
-// power-of-two n_fft: the framing and transform of stft_pow2_kernel, the TSST epilogue
-template <typename T, int LOG_M, int EPI>
-__global__ void __launch_bounds__(Tile<T>::NT)
-tssq_stft_pow2_kernel(const TssqStftArgs<T> P) {
-  constexpr int NT = Tile<T>::NT;
-  constexpr int M = 1 << LOG_M;
-  constexpr int R = Tile<T>::ELEMS / M;
-  constexpr int STRIDE = R + 1;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  cx<T>* s = reinterpret_cast<cx<T>*>(smem_raw);          // [M][STRIDE]
-  cx<T>* tw = s + (size_t)M * STRIDE;                     // [M]
-  const StftArgs<T>& A = P.A;
-  const int tid = threadIdx.x;
-  const long long total_frames = (long long)A.B * A.n_hops;
-  const long long f0 = (long long)blockIdx.x * R;
-
-  for (int m = tid; m < M; m += NT) tw[m] = A.tw[m];
-#pragma unroll 1
-  for (int lin = tid; lin < M * R; lin += NT) {
-    const int r = lin % R, l = lin / R;
-    const long long fr = f0 + r;
-    cx<T> z = mkc<T>((T)0, (T)0);
-    if (fr < total_frames) {
-      const int b = (int)(fr / A.n_hops);
-      const long long i = fr - (long long)b * A.n_hops;
-      const long long src = pad_src_index(frame_src(l, i, A.hop, M, A.modulated), A.n1, A.N, A.padtype);
-      const T v = (src >= 0) ? A.x[(long long)b * A.N + src] : (T)0;
-      z = mkc<T>(v * A.win[l], -(v * A.dwin[l]) * A.kappa);  // conj(c)
-    }
-    s[l * STRIDE + r] = z;
+  template <int EPI, class Bins>
+  __device__ __forceinline__ void emit(int b, int k, long long frame, const Bins& C, int mk) const {
+    const StftArgs<T>& A = this->A;
+    cx<T> S, St;
+    hermitian_split<T>(C(0, k), C(0, mk), A.inv_kappa, S, St);
+    const int nrows = A.n_fft / 2 + 1;
+    const long long row = ((long long)b * nrows + k) * A.n_hops;
+    if (EPI & TSSQ_EPI_SX) A.Sx[row + frame] = S;
+    if (A.write_dSx) A.dSx[row + frame] = St;
+    tssq_point<T, (EPI & TSSQ_EPI_TGT) != 0>(FORM_STFT, S, St, frame, A.hop, A.n_hops,
+                                             A.grid.gamma, A.Tx + row, tgt, tau, row + frame);
   }
-  __syncthreads();
-  block_ifft<T, LOG_M, R, NT, STRIDE>(s, tw);
-#pragma unroll 1
-  for (int lin = tid; lin < (M / 2 + 1) * R; lin += NT) {
-    const int r = lin % R, k = lin / R;
-    const long long fr = f0 + r;
-    if (fr >= total_frames) continue;
-    const int b = (int)(fr / A.n_hops);
-    const long long i = fr - (long long)b * A.n_hops;
-    tssq_stft_emit<T, EPI>(P, b, k, i, cconj<T>(s[k * STRIDE + r]),
-                           cconj<T>(s[((M - k) & (M - 1)) * STRIDE + r]));
-  }
-}
-
-// any other n_fft: the frames come from stft_frames_kernel<T, STFT_EPI_PLAIN> (the same packing),
-// then one batched Gfft, then this epilogue
-template <typename T, int EPI>
-__global__ void __launch_bounds__(256)
-tssq_stft_emit_kernel(const TssqStftArgs<T> P, const cx<T>* __restrict__ C, long long f0, long long nf) {
-  const int M = P.A.n_fft, nrows = M / 2 + 1;
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= nf * nrows) return;
-  const int k = (int)(idx / nf); const long long fl = idx - (long long)k * nf;   // frames fastest
-  const long long fr = f0 + fl;
-  const int b = (int)(fr / P.A.n_hops);
-  const long long i = fr - (long long)b * P.A.n_hops;
-  tssq_stft_emit<T, EPI>(P, b, k, i, C[fl * M + k], C[fl * M + (k ? M - k : 0)]);
-}
+};
 
 // ---- CWT: one thread per point of the [rows][ncols] planes W, A (rows = B * na) ---------------
 template <typename T, bool TGT>

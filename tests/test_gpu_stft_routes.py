@@ -1,12 +1,12 @@
 # -*- coding: utf-8 -*-
 """stft, ssq_stft and istft on every transform route, against float64 references.
 
-`stft` / `ssq_stft` choose their kernels by n_fft and dtype (stft_ops.cu:173-178):
-  n_fft = 2^L, L = 1 .. 12   one `stft_pow2_kernel<T, L, EPI>` launch, TILE / n_fft frames per
-                             CTA (stft_ops.cu:44-66; TILE = 8192 float32, 4096 float64,
-                             cwt_kernels.cuh:25-26)
+`stft` / `ssq_stft` choose their kernels by n_fft and dtype (`launch_route` in stft_ops.cu):
+  n_fft = 2^L, L = 1 .. 12   one `stft_tile_kernel<T, Stft1Args<T>, L, EPI>` launch, TILE / n_fft
+                             frames per CTA (`StftTile` in stft_kernels.cuh; TILE = 8192 float32,
+                             4096 float64, cwt_kernels.cuh:25-26)
   any other n_fft            frames -> generic-length FFT `Gfft` -> epilogue, in chunks of
-                             2^27 bytes of complex frames (stft_ops.cu:79-103).  Gfft is kind 0
+                             2^27 bytes of complex frames (`generic_frames`).  Gfft is kind 0
                              (shared-memory Stockham, n <= 4096, prime factors <= 31), kind 1
                              (two passes n = n1 n2) or kind 2 (Bluestein over a kind-0 or kind-1
                              power of two, in chunks of 2^28 bytes) (cwt_generic.cuh:27-122)
@@ -106,7 +106,7 @@ def _frame_chunk(n_fft, frames, dtype):
 def _stft_launches(n_fft, frames, dtype):
     """(launches of one stft / fused ssq_stft call, route name)."""
     if _is_pow2_tile(n_fft, dtype):
-        return 1, 'stft_pow2_kernel LOG_M=%d' % (n_fft.bit_length() - 1)
+        return 1, 'stft_tile_kernel LOG_M=%d' % (n_fft.bit_length() - 1)
     chunk = _frame_chunk(n_fft, frames, dtype)
     n = 0
     for f0 in range(0, frames, chunk):             # frames + Gfft + emit per chunk
