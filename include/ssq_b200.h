@@ -300,6 +300,40 @@ int ssqb_tssq_backward(int dtype, int form, const void* V_dev, const void* P_dev
                        const void* gTs_dev, const void* gV_dev, void* gVout_dev, int64_t B,
                        int nrows, int64_t n_cols, int64_t hop, double gamma, void* stream);
 
+/* ---- time-reassigned multisynchrosqueezing (TMSST; Yu, Lin, Wang & Li, IEEE Trans. Ind.
+ * Electron. 2021; not in the reference) -- the tssq_* reassignment applied again at the column
+ * where the previous step put the coefficient.  jt(k, j) is the ssqb_tssq_* target column and
+ * kept(k, j) its test (|V| > gamma, finite delay, 0 <= jt < n_cols).  For a kept point (k, j):
+ *   c = jt(k, j); up to n_iter - 1 times: stop if not kept(k, c); c = jt(k, c).
+ *   Ts[k][c] += V[k][j]                                            (no weight)
+ * A chain never leaves its row or [0, n_cols); n_iter = 1 gives the tssq_* targets bit for bit,
+ * and the kept set does not depend on n_iter.  1 <= n_iter <= 64.  With hop > 1 the chain walks
+ * the decimated columns.  Ts is zeroed here; its sums use atomics (the order of additions into
+ * one entry is not fixed).  Optional target planes: tgt_dev int32 (final column, -1 = dropped)
+ * and, with it, tau_dev in the data dtype (c_prev hop + delay(k, c_prev) in samples, the time of
+ * the last step taken, inf where tgt is -1).
+ * Scratch is the caller's: t1_dev, an int32 plane of the shape of Ts, receives the first-step
+ * targets; it is read by the second pass, so it must stay untouched until the call's kernels end
+ * (stream order).                                                                              */
+/* STFT: d and twin_host as for ssqb_tssq_stft_exec.  Sx_dev [B][n_fft/2+1][n_hops] is required
+ * and receives V (tssq_stft's bits on the power-of-two route; pass scratch when V is not kept);
+ * Vt_dev receives V^{tau g} when not NULL and is required with tau_dev.                       */
+int ssqb_tmssq_stft_exec(const ssqb_stft_desc* d, const void* twin_host, double gamma, int n_iter,
+                         const void* x_dev, int64_t B, void* Sx_dev, void* Ts_dev,
+                         int32_t* tgt_dev, void* tau_dev, void* Vt_dev, int32_t* t1_dev,
+                         void* stream);
+/* CWT: W_dev, A_dev [B][na][n_cols] complex as for ssqb_tssq_cwt_reassign; Ts_dev, the target
+ * planes and t1_dev the same shape.                                                            */
+int ssqb_tmssq_cwt_reassign(int dtype, const void* W_dev, const void* A_dev, int64_t B, int na,
+                            int64_t n_cols, int64_t hop, double gamma, int n_iter, void* Ts_dev,
+                            int32_t* tgt_dev, void* tau_dev, int32_t* t1_dev, void* stream);
+/* backward of both (torch.autograd), final targets held: gVout = gV + gTs[k][fin] where
+ * fin_dev >= 0 (the forward's tgt plane), gV elsewhere (gV_dev may be NULL = 0 and may alias
+ * gVout_dev).  One thread per point, no atomics.  Planes [B][nrows][n_cols].                   */
+int ssqb_tmssq_backward(int dtype, const int32_t* fin_dev, const void* gTs_dev,
+                        const void* gV_dev, void* gVout_dev, int64_t B, int nrows, int64_t n_cols,
+                        void* stream);
+
 /* ---- reassigned spectrogram / scalogram (Auger & Flandrin, IEEE TSP 1995; not in the
  * reference) -- the energy of every point moves in time and frequency at once:
  *   Rx[kk][jt] += |V[k][j]|^2        (real plane of the data dtype, the shape of Tx)

@@ -17,6 +17,7 @@ from ._ssq_stft import ssq_stft, issq_stft, phase_stft
 from ._tssq import tssq_stft, tssq_cwt
 from ._reassigned import reassigned_stft, reassigned_cwt
 from ._mssq import mssq_stft, mssq_cwt
+from ._tmssq import tmssq_stft, tmssq_cwt
 from ._extract import (synchroextract_stft, transient_extract_stft, synchroextract_cwt,
                        transient_extract_cwt, isynchroextract_stft, isynchroextract_cwt)
 from .ssqueezing import ssqueeze

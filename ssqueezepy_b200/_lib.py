@@ -39,6 +39,7 @@ SYMBOLS = [
     'ssqb_rs_stft_exec', 'ssqb_rs_cwt_reassign', 'ssqb_rs_backward',
     'ssqb_mssq_stft_exec', 'ssqb_mssq_cwt_reassign', 'ssqb_mssq_backward',
     'ssqb_extract_stft_exec', 'ssqb_extract_cwt', 'ssqb_extract_backward',
+    'ssqb_tmssq_stft_exec', 'ssqb_tmssq_cwt_reassign', 'ssqb_tmssq_backward',
 ]
 
 
@@ -150,6 +151,11 @@ def _bind(lib):
     lib.ssqb_extract_cwt.argtypes = [ci, ci, vp, vp, C.POINTER(ReassignDesc), vp, i64, ci, i64,
                                      i64, dbl, vp, vp, vp]
     lib.ssqb_extract_backward.argtypes = [ci, vp, vp, vp, vp, i64, vp]
+    lib.ssqb_tmssq_stft_exec.argtypes = [C.POINTER(StftDesc), vp, dbl, ci, vp, i64, vp, vp, vp,
+                                         vp, vp, vp, vp]
+    lib.ssqb_tmssq_cwt_reassign.argtypes = [ci, vp, vp, i64, ci, i64, i64, dbl, ci, vp, vp, vp,
+                                            vp, vp]
+    lib.ssqb_tmssq_backward.argtypes = [ci, vp, vp, vp, vp, i64, ci, i64, vp]
     lib.ssqb_colsum_real.argtypes = [ci, ci, vp, i64, ci, i64, C.POINTER(dbl), dbl, ci, vp, vp]
     lib.ssqb_invert_components.argtypes = [ci, vp, ci, i64, vp, vp, ci, dbl, vp, vp]
     lib.ssqb_istft_exec.argtypes = [C.POINTER(IstftDesc), vp, i64, vp, vp]

@@ -317,6 +317,25 @@ int ssqb_tssq_backward(int dtype, int form, const void* V, const void* P, const 
                            (cudaStream_t)stream);
 }
 
+int ssqb_tmssq_stft_exec(const ssqb_stft_desc* d, const void* twin_host, double gamma, int n_iter,
+                         const void* x, int64_t B, void* Sx, void* Ts, int32_t* tgt, void* tau,
+                         void* Vt, int32_t* t1, void* stream) {
+  return run_tmssq_stft(d, twin_host, gamma, n_iter, x, B, Sx, Ts, tgt, tau, Vt, t1,
+                        (cudaStream_t)stream);
+}
+
+int ssqb_tmssq_cwt_reassign(int dtype, const void* W, const void* A, int64_t B, int na,
+                            int64_t n_cols, int64_t hop, double gamma, int n_iter, void* Ts,
+                            int32_t* tgt, void* tau, int32_t* t1, void* stream) {
+  return run_tmssq_cwt(dtype, W, A, B, na, n_cols, hop, gamma, n_iter, Ts, tgt, tau, t1,
+                       (cudaStream_t)stream);
+}
+
+int ssqb_tmssq_backward(int dtype, const int32_t* fin, const void* gTs, const void* gV,
+                        void* gVout, int64_t B, int nrows, int64_t n_cols, void* stream) {
+  return run_tmssq_backward(dtype, fin, gTs, gV, gVout, B, nrows, n_cols, (cudaStream_t)stream);
+}
+
 int ssqb_rs_stft_exec(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reassign_desc* r,
                       double gamma, const void* x, int64_t B, void* Sx, void* Rx, void* dSx,
                       void* Vt, int32_t* kk, int32_t* jt, void* w, void* tau, void* stream) {

@@ -276,6 +276,18 @@ int run_extract_cwt(int dtype, int mode, const void* W, const void* P, const ssq
                     double gamma, void* Te, unsigned char* mask, cudaStream_t st);
 int run_extract_backward(int dtype, const unsigned char* mask, const void* gTe, const void* gV,
                          void* gVout, long long total, cudaStream_t st);
+// time-reassigned multisynchrosqueezing (stft_ops.cu, tmssq_ops.cu)
+int run_tmssq_stft(const ssqb_stft_desc* d, const void* twin_host, double gamma, int n_iter,
+                   const void* x, long long B, void* Sx, void* Ts, int* tgt, void* tau, void* Vt,
+                   int* t1, cudaStream_t st);
+int run_tmssq_cwt(int dtype, const void* W, const void* Ap, long long B, int na, long long ncols,
+                  long long hop, double gamma, int n_iter, void* Ts, int* tgt, void* tau, int* t1,
+                  cudaStream_t st);
+int run_tmssq_chain(int dtype, int form, const void* V, const void* P, const int* t1, void* Ts,
+                    int* tgt, void* tau, long long total, long long ncols, long long hop,
+                    int n_iter, cudaStream_t st);
+int run_tmssq_backward(int dtype, const int* fin, const void* gTs, const void* gV, void* gVout,
+                       long long B, int nrows, long long ncols, cudaStream_t st);
 int run_istft_backward(const ssqb_istft_desc* d, const void* gx, long long B, void* gSx,
                        cudaStream_t st);
 // inverse_ops.cu

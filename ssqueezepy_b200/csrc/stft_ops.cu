@@ -2,6 +2,7 @@
 #include "host_common.h"
 #include "stft_kernels.cuh"
 #include "tssq_kernels.cuh"
+#include "tmssq_kernels.cuh"
 #include "rs_kernels.cuh"
 #include "mssq_kernels.cuh"
 #include "extract_kernels.cuh"
@@ -455,6 +456,40 @@ int run_tssq_stft(const ssqb_stft_desc* d, const void* twin_host, double gamma, 
   if (!(gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
   return stft_dispatch(d, B, [&](auto t) {
     return tssq_stft_t<decltype(t)>(d, twin_host, gamma, x, B, Sx, Ts, Vt, tgt, tau, st);
+  });
+}
+
+// ---- time-reassigned multisynchrosqueezed STFT (tmssq_kernels.cuh) ---------------------------
+// First pass: tssq_stft's packing in the shared tile (or frames -> Gfft -> emit), storing V into
+// Sx, V^{tau g} into Vt when given and the first-step targets into t1.  Second pass: the chains.
+template <typename T>
+static int tmssq_stft_t(const ssqb_stft_desc* d, const void* twin_host, double gamma, int n_iter,
+                        const void* x, long long B, void* Sx, void* Ts, int* tgt, void* tau,
+                        void* Vt, int* t1, cudaStream_t st) {
+  TmssqStftArgs<T> P;
+  memset(&P, 0, sizeof(P));
+  StftArgs<T>& A = P.A;
+  stft_args(A, d, x, B, Sx, Vt, Ts, d->win_host, twin_host);     // g + i kappa tau g
+  A.grid.gamma = gamma;
+  P.t1 = t1;
+  int rc = stft_tables(A, d, twin_host, nullptr, false, st); if (rc) return rc;
+  rc = launch_route<T, TmssqStftArgs<T>, 0>(P, st); if (rc) return rc;
+  const long long total = B * (long long)(d->n_fft / 2 + 1) * A.n_hops;
+  return run_tmssq_chain(d->dtype, FORM_STFT, Sx, Vt, t1, Ts, tgt, tau, total, A.n_hops, d->hop,
+                         n_iter, st);
+}
+
+int run_tmssq_stft(const ssqb_stft_desc* d, const void* twin_host, double gamma, int n_iter,
+                   const void* x, long long B, void* Sx, void* Ts, int* tgt, void* tau, void* Vt,
+                   int* t1, cudaStream_t st) {
+  if (!d || !x || !Sx || !Ts || !t1) return set_error(SSQB_E_ARG, "null pointer");
+  if (!d->win_host || !twin_host) return set_error(SSQB_E_ARG, "null table");
+  if (tau && !tgt) return set_error(SSQB_E_ARG, "tau needs the target plane");
+  if (tau && !Vt) return set_error(SSQB_E_ARG, "tau needs the V^{tau g} plane");
+  if (n_iter < 1 || n_iter > SSQB_TMSSQ_MAX_ITER) return set_error(SSQB_E_ARG, "n_iter must be in [1, 64]");
+  if (!(gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
+  return stft_dispatch(d, B, [&](auto t) {
+    return tmssq_stft_t<decltype(t)>(d, twin_host, gamma, n_iter, x, B, Sx, Ts, tgt, tau, Vt, t1, st);
   });
 }
 
