@@ -300,6 +300,37 @@ int ssqb_tssq_backward(int dtype, int form, const void* V_dev, const void* P_dev
                        const void* gTs_dev, const void* gV_dev, void* gVout_dev, int64_t B,
                        int nrows, int64_t n_cols, int64_t hop, double gamma, void* stream);
 
+/* ---- second-order time-reassigned synchrosqueezing (not in the reference) -- ssqb_tssq_* with
+ * the delay corrected by the chirp rate phi'' = Nm / D (STFT) or Num / Den (CWT), so that on a
+ * linear chirp a point goes to the time at which the chirp's frequency is its row's:
+ *   STFT  delay2 = (Re(V^{tau g} / V^g) + Re(V^g' D / (V^g Nm))) fs,
+ *         D = V^{tau g} V^g' - V^{tau g'} V^g,  Nm = V^g'' V^g - (V^g')^2
+ *   CWT   delay2 = Im(A / W) + Re((i Om_a W - dW) Den / (Num W)) / dt,
+ *         Den = W^2 + i dt (dW A - W dA),  Num = D2 W - dW^2
+ * in samples.  delay2 is used where |phi''| sig^2 > 0.05 (sig^2 the window's or the row
+ * wavelet's time variance, seconds^2), it is finite and its column rint((j hop + delay2) / hop)
+ * lies in [0, n_cols); otherwise the point takes its first-order column.  The kept set is
+ * ssqb_tssq_*'s (|V| > gamma, finite first-order delay, first-order column inside), so every row
+ * of Ts sums the same coefficients.  Ts is zeroed here and summed with atomics; tgt_dev (int32,
+ * -1 = dropped) and, with it, tau_dev (j hop + the delay taken, samples, inf where dropped) are
+ * optional.  The backward is ssqb_tmssq_backward on the tgt plane.                            */
+/* STFT, fused (modulated frames only): d and t as for ssqb_ssq_stft2_exec; fs the sampling rate
+ * the tables were built with; sig2 = sum tau^2 g^2 / sum g^2 (seconds^2) of the unshifted window.
+ * Sx_dev may be NULL (not stored; ssq_stft2's bits otherwise); spec_dev, when not NULL,
+ * [4][B][n_fft/2+1][n_hops] complex, receives V^g', V^g'', V^{tau g} and V^{tau g'}.         */
+int ssqb_tssq2_stft_exec(const ssqb_stft_desc* d, const ssqb_stft2_tables* t, double fs,
+                         double sig2, double gamma, const void* x_dev, int64_t B, void* Sx_dev,
+                         void* Ts_dev, int32_t* tgt_dev, void* tau_dev, void* spec_dev,
+                         void* stream);
+/* CWT: the five planes of ssqb_ssq_cwt2_reassign, [B][na][n_cols] (the columns j * hop), Ts_dev
+ * the same shape; Om_host [na] the peak of psih(a xi) in rad/s and sig2_host [na] the row
+ * wavelet's time variance in seconds^2 (host float64, copied on the stream).                  */
+int ssqb_tssq2_cwt_reassign(int dtype, const void* W_dev, const void* dW_dev, const void* A_dev,
+                            const void* dA_dev, const void* D2_dev, const double* Om_host,
+                            const double* sig2_host, double dt, int64_t B, int na,
+                            int64_t n_cols, int64_t hop, double gamma, void* Ts_dev,
+                            int32_t* tgt_dev, void* tau_dev, void* stream);
+
 /* ---- time-reassigned multisynchrosqueezing (TMSST; Yu, Lin, Wang & Li, IEEE Trans. Ind.
  * Electron. 2021; not in the reference) -- the tssq_* reassignment applied again at the column
  * where the previous step put the coefficient.  jt(k, j) is the ssqb_tssq_* target column and

@@ -40,6 +40,7 @@ SYMBOLS = [
     'ssqb_mssq_stft_exec', 'ssqb_mssq_cwt_reassign', 'ssqb_mssq_backward',
     'ssqb_extract_stft_exec', 'ssqb_extract_cwt', 'ssqb_extract_backward',
     'ssqb_tmssq_stft_exec', 'ssqb_tmssq_cwt_reassign', 'ssqb_tmssq_backward',
+    'ssqb_tssq2_stft_exec', 'ssqb_tssq2_cwt_reassign',
 ]
 
 
@@ -156,6 +157,10 @@ def _bind(lib):
     lib.ssqb_tmssq_cwt_reassign.argtypes = [ci, vp, vp, i64, ci, i64, i64, dbl, ci, vp, vp, vp,
                                             vp, vp]
     lib.ssqb_tmssq_backward.argtypes = [ci, vp, vp, vp, vp, i64, ci, i64, vp]
+    lib.ssqb_tssq2_stft_exec.argtypes = [C.POINTER(StftDesc), C.POINTER(Stft2Tables), dbl, dbl,
+                                         dbl, vp, i64, vp, vp, vp, vp, vp, vp]
+    lib.ssqb_tssq2_cwt_reassign.argtypes = [ci, vp, vp, vp, vp, vp, vp, vp, dbl, i64, ci, i64,
+                                            i64, dbl, vp, vp, vp, vp]
     lib.ssqb_colsum_real.argtypes = [ci, ci, vp, i64, ci, i64, C.POINTER(dbl), dbl, ci, vp, vp]
     lib.ssqb_invert_components.argtypes = [ci, vp, ci, i64, vp, vp, ci, dbl, vp, vp]
     lib.ssqb_istft_exec.argtypes = [C.POINTER(IstftDesc), vp, i64, vp, vp]

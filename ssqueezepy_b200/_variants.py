@@ -28,6 +28,12 @@ def check_gamma(gamma):
     return float(gamma)
 
 
+def check_tssq_order(tssq_order):
+    if isinstance(tssq_order, bool) or tssq_order not in (1, 2):
+        raise ValueError("`tssq_order` must be 1 or 2 (got %r)" % (tssq_order,))
+    return int(tssq_order)
+
+
 def default_gamma(gamma, dtype):
     return 10 * (EPS64 if dtype == 'float64' else EPS32) if gamma is None else gamma
 

@@ -317,6 +317,22 @@ int ssqb_tssq_backward(int dtype, int form, const void* V, const void* P, const 
                            (cudaStream_t)stream);
 }
 
+int ssqb_tssq2_stft_exec(const ssqb_stft_desc* d, const ssqb_stft2_tables* t, double fs,
+                         double sig2, double gamma, const void* x, int64_t B, void* Sx, void* Ts,
+                         int32_t* tgt, void* tau, void* spec, void* stream) {
+  return run_tssq2_stft(d, t, fs, sig2, gamma, x, B, Sx, Ts, tgt, tau, spec, (cudaStream_t)stream);
+}
+
+int ssqb_tssq2_cwt_reassign(int dtype, const void* W, const void* dW, const void* A,
+                            const void* dA, const void* D2, const double* Om_host,
+                            const double* sig2_host, double dt, int64_t B, int na,
+                            int64_t n_cols, int64_t hop, double gamma, void* Ts, int32_t* tgt,
+                            void* tau, void* stream) {
+  const void* planes[5] = {W, dW, A, dA, D2};
+  return run_tssq2_cwt(dtype, planes, Om_host, sig2_host, dt, B, na, n_cols, hop, gamma, Ts, tgt,
+                       tau, (cudaStream_t)stream);
+}
+
 int ssqb_tmssq_stft_exec(const ssqb_stft_desc* d, const void* twin_host, double gamma, int n_iter,
                          const void* x, int64_t B, void* Sx, void* Ts, int32_t* tgt, void* tau,
                          void* Vt, int32_t* t1, void* stream) {

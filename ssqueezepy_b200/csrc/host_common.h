@@ -245,6 +245,13 @@ int run_tssq_cwt(int dtype, const void* W, const void* Ap, long long B, int na, 
 int run_tssq_backward(int dtype, int form, const void* V, const void* P, const void* gTs,
                       const void* gV, void* gVout, long long B, int nrows, long long ncols,
                       long long hop, double gamma, cudaStream_t st);
+// second-order time-reassigned synchrosqueezing (stft_ops.cu, tssq_ops.cu)
+int run_tssq2_stft(const ssqb_stft_desc* d, const ssqb_stft2_tables* t2, double fs, double sig2,
+                   double gamma, const void* x, long long B, void* Sx, void* Ts, int* tgt,
+                   void* tau, void* spec, cudaStream_t st);
+int run_tssq2_cwt(int dtype, const void* const* planes, const double* Om_host,
+                  const double* sig2_host, double dt, long long B, int na, long long ncols,
+                  long long hop, double gamma, void* Ts, int* tgt, void* tau, cudaStream_t st);
 // reassigned spectrogram / scalogram (stft_ops.cu, rs_ops.cu)
 int run_rs_stft(const ssqb_stft_desc* d, const void* twin_host, const ssqb_reassign_desc* r,
                 double gamma, const void* x, long long B, void* Sx, void* Rx, void* dSx, void* Vt,

@@ -459,6 +459,47 @@ int run_tssq_stft(const ssqb_stft_desc* d, const void* twin_host, double gamma, 
   });
 }
 
+// ---- second-order time-reassigned ssq_stft (tssq_kernels.cuh) --------------------------------
+// The second order's framing, packing and tables (stft2_t), the tssq epilogue variants.
+template <typename T>
+static int tssq2_stft_t(const ssqb_stft_desc* d, const ssqb_stft2_tables* t2, double fs,
+                        double sig2, double gamma, const void* x, long long B, void* Sx, void* Ts,
+                        int* tgt, void* tau, void* spec, cudaStream_t st) {
+  const int nrows = d->n_fft / 2 + 1;
+  Tssq2StftArgs<T> P;
+  memset(&P, 0, sizeof(P));
+  StftArgs<T>& A = P.A;
+  stft_args(A, d, x, B, Sx, nullptr, Ts, d->win_host, d->dwin_host);
+  A.grid.gamma = gamma;
+  P.tgt = tgt; P.tau = (T*)tau; P.spec = (cx<T>*)spec; P.fs = fs; P.sig2 = sig2;
+  const double kap2 = pack_kappa((const T*)t2->twin_host, (const T*)t2->tdwin_host, d->n_fft);
+  P.kappa2 = (T)kap2; P.inv_kappa2 = (T)(1.0 / kap2);
+  const T* extra[3];
+  int rc = stft_tables(A, d, d->dwin_host, nullptr, false, st,
+                       {t2->ddwin_host, t2->twin_host, t2->tdwin_host}, extra);
+  if (rc) return rc;
+  P.ddwin = extra[0]; P.twin = extra[1]; P.tdwin = extra[2];
+  SSQB_CUDA(cudaMemsetAsync(Ts, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(cx<T>), st));
+  return dispatch_sx_tgt<TSSQ_EPI_SX, TSSQ_EPI_TGT>(Sx, tgt, [&](auto E) {
+    return launch_route<T, Tssq2StftArgs<T>, E>(P, st);
+  });
+}
+
+int run_tssq2_stft(const ssqb_stft_desc* d, const ssqb_stft2_tables* t2, double fs, double sig2,
+                   double gamma, const void* x, long long B, void* Sx, void* Ts, int* tgt,
+                   void* tau, void* spec, cudaStream_t st) {
+  if (!d || !t2 || !x || !Ts) return set_error(SSQB_E_ARG, "null pointer");
+  if (!d->win_host || !d->dwin_host || !t2->ddwin_host || !t2->twin_host || !t2->tdwin_host)
+    return set_error(SSQB_E_ARG, "null table");
+  if (tau && !tgt) return set_error(SSQB_E_ARG, "tau needs the target plane");
+  if (!(gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
+  if (!(fs > 0) || !(sig2 >= 0)) return set_error(SSQB_E_ARG, "fs must be > 0 and sig2 >= 0");
+  if (!d->modulated) return set_error(SSQB_E_UNSUPP, "second-order tssq_stft needs modulated frames");
+  return stft_dispatch(d, B, [&](auto t) {
+    return tssq2_stft_t<decltype(t)>(d, t2, fs, sig2, gamma, x, B, Sx, Ts, tgt, tau, spec, st);
+  });
+}
+
 // ---- time-reassigned multisynchrosqueezed STFT (tmssq_kernels.cuh) ---------------------------
 // First pass: tssq_stft's packing in the shared tile (or frames -> Gfft -> emit), storing V into
 // Sx, V^{tau g} into Vt when given and the first-step targets into t1.  Second pass: the chains.
