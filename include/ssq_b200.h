@@ -331,6 +331,36 @@ int ssqb_tssq2_cwt_reassign(int dtype, const void* W_dev, const void* dW_dev, co
                             int64_t n_cols, int64_t hop, double gamma, void* Ts_dev,
                             int32_t* tgt_dev, void* tau_dev, void* stream);
 
+/* ---- multitapered synchrosqueezing, ConceFT (Daubechies, Wang & Wu, Phil. Trans. R. Soc. A
+ * 374, 2016; not in the reference) -- K orthonormal windows g_j give K pairs (V_j, dV_j) per
+ * point; each of R draws c_r (complex [K]) synchrosqueezes the combined window sum_j c_rj g_j:
+ *   V_r = sum_j c_rj V_j, dV_r = sum_j c_rj dV_j  (float64, j ascending, one rounding per op)
+ *   kept where |V_r| > gamma; bin = the first-order bin of (V_r, dV_r) in float64 on r's grid
+ *   (flip included): w = |Sfs[k] - ratio| (STFT) or |ratio| (CWT)
+ *   Cx[bin][j] += |V_r| cst[k] / R                                  (Cx real, the data dtype)
+ * 1 <= K <= 8 and 1 <= R <= 256; coefs_host is [R][K] complex128 (re, im interleaved), every row
+ * finite and non-zero.                                                                         */
+/* STFT: modulated frames only.  d as for ssqb_ssq_stft_exec (win_host / dwin_host unused);
+ * wins_host [2K][n_fft] in the data dtype holds g_j at row j and g_j' (times fs) at row K + j,
+ * laid out like d->win_host / d->dwin_host (ifftshifted); r gives the grid, gamma and cst.
+ * Cx_dev [B][n_fft/2+1][n_hops].  Where the power-of-two tile fits one CTA, each CTA sums its
+ * frames' columns in shared memory and stores them once; otherwise Cx is zeroed here and summed
+ * with atomics.  Either way the order of additions into one entry is not fixed.  spec_dev, when
+ * not NULL, [2K][B][n_fft/2+1][n_hops] complex, receives V_j at plane j and dV_j at K + j;
+ * bins_dev, when not NULL, [R][B][n_fft/2+1][n_hops] int32, receives every draw's bin (after the
+ * flip; -1 where |V_r| <= gamma).  Both are for tests; pass NULL in normal calls.             */
+int ssqb_conceft_stft_exec(const ssqb_stft_desc* d, const void* wins_host, int K,
+                           const double* coefs_host, int R, const ssqb_reassign_desc* r,
+                           const void* x_dev, int64_t B, void* Cx_dev, void* spec_dev,
+                           int32_t* bins_dev, void* stream);
+/* CWT: planes is a host array of 2K device pointers, W_j at j and dW_j at K + j, each
+ * [B][na][n_cols] complex; r is the fused ssq_cwt's descriptor (grid, gamma, cst [na]).
+ * Cx_dev [B][na][n_cols]: every entry is stored, each by one thread that adds its terms in
+ * ascending (row, draw), so Cx is bit-reproducible and independent of B.  na <= 32767.         */
+int ssqb_conceft_cwt_reassign(int dtype, const void* const* planes, int K,
+                              const double* coefs_host, int R, const ssqb_reassign_desc* r,
+                              int64_t B, int na, int64_t n_cols, void* Cx_dev, void* stream);
+
 /* ---- time-reassigned multisynchrosqueezing (TMSST; Yu, Lin, Wang & Li, IEEE Trans. Ind.
  * Electron. 2021; not in the reference) -- the tssq_* reassignment applied again at the column
  * where the previous step put the coefficient.  jt(k, j) is the ssqb_tssq_* target column and

@@ -41,6 +41,7 @@ SYMBOLS = [
     'ssqb_extract_stft_exec', 'ssqb_extract_cwt', 'ssqb_extract_backward',
     'ssqb_tmssq_stft_exec', 'ssqb_tmssq_cwt_reassign', 'ssqb_tmssq_backward',
     'ssqb_tssq2_stft_exec', 'ssqb_tssq2_cwt_reassign',
+    'ssqb_conceft_stft_exec', 'ssqb_conceft_cwt_reassign',
 ]
 
 
@@ -161,6 +162,10 @@ def _bind(lib):
                                          dbl, vp, i64, vp, vp, vp, vp, vp, vp]
     lib.ssqb_tssq2_cwt_reassign.argtypes = [ci, vp, vp, vp, vp, vp, vp, vp, dbl, i64, ci, i64,
                                             i64, dbl, vp, vp, vp, vp]
+    lib.ssqb_conceft_stft_exec.argtypes = [C.POINTER(StftDesc), vp, ci, vp, ci,
+                                           C.POINTER(ReassignDesc), vp, i64, vp, vp, vp, vp]
+    lib.ssqb_conceft_cwt_reassign.argtypes = [ci, C.POINTER(vp), ci, vp, ci,
+                                              C.POINTER(ReassignDesc), i64, ci, i64, vp, vp]
     lib.ssqb_colsum_real.argtypes = [ci, ci, vp, i64, ci, i64, C.POINTER(dbl), dbl, ci, vp, vp]
     lib.ssqb_invert_components.argtypes = [ci, vp, ci, i64, vp, vp, ci, dbl, vp, vp]
     lib.ssqb_istft_exec.argtypes = [C.POINTER(IstftDesc), vp, i64, vp, vp]

@@ -333,6 +333,21 @@ int ssqb_tssq2_cwt_reassign(int dtype, const void* W, const void* dW, const void
                        tau, (cudaStream_t)stream);
 }
 
+int ssqb_conceft_stft_exec(const ssqb_stft_desc* d, const void* wins_host, int K,
+                           const double* coefs_host, int R, const ssqb_reassign_desc* r,
+                           const void* x, int64_t B, void* Cx, void* spec, int32_t* bins,
+                           void* stream) {
+  return run_conceft_stft(d, wins_host, K, coefs_host, R, r, x, B, Cx, spec, bins,
+                          (cudaStream_t)stream);
+}
+
+int ssqb_conceft_cwt_reassign(int dtype, const void* const* planes, int K, const double* coefs_host,
+                              int R, const ssqb_reassign_desc* r, int64_t B, int na,
+                              int64_t n_cols, void* Cx, void* stream) {
+  return run_conceft_cwt(dtype, planes, K, coefs_host, R, r, B, na, n_cols, Cx,
+                         (cudaStream_t)stream);
+}
+
 int ssqb_tmssq_stft_exec(const ssqb_stft_desc* d, const void* twin_host, double gamma, int n_iter,
                          const void* x, int64_t B, void* Sx, void* Ts, int32_t* tgt, void* tau,
                          void* Vt, int32_t* t1, void* stream) {

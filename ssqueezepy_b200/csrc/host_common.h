@@ -297,6 +297,15 @@ int run_tmssq_backward(int dtype, const int* fin, const void* gTs, const void* g
                        long long B, int nrows, long long ncols, cudaStream_t st);
 int run_istft_backward(const ssqb_istft_desc* d, const void* gx, long long B, void* gSx,
                        cudaStream_t st);
+// multitapered synchrosqueezing, ConceFT (stft_ops.cu, conceft_ops.cu); conceft_check validates
+// K, R and the [R][K] complex draws for both
+int conceft_check(int K, const double* coefs_host, int R);
+int run_conceft_stft(const ssqb_stft_desc* d, const void* wins_host, int K, const double* coefs_host,
+                     int R, const ssqb_reassign_desc* r, const void* x, long long B, void* Cx,
+                     void* spec, int* bins, cudaStream_t st);
+int run_conceft_cwt(int dtype, const void* const* planes, int K, const double* coefs_host, int R,
+                    const ssqb_reassign_desc* r, long long B, int na, long long ncols, void* Cx,
+                    cudaStream_t st);
 // inverse_ops.cu
 int run_colsum_real(int dtype, int wide, const void* M, long long B, int na, long long N,
                     const double* div_host, double scale, int has_scale, void* out,

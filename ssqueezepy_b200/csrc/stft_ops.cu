@@ -6,6 +6,7 @@
 #include "rs_kernels.cuh"
 #include "mssq_kernels.cuh"
 #include "extract_kernels.cuh"
+#include "conceft_kernels.cuh"
 #include "inverse_kernels.cuh"   // IstftArgs, istft_bwd_norm_kernel
 #include "cwt_generic.cuh"      // Gfft<T>: generic-length FFT
 #include <algorithm>
@@ -120,7 +121,8 @@ static int launch_pow2_tile(const Route& P, int logm, KernelOf kernel_of, cudaSt
 // dtypes; the second order and rs up to 4096 in float32, 2048 in float64), otherwise the
 // route's packed frames -> one batched Gfft of SEQ transforms per frame -> its epilogue.  The
 // MSST walks its chains in two passes over the tile's bins: its own tile kernel, and one CTA per
-// frame with the frame's bins in shared memory on the generic route.
+// frame with the frame's bins in shared memory on the generic route.  ConceFT has its own tile
+// kernel too, which sums its frames' Cx columns in shared memory.
 template <typename T, class Route, int EPI>
 static int launch_route(const Route& P, cudaStream_t st) {
   constexpr bool mssq = std::is_same<Route, MssqStftArgs<T>>::value;
@@ -128,6 +130,7 @@ static int launch_route(const Route& P, cudaStream_t st) {
   if (pow2_tile_fits<Route>(logm))
     return launch_pow2_tile<T>(P, logm, [](auto L) {
       if constexpr (mssq) return mssq_stft_pow2_kernel<T, L, EPI>;
+      else if constexpr (is_conceft_stft<Route>::value) return conceft_stft_pow2_kernel<T, Route, L>;
       else return stft_tile_kernel<T, Route, L, EPI>;
     }, st);
   const long long M = P.A.n_fft, nrows = M / 2 + 1;
@@ -642,6 +645,62 @@ int run_extract_stft(const ssqb_stft_desc* d, const void* twin_host, const ssqb_
   if (!(gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
   return stft_dispatch(d, B, [&](auto t) {
     return extract_stft_t<decltype(t)>(d, twin_host, r, mode, gamma, x, B, Sx, Te, mask, st);
+  });
+}
+
+// ---- multitapered synchrosqueezing, ConceFT (conceft_kernels.cuh) -----------------------------
+// K packed transforms per frame in the shared tile (Cx summed per CTA in shared memory and
+// stored once), or frames -> Gfft -> red.add into a zeroed Cx.
+template <typename T, int K>
+static int conceft_stft_t(const ssqb_stft_desc* d, const void* wins_host, const double* coefs_host,
+                          int R, const ssqb_reassign_desc* r, const void* x, long long B, void* Cx,
+                          void* spec, int* bins, cudaStream_t st) {
+  using Route = ConceftStftArgs<T, K>;
+  const int M = d->n_fft, nrows = M / 2 + 1;
+  Route P;
+  memset(&P, 0, sizeof(P));
+  StftArgs<T>& A = P.A;
+  const T* wh = (const T*)wins_host;
+  stft_args(A, d, x, B, nullptr, nullptr, nullptr, wh, wh + (size_t)K * M);
+  A.win = A.dwin = nullptr;                   // host tables: the route packs from P.wins
+  for (int j = 0; j < K; ++j) {
+    const double kap = pack_kappa(wh + (size_t)j * M, wh + (size_t)(K + j) * M, M);
+    P.kappa[j] = (T)kap; P.inv_kappa[j] = (T)(1.0 / kap);
+  }
+  std::vector<double> cw((size_t)nrows);
+  for (int k = 0; k < nrows; ++k) cw[(size_t)k] = r->cst_host[k] / (double)R;
+  BlobBuilder bb;
+  const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
+  const size_t o_sfs = bb.put(d->Sfs_host, sizeof(T) * nrows);
+  const size_t o_win = bb.put(wh, sizeof(T) * 2 * K * (size_t)M);
+  const size_t o_c = bb.put(coefs_host, sizeof(double2) * (size_t)R * K);
+  const size_t o_cw = bb.put(cw.data(), sizeof(double) * nrows);
+  unsigned char* blob = nullptr;
+  int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
+  A.tw = (const cx<T>*)(blob + o_tw); A.Sfs = (const T*)(blob + o_sfs);
+  P.wins = (const T*)(blob + o_win);
+  P.coefs = (const double2*)(blob + o_c); P.cw = (const double*)(blob + o_cw);
+  P.R = R; P.Cx = (T*)Cx; P.spec = (cx<T>*)spec; P.bins = bins;
+  rc = fill_form_grid(r, nrows, FORM_STFT, &A.grid); if (rc) return rc;
+  if (!pow2_tile_fits<Route>(ilog2_exact(M)))
+    SSQB_CUDA(cudaMemsetAsync(Cx, 0, (size_t)B * nrows * (size_t)A.n_hops * sizeof(T), st));
+  return launch_route<T, Route, 0>(P, st);
+}
+
+int run_conceft_stft(const ssqb_stft_desc* d, const void* wins_host, int K, const double* coefs_host,
+                     int R, const ssqb_reassign_desc* r, const void* x, long long B, void* Cx,
+                     void* spec, int* bins, cudaStream_t st) {
+  if (!d || !r || !x || !Cx) return set_error(SSQB_E_ARG, "null pointer");
+  if (!wins_host || !coefs_host || !d->Sfs_host || !r->cst_host)
+    return set_error(SSQB_E_ARG, "null table");
+  int rc = conceft_check(K, coefs_host, R); if (rc) return rc;
+  if (!(r->gamma >= 0)) return set_error(SSQB_E_ARG, "gamma must be >= 0");
+  if (!d->modulated) return set_error(SSQB_E_UNSUPP, "conceft_stft needs modulated frames");
+  return stft_dispatch(d, B, [&](auto t) {
+    return dispatch_log2<1, SSQB_CONCEFT_MAX_K>(K, [&](auto KK) {     // any small int: K here
+      return conceft_stft_t<decltype(t), KK>(d, wins_host, coefs_host, R, r, x, B, Cx, spec, bins,
+                                                   st);
+    });
   });
 }
 
