@@ -160,13 +160,43 @@ def _pack(Tx, Sx, ssq_freqs, Sfs_out, w, dSx, astensor, get_w, get_dWx):
     return Tx, Sx, ssq_freqs, Sfs_out
 
 
+class _Ssq2PlanesFn(torch.autograd.Function):
+    """(Sx, dSx, w) of `ssqb_ssq_stft2_exec` in w-only mode as a differentiable op: the planes
+    are the kernel's own, so the call returns the same Sx and Tx with and without
+    `x.requires_grad` (the separate `stft` differs from them by rounding where its transform
+    route differs, e.g. float64 at n_fft = 4096); the backward is the stft adjoint.  `w` only
+    chooses bins and receives no gradient."""
+
+    @staticmethod
+    def forward(ctx, x2, call, desc):
+        ctx.set_materialize_grads(False)
+        ctx.call = call
+        B = x2.shape[0]
+        Sx, dSx = call.outputs(B, 2)
+        w = torch.empty((B, call.n_rows, call.n_hops), dtype=Bk.real_dtype(call.dtype),
+                        device='cuda')
+        _lib.check(Bk.require_cuda().ssqb_ssq_stft2_exec(
+            C.byref(call.desc), C.byref(call.order2_tables()), C.byref(desc),
+            x2.detach().data_ptr(), B, Sx.data_ptr(), None, dSx.data_ptr(), w.data_ptr(),
+            Bk.stream_ptr()))
+        ctx.mark_non_differentiable(w)
+        return Sx, dSx, w
+
+    @staticmethod
+    def backward(ctx, gS, gdS, gw):
+        if gS is None and gdS is None:
+            return None, None, None
+        B = (gS if gS is not None else gdS).shape[0]
+        return stft_adjoint(ctx.call, gS, gdS, B), None, None
+
+
 def _ssq_stft2_twostep(x, N, window, n_fft, win_len, hop_len, fs, modulated, ssq_freqs,
                        padtype, squeezing, gamma, dtype, astensor, flipud, get_w, get_dWx,
                        get_Sx):
     """Second order, every route but the fused one: the second-order `w` from
-    `ssqb_ssq_stft2_exec` in w-only mode, then `ssqueeze(Sx, w, ...)`.  With `x.requires_grad`,
-    `Sx` comes from the differentiable `stft` and `w` (which only chooses bins) from a detached
-    call, so the gradient is that of `indexed_sum_onfly` with the bins held."""
+    `ssqb_ssq_stft2_exec` in w-only mode, then `ssqueeze(Sx, w, ...)`.  With `x.requires_grad`
+    the same kernel's Sx and dSx are differentiable (`_Ssq2PlanesFn`) and `w` only chooses
+    bins, so the gradient is that of `indexed_sum_onfly` with the bins held."""
     lib = Bk.require_cuda()
     call = _get_call(N, window, n_fft, win_len, hop_len, fs, padtype, modulated, dtype)
     if gamma is None:
@@ -176,17 +206,16 @@ def _ssq_stft2_twostep(x, N, window, n_fft, win_len, hop_len, fs, modulated, ssq
     xd = Bk.to_device(x, call.dtype)
     x2 = xd if xd.ndim == 2 else xd.unsqueeze(0)
     B = x2.shape[0]
-    w = torch.empty((B, call.n_rows, call.n_hops), dtype=Bk.real_dtype(call.dtype), device='cuda')
     if torch.is_tensor(x) and x.requires_grad:
-        Sx, dSx = stft(x, window, n_fft=n_fft, win_len=win_len, hop_len=hop_len, fs=fs,
-                       padtype=padtype, modulated=modulated, derivative=True, dtype=dtype)
-        S_, dS_ = None, None
+        Sx, dSx, w = _Ssq2PlanesFn.apply(x2, call, desc)
     else:
+        w = torch.empty((B, call.n_rows, call.n_hops), dtype=Bk.real_dtype(call.dtype),
+                        device='cuda')
         Sx, dSx = call.outputs(B, 2)
-        S_, dS_ = Sx, (dSx if get_dWx else None)
-    _lib.check(lib.ssqb_ssq_stft2_exec(C.byref(call.desc), C.byref(call.order2_tables()),
-                                       C.byref(desc), x2.detach().data_ptr(), B, Bk.ptr(S_),
-                                       None, Bk.ptr(dS_), w.data_ptr(), Bk.stream_ptr()))
+        _lib.check(lib.ssqb_ssq_stft2_exec(C.byref(call.desc), C.byref(call.order2_tables()),
+                                           C.byref(desc), x2.data_ptr(), B, Sx.data_ptr(), None,
+                                           Bk.ptr(dSx if get_dWx else None), w.data_ptr(),
+                                           Bk.stream_ptr()))
     if x.ndim == 1:
         w = w[0]
         Sx, dSx = (Sx, dSx) if Sx.ndim == 2 else (Sx[0], dSx[0])
