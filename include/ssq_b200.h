@@ -461,6 +461,36 @@ int ssqb_mssq_backward(int dtype, int form, const void* V_dev, const void* dV_de
                        const void* gV_dev, void* gVout_dev, int64_t B, int nrows, int64_t n_cols,
                        void* stream);
 
+/* ---- local maximum synchrosqueezing (LMSST; Yu, Yu, Li & Wang, Mech. Syst. Signal Process.
+ * 2019; not in the reference) -- each kept coefficient moves along its column to the row where
+ * |V| peaks within a window around it.  For a point (a, j) with |V[a][j]| > gamma (r->gamma, the
+ * exact test of ssqb_ssq_stft_exec):
+ *   t(a, j) = the row in [win[a][0], win[a][1]] with the largest |V[t][j]|^2, the lowest on a tie
+ *   Tx[row_bin[t]][j] += cst[a] V[a][j]          (r->cst_host and r->const_wide: the first order's)
+ * |V|^2 = re re + im im in the data dtype, one rounding per operation.  win_host int32 [rows][2]
+ * holds each row's search window (lo <= a <= hi, inside [0, rows)); row_bin_host int32 [rows]
+ * maps a row to a bin of Tx (the first-order bin of the row's frequency on the call's grid, flip
+ * included).  The grid of r is not read.  Every entry of Tx is stored once, by one thread that
+ * adds its sources in ascending row a: Tx needs no zero fill, has no atomics and is
+ * bit-reproducible and independent of the batch and the route.  rows <= 32767.  Optional tgt_dev:
+ * int32 plane with the shape of Tx, t(a, j), -1 where a point is dropped.                      */
+/* STFT, fused: d as for ssqb_stft_exec (the packing of ssq_stft: Sx_dev, when not NULL, holds
+ * ssq_stft's bits on the power-of-two route).  Planes [B][n_fft/2+1][n_hops].                  */
+int ssqb_lmssq_stft_exec(const ssqb_stft_desc* d, const ssqb_reassign_desc* r,
+                         const int32_t* win_host, const int32_t* row_bin_host, const void* x_dev,
+                         int64_t B, void* Sx_dev, void* Tx_dev, int32_t* tgt_dev, void* stream);
+/* CWT: W_dev [B][na][n_cols] complex (any plan, any hop), r the descriptor of the fused ssq_cwt.
+ * B <= 65535.                                                                                   */
+int ssqb_lmssq_cwt_reassign(int dtype, const void* W_dev, const ssqb_reassign_desc* r,
+                            const int32_t* win_host, const int32_t* row_bin_host, int64_t B,
+                            int na, int64_t n_cols, void* Tx_dev, int32_t* tgt_dev, void* stream);
+/* backward of both (torch.autograd), targets held: gVout = gV + cst[a] gTx[row_bin[t]][j] where
+ * tgt_dev (the forward's t plane) is >= 0, gV elsewhere (gV_dev may be NULL = 0 and may alias
+ * gVout_dev).  One thread per point, no atomics.  Planes [B][nrows][n_cols].                   */
+int ssqb_lmssq_backward(int dtype, const int32_t* tgt_dev, const ssqb_reassign_desc* r,
+                        const int32_t* row_bin_host, const void* gTx_dev, const void* gV_dev,
+                        void* gVout_dev, int64_t B, int nrows, int64_t n_cols, void* stream);
+
 /* ---- synchroextracting / transient-extracting transforms (SET: Yu, Wang & Zhao, IEEE Trans.
  * Ind. Electron. 64(10), 2017; TET: Yu, IEEE Trans. Instrum. Meas. 69(2), 2020; not in the
  * reference) -- the transform's own coefficients, kept where the reassignment leaves them:

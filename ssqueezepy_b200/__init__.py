@@ -19,6 +19,7 @@ from ._reassigned import reassigned_stft, reassigned_cwt
 from ._mssq import mssq_stft, mssq_cwt
 from ._tmssq import tmssq_stft, tmssq_cwt
 from ._conceft import conceft_stft, conceft_cwt
+from ._lmssq import lmssq_stft, lmssq_cwt
 from ._extract import (synchroextract_stft, transient_extract_stft, synchroextract_cwt,
                        transient_extract_cwt, isynchroextract_stft, isynchroextract_cwt)
 from .ssqueezing import ssqueeze

@@ -42,6 +42,7 @@ SYMBOLS = [
     'ssqb_tmssq_stft_exec', 'ssqb_tmssq_cwt_reassign', 'ssqb_tmssq_backward',
     'ssqb_tssq2_stft_exec', 'ssqb_tssq2_cwt_reassign',
     'ssqb_conceft_stft_exec', 'ssqb_conceft_cwt_reassign',
+    'ssqb_lmssq_stft_exec', 'ssqb_lmssq_cwt_reassign', 'ssqb_lmssq_backward',
 ]
 
 
@@ -166,6 +167,12 @@ def _bind(lib):
                                            C.POINTER(ReassignDesc), vp, i64, vp, vp, vp, vp]
     lib.ssqb_conceft_cwt_reassign.argtypes = [ci, C.POINTER(vp), ci, vp, ci,
                                               C.POINTER(ReassignDesc), i64, ci, i64, vp, vp]
+    lib.ssqb_lmssq_stft_exec.argtypes = [C.POINTER(StftDesc), C.POINTER(ReassignDesc), vp, vp,
+                                         vp, i64, vp, vp, vp, vp]
+    lib.ssqb_lmssq_cwt_reassign.argtypes = [ci, vp, C.POINTER(ReassignDesc), vp, vp, i64, ci,
+                                            i64, vp, vp, vp]
+    lib.ssqb_lmssq_backward.argtypes = [ci, vp, C.POINTER(ReassignDesc), vp, vp, vp, vp, i64,
+                                        ci, i64, vp]
     lib.ssqb_colsum_real.argtypes = [ci, ci, vp, i64, ci, i64, C.POINTER(dbl), dbl, ci, vp, vp]
     lib.ssqb_invert_components.argtypes = [ci, vp, ci, i64, vp, vp, ci, dbl, vp, vp]
     lib.ssqb_istft_exec.argtypes = [C.POINTER(IstftDesc), vp, i64, vp, vp]

@@ -436,4 +436,24 @@ int ssqb_extract_ridges(int dtype, const void* Tf, int64_t B, int na, int64_t N,
                             (long long*)idx_dev, f_dev, e_dev, (cudaStream_t)stream);
 }
 
+int ssqb_lmssq_stft_exec(const ssqb_stft_desc* d, const ssqb_reassign_desc* r,
+                         const int32_t* win_host, const int32_t* row_bin_host, const void* x,
+                         int64_t B, void* Sx, void* Tx, int32_t* tgt, void* stream) {
+  return run_lmssq_stft(d, r, win_host, row_bin_host, x, B, Sx, Tx, tgt, (cudaStream_t)stream);
+}
+
+int ssqb_lmssq_cwt_reassign(int dtype, const void* W, const ssqb_reassign_desc* r,
+                            const int32_t* win_host, const int32_t* row_bin_host, int64_t B,
+                            int na, int64_t n_cols, void* Tx, int32_t* tgt, void* stream) {
+  return run_lmssq_cwt(dtype, W, r, win_host, row_bin_host, B, na, n_cols, Tx, tgt,
+                       (cudaStream_t)stream);
+}
+
+int ssqb_lmssq_backward(int dtype, const int32_t* tgt, const ssqb_reassign_desc* r,
+                        const int32_t* row_bin_host, const void* gTx, const void* gV, void* gVout,
+                        int64_t B, int nrows, int64_t n_cols, void* stream) {
+  return run_lmssq_backward(dtype, tgt, r, row_bin_host, gTx, gV, gVout, B, nrows, n_cols,
+                            (cudaStream_t)stream);
+}
+
 }  // extern "C"

@@ -306,6 +306,16 @@ int run_conceft_stft(const ssqb_stft_desc* d, const void* wins_host, int K, cons
 int run_conceft_cwt(int dtype, const void* const* planes, int K, const double* coefs_host, int R,
                     const ssqb_reassign_desc* r, long long B, int na, long long ncols, void* Cx,
                     cudaStream_t st);
+// local maximum synchrosqueezing (stft_ops.cu, lmssq_ops.cu)
+int run_lmssq_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const int* win_host,
+                   const int* rb_host, const void* x, long long B, void* Sx, void* Tx, int* tgt,
+                   cudaStream_t st);
+int run_lmssq_cwt(int dtype, const void* W, const ssqb_reassign_desc* r, const int* win_host,
+                  const int* rb_host, long long B, int na, long long ncols, void* Tx, int* tgt,
+                  cudaStream_t st);
+int run_lmssq_backward(int dtype, const int* tgt, const ssqb_reassign_desc* r, const int* rb_host,
+                       const void* gTx, const void* gV, void* gVout, long long B, int nrows,
+                       long long ncols, cudaStream_t st);
 // inverse_ops.cu
 int run_colsum_real(int dtype, int wide, const void* M, long long B, int na, long long N,
                     const double* div_host, double scale, int has_scale, void* out,

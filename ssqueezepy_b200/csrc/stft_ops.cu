@@ -7,6 +7,7 @@
 #include "mssq_kernels.cuh"
 #include "extract_kernels.cuh"
 #include "conceft_kernels.cuh"
+#include "lmssq_kernels.cuh"
 #include "inverse_kernels.cuh"   // IstftArgs, istft_bwd_norm_kernel
 #include "cwt_generic.cuh"      // Gfft<T>: generic-length FFT
 #include <algorithm>
@@ -122,22 +123,28 @@ static int launch_pow2_tile(const Route& P, int logm, KernelOf kernel_of, cudaSt
 // route's packed frames -> one batched Gfft of SEQ transforms per frame -> its epilogue.  The
 // MSST walks its chains in two passes over the tile's bins: its own tile kernel, and one CTA per
 // frame with the frame's bins in shared memory on the generic route.  ConceFT has its own tile
-// kernel too, which sums its frames' Cx columns in shared memory.
+// kernel too, which sums its frames' Cx columns in shared memory.  The LMSST gathers each frame's
+// Tx column in three passes over the frame's V and target bins, in the tile and, on the generic
+// route, in one CTA per frame.
 template <typename T, class Route, int EPI>
 static int launch_route(const Route& P, cudaStream_t st) {
   constexpr bool mssq = std::is_same<Route, MssqStftArgs<T>>::value;
+  constexpr bool lmssq = std::is_same<Route, LmssqStftArgs<T>>::value;
   const int logm = ilog2_exact(P.A.n_fft);
   if (pow2_tile_fits<Route>(logm))
     return launch_pow2_tile<T>(P, logm, [](auto L) {
       if constexpr (mssq) return mssq_stft_pow2_kernel<T, L, EPI>;
+      else if constexpr (lmssq) return lmssq_stft_pow2_kernel<T, L, EPI>;
       else if constexpr (is_conceft_stft<Route>::value) return conceft_stft_pow2_kernel<T, Route, L>;
       else return stft_tile_kernel<T, Route, L, EPI>;
     }, st);
   const long long M = P.A.n_fft, nrows = M / 2 + 1;
-  const size_t smem = mssq ? sizeof(short) * (size_t)nrows : 0;
-  if constexpr (mssq) {
+  const size_t smem = mssq ? sizeof(short) * (size_t)nrows
+                    : lmssq ? (sizeof(cx<T>) + sizeof(short)) * (size_t)nrows : 0;
+  if constexpr (mssq || lmssq) {
     if (smem > kMaxBlockSmem) return set_error(SSQB_E_UNSUPP, "n_fft = %d: the bins of a frame do not fit one CTA", P.A.n_fft);
-    SSQB_CUDA(opt_in_smem(mssq_stft_emit_kernel<T, EPI>, smem));
+    if constexpr (mssq) SSQB_CUDA(opt_in_smem(mssq_stft_emit_kernel<T, EPI>, smem));
+    else SSQB_CUDA(opt_in_smem(lmssq_stft_emit_kernel<T, EPI>, smem));
   }
   return generic_frames<T>(P.A.n_fft, (long long)P.A.B * P.A.n_hops, Route::SEQ, -1,
       [&](cx<T>* c, long long f0, long long nf) {
@@ -149,6 +156,7 @@ static int launch_route(const Route& P, cudaStream_t st) {
       },
       [&](const cx<T>* C, long long f0, long long nf) {
         if constexpr (mssq) mssq_stft_emit_kernel<T, EPI><<<(unsigned)nf, 256, smem, st>>>(P, C, f0);
+        else if constexpr (lmssq) lmssq_stft_emit_kernel<T, EPI><<<(unsigned)nf, 256, smem, st>>>(P, C, f0);
         else stft_emit_kernel<T, Route, EPI><<<(unsigned)((nf * nrows + 255) / 256), 256, 0, st>>>(P, C, f0, nf);
         SSQB_LAUNCH_CHECK();
         return 0;
@@ -701,6 +709,36 @@ int run_conceft_stft(const ssqb_stft_desc* d, const void* wins_host, int K, cons
       return conceft_stft_t<decltype(t), KK>(d, wins_host, coefs_host, R, r, x, B, Cx, spec, bins,
                                                    st);
     });
+  });
+}
+
+
+// ---- local maximum synchrosqueezed STFT (lmssq_kernels.cuh) -----------------------------------
+// ssq_stft's packing and tables; every entry of Tx (and of tgt, when given) is stored once.
+template <typename T>
+static int lmssq_stft_t(const ssqb_stft_desc* d, const LmTables& L, const void* x, long long B,
+                        void* Sx, void* Tx, int* tgt, cudaStream_t st) {
+  LmssqStftArgs<T> P;
+  memset(&P, 0, sizeof(P));
+  StftArgs<T>& A = P.A;
+  stft_args(A, d, x, B, Sx, nullptr, Tx, d->win_host, d->dwin_host);
+  P.L = L; P.tgt = tgt;
+  int rc = stft_tables(A, d, d->dwin_host, nullptr, false, st); if (rc) return rc;
+  return dispatch_sx_tgt<LMSSQ_EPI_SX, LMSSQ_EPI_TGT>(Sx, tgt, [&](auto E) {
+    return launch_route<T, LmssqStftArgs<T>, E>(P, st);
+  });
+}
+
+int run_lmssq_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const int* win_host,
+                   const int* rb_host, const void* x, long long B, void* Sx, void* Tx, int* tgt,
+                   cudaStream_t st) {
+  if (!d || !x || !Tx) return set_error(SSQB_E_ARG, "null pointer");
+  if (!d->win_host || !d->dwin_host) return set_error(SSQB_E_ARG, "null table");
+  if (d->n_fft < 2) return set_error(SSQB_E_ARG, "bad shape");
+  LmTables L;
+  int rc = lmssq_tables(r, win_host, rb_host, d->n_fft / 2 + 1, st, &L); if (rc) return rc;
+  return stft_dispatch(d, B, [&](auto t) {
+    return lmssq_stft_t<decltype(t)>(d, L, x, B, Sx, Tx, tgt, st);
   });
 }
 
