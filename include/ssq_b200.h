@@ -491,6 +491,36 @@ int ssqb_lmssq_backward(int dtype, const int32_t* tgt_dev, const ssqb_reassign_d
                         const int32_t* row_bin_host, const void* gTx_dev, const void* gV_dev,
                         void* gVout_dev, int64_t B, int nrows, int64_t n_cols, void* stream);
 
+/* ---- adaptive-window synchrosqueezed STFT (Sheu, Hsu, Chou & Wu, Int. J. Data Sci. Anal. 2017;
+ * not in the reference) -- K candidate windows g_0 .. g_{K-1} (1 <= K <= 8) share n_fft, the rows
+ * and Sfs; each frame j is synchrosqueezed with the candidate win_idx[j].  bank_host [2K][n_fft]
+ * in the data dtype holds the windows, then their derivative windows, ifftshifted and scaled as
+ * d->win_host / d->dwin_host of a fixed-window call of each (whose kappa each candidate keeps);
+ * d->win_host and d->dwin_host are not read.  r is the descriptor of the fused ssq_stft (its grid,
+ * flip, weights and gamma).  Modulated frames only.
+ * Selection: T_k = frame j's first-order synchrosqueezed column under g_k (never stored), and with
+ * e = the exponent of its largest |re| or |im| and p = |2^-e T_k[r]|^2, E'_k = sum p and
+ * Q'_k = sum p^alpha (float64, rows ascending).  Over the frames i in [j - span, j + span] that
+ * exist, with m = max e_i,
+ *   H_k(j) = (log2 sum 2^(2 alpha (e_i - m)) Q'_k(i) - alpha log2 sum 2^(2 (e_i - m)) E'_k(i)) / (1 - alpha)
+ * (frames ascending; all-zero columns add nothing) and win_idx[j] = the k of least finite H_k(j),
+ * the lowest on a tie, 0 where none is finite.  H is invariant to the scale of x and finite for
+ * every finite transform.  Every sum has one owner and a fixed order: win_idx_dev int64
+ * [B][n_hops] and H_dev float64 [B][K][n_hops] (may be NULL) are bit-reproducible and the same
+ * batched or one signal at a time.  alpha > 0, alpha != 1; span >= 0.                          */
+int ssqb_adaptive_stft_select(const ssqb_stft_desc* d, const void* bank_host, int K,
+                              const ssqb_reassign_desc* r, double alpha, int span,
+                              const void* x_dev, int64_t B, int64_t* win_idx_dev, double* H_dev,
+                              void* stream);
+/* Squeeze: frame j packs, splits and reassigns with candidate win_idx_dev[j] (each in [0, K),
+ * not checked here) exactly as ssqb_ssq_stft_exec with that window, so column j of Sx holds that
+ * call's bits.  Tx_dev is zeroed here and added with red.add; Sx_dev and dSx_dev are stored when
+ * not NULL.  Planes [B][n_fft/2+1][n_hops].                                                    */
+int ssqb_adaptive_stft_exec(const ssqb_stft_desc* d, const void* bank_host, int K,
+                            const ssqb_reassign_desc* r, const int64_t* win_idx_dev,
+                            const void* x_dev, int64_t B, void* Sx_dev, void* Tx_dev,
+                            void* dSx_dev, void* stream);
+
 /* ---- synchroextracting / transient-extracting transforms (SET: Yu, Wang & Zhao, IEEE Trans.
  * Ind. Electron. 64(10), 2017; TET: Yu, IEEE Trans. Instrum. Meas. 69(2), 2020; not in the
  * reference) -- the transform's own coefficients, kept where the reassignment leaves them:
@@ -543,6 +573,13 @@ int ssqb_colsum_real(int dtype, int wide, const void* M_dev, int64_t B, int na, 
 int ssqb_colsum_real_backward(int dtype, int wide, const void* gout_dev, int64_t B, int na,
                               int64_t N, const double* div_host, double scale, int has_scale,
                               void* gM_dev, void* stream);
+/* ssqb_colsum_real with a per-column scale, the inverse of the adaptive-window ssq_stft:
+ *   out[b][j] = (double)( sum_a Re M[b][a][j] ) * scale_host[sel_dev[b][j]], rounded to the dtype
+ * M_dev [B][na][N] complex dtype, sel_dev int64 [B][N] (each in [0, K), not checked here),
+ * scale_host float64 [K].  Rows are added in ascending order in the real dtype of M.  B <= 65535. */
+int ssqb_colsum_real_select(int dtype, const void* M_dev, int64_t B, int na, int64_t N,
+                            const int64_t* sel_dev, const double* scale_host, int K,
+                            void* out_dev, void* stream);
 /* `_invert_components` (_ssq_cwt.py:380-403): M_dev [na][N]; cc_dev, cw_dev int32 [N][K];
  * out_dev float64 [K+1][N] (components, then the uncovered remainder), times `scale`.  */
 int ssqb_invert_components(int dtype, const void* M_dev, int na, int64_t N,

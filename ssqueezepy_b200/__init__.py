@@ -20,6 +20,7 @@ from ._mssq import mssq_stft, mssq_cwt
 from ._tmssq import tmssq_stft, tmssq_cwt
 from ._conceft import conceft_stft, conceft_cwt
 from ._lmssq import lmssq_stft, lmssq_cwt
+from ._adaptive import adaptive_ssq_stft, iadaptive_ssq_stft
 from ._extract import (synchroextract_stft, transient_extract_stft, synchroextract_cwt,
                        transient_extract_cwt, isynchroextract_stft, isynchroextract_cwt)
 from .ssqueezing import ssqueeze

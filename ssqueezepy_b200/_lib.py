@@ -43,6 +43,7 @@ SYMBOLS = [
     'ssqb_tssq2_stft_exec', 'ssqb_tssq2_cwt_reassign',
     'ssqb_conceft_stft_exec', 'ssqb_conceft_cwt_reassign',
     'ssqb_lmssq_stft_exec', 'ssqb_lmssq_cwt_reassign', 'ssqb_lmssq_backward',
+    'ssqb_adaptive_stft_select', 'ssqb_adaptive_stft_exec', 'ssqb_colsum_real_select',
 ]
 
 
@@ -173,6 +174,11 @@ def _bind(lib):
                                             i64, vp, vp, vp]
     lib.ssqb_lmssq_backward.argtypes = [ci, vp, C.POINTER(ReassignDesc), vp, vp, vp, vp, i64,
                                         ci, i64, vp]
+    lib.ssqb_adaptive_stft_select.argtypes = [C.POINTER(StftDesc), vp, ci, C.POINTER(ReassignDesc),
+                                              dbl, ci, vp, i64, vp, vp, vp]
+    lib.ssqb_adaptive_stft_exec.argtypes = [C.POINTER(StftDesc), vp, ci, C.POINTER(ReassignDesc),
+                                            vp, vp, i64, vp, vp, vp, vp]
+    lib.ssqb_colsum_real_select.argtypes = [ci, vp, i64, ci, i64, vp, C.POINTER(dbl), ci, vp, vp]
     lib.ssqb_colsum_real.argtypes = [ci, ci, vp, i64, ci, i64, C.POINTER(dbl), dbl, ci, vp, vp]
     lib.ssqb_invert_components.argtypes = [ci, vp, ci, i64, vp, vp, ci, dbl, vp, vp]
     lib.ssqb_istft_exec.argtypes = [C.POINTER(IstftDesc), vp, i64, vp, vp]

@@ -456,4 +456,25 @@ int ssqb_lmssq_backward(int dtype, const int32_t* tgt, const ssqb_reassign_desc*
                             (cudaStream_t)stream);
 }
 
+int ssqb_adaptive_stft_select(const ssqb_stft_desc* d, const void* bank_host, int K,
+                              const ssqb_reassign_desc* r, double alpha, int span, const void* x,
+                              int64_t B, int64_t* win_idx, double* H, void* stream) {
+  return run_adaptive_select(d, bank_host, K, r, alpha, span, x, B, (long long*)win_idx, H,
+                             (cudaStream_t)stream);
+}
+
+int ssqb_adaptive_stft_exec(const ssqb_stft_desc* d, const void* bank_host, int K,
+                            const ssqb_reassign_desc* r, const int64_t* win_idx, const void* x,
+                            int64_t B, void* Sx, void* Tx, void* dSx, void* stream) {
+  return run_adaptive_stft(d, bank_host, K, r, (const long long*)win_idx, x, B, Sx, Tx, dSx,
+                           (cudaStream_t)stream);
+}
+
+int ssqb_colsum_real_select(int dtype, const void* M, int64_t B, int na, int64_t N,
+                            const int64_t* sel, const double* scale_host, int K, void* out,
+                            void* stream) {
+  return run_colsum_real_select(dtype, M, B, na, N, (const long long*)sel, scale_host, K, out,
+                                (cudaStream_t)stream);
+}
+
 }  // extern "C"

@@ -90,7 +90,7 @@ struct ConceftStftArgs {
   using Framing = ConceftStftArgs;
 
   template <bool CONJ>
-  __device__ __forceinline__ cx<T> pack(T v, int l, int j) const {
+  __device__ __forceinline__ cx<T> pack(T v, int l, int j, long long) const {
     const int M = A.n_fft;
     return pack_pair<T, CONJ>(v, wins[j * M + l], wins[(K + j) * M + l], kappa[j]);
   }

@@ -316,6 +316,22 @@ int run_lmssq_cwt(int dtype, const void* W, const ssqb_reassign_desc* r, const i
 int run_lmssq_backward(int dtype, const int* tgt, const ssqb_reassign_desc* r, const int* rb_host,
                        const void* gTx, const void* gV, void* gVout, long long B, int nrows,
                        long long ncols, cudaStream_t st);
+// adaptive-window synchrosqueezed STFT (stft_ops.cu, adaptive_ops.cu); adaptive_check validates the
+// tables, K, gamma and the framing for both passes
+int adaptive_check(const ssqb_stft_desc* d, const void* bank_host, int K,
+                   const ssqb_reassign_desc* r);
+int run_adaptive_score(const ssqb_stft_desc* d, const void* bank_host, int K,
+                       const ssqb_reassign_desc* r, double alpha, const void* x, long long B,
+                       double2* eq, int* ex, cudaStream_t st);
+int run_adaptive_select(const ssqb_stft_desc* d, const void* bank_host, int K,
+                        const ssqb_reassign_desc* r, double alpha, int span, const void* x,
+                        long long B, long long* sel, double* H, cudaStream_t st);
+int run_adaptive_stft(const ssqb_stft_desc* d, const void* bank_host, int K,
+                      const ssqb_reassign_desc* r, const long long* sel, const void* x,
+                      long long B, void* Sx, void* Tx, void* dSx, cudaStream_t st);
+int run_colsum_real_select(int dtype, const void* M, long long B, int na, long long N,
+                           const long long* sel, const double* scale_host, int K, void* out,
+                           cudaStream_t st);
 // inverse_ops.cu
 int run_colsum_real(int dtype, int wide, const void* M, long long B, int na, long long N,
                     const double* div_host, double scale, int has_scale, void* out,

@@ -91,7 +91,7 @@ struct RsStftArgs {
   using Framing = RsStftArgs;
 
   template <bool CONJ>
-  __device__ __forceinline__ cx<T> pack(T v, int l, int j) const {
+  __device__ __forceinline__ cx<T> pack(T v, int l, int j, long long) const {
     return j == 0 ? pack_pair<T, CONJ>(v, A.win[l], A.dwin[l], A.kappa) : mkc<T>(v * twin[l], (T)0);
   }
 

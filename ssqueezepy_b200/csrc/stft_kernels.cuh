@@ -74,7 +74,9 @@ __device__ __forceinline__ void hermitian_split(cx<T> Ck, cx<T> Cmk, T inv_kappa
 // ---- routes ---------------------------------------------------------------------------------
 // A route is the argument struct of one STFT variant.  It holds the framing in A and gives the
 // framed-transform tile and the generic-length kernels below two things:
-//   pack<CONJ>(v, l, j)           packed sequence j (of SEQ) at frame sample l, sample value v
+//   pack<CONJ>(v, l, j, fr)       packed sequence j (of SEQ) at frame sample l, sample value v, of
+//                                 frame fr of the flattened batch (read only by the routes whose
+//                                 window changes from frame to frame)
 //   emit<EPI>(b, k, frame, C, mk) the outputs of bin k of the frame, where C(j, k) is bin k of
 //                                 the transform of sequence j and mk is the bin M - k (0 at k = 0)
 // Tile<LOG_M> is its power-of-two tile: F frames per CTA, SMEM bytes.  Routes that frame like the
@@ -91,6 +93,26 @@ template <typename T, int LOG_M> struct StftTile {
 // reassignment into Tx, SSQ_TX is SSQ without the Sx store (the caller asked for Tx only).
 enum { STFT_EPI_PLAIN = 0, STFT_EPI_SSQ = 1, STFT_EPI_SSQ_TX = 3 };
 
+// The first order's outputs of bin k of a frame from bins k and M - k of its packed transform:
+// Sx (unless SSQ_TX), dSx when asked for, and the fused reassignment into Tx
+template <typename T, int EPI>
+__device__ __forceinline__ void ssq1_emit(const StftArgs<T>& A, int b, int k, long long frame,
+                                          cx<T> Ck, cx<T> Cmk, T inv_kappa) {
+  cx<T> S, dS;
+  hermitian_split<T>(Ck, Cmk, inv_kappa, S, dS);
+  const int nrows = A.n_fft / 2 + 1;
+  const long long o = ((long long)b * nrows + k) * A.n_hops + frame;
+  if (EPI != STFT_EPI_SSQ_TX) A.Sx[o] = S;
+  if (A.write_dSx) A.dSx[o] = dS;
+  if ((EPI == STFT_EPI_SSQ || EPI == STFT_EPI_SSQ_TX) && is_active_exact(S.x, S.y, A.grid.gamma)) {
+    double r = phase_ratio_exact<T>(dS.x, dS.y, S.x, S.y);
+    double w = fabs((double)A.Sfs[k] - r);
+    int kk = bin_from_w_exact(w, A.grid);
+    T cc = (T)A.cst[k];
+    atomic_add_cx<T>(&A.Tx[((long long)b * nrows + kk) * A.n_hops + frame], S.x * cc, S.y * cc);
+  }
+}
+
 template <typename T>
 struct Stft1Args {
   StftArgs<T> A;
@@ -99,25 +121,13 @@ struct Stft1Args {
   using Framing = Stft1Args;
 
   template <bool CONJ>
-  __device__ __forceinline__ cx<T> pack(T v, int l, int) const {
+  __device__ __forceinline__ cx<T> pack(T v, int l, int, long long) const {
     return pack_pair<T, CONJ>(v, A.win[l], A.dwin[l], A.kappa);
   }
 
   template <int EPI, class Bins>
   __device__ __forceinline__ void emit(int b, int k, long long frame, const Bins& C, int mk) const {
-    cx<T> S, dS;
-    hermitian_split<T>(C(0, k), C(0, mk), A.inv_kappa, S, dS);
-    const int nrows = A.n_fft / 2 + 1;
-    const long long o = ((long long)b * nrows + k) * A.n_hops + frame;
-    if (EPI != STFT_EPI_SSQ_TX) A.Sx[o] = S;
-    if (A.write_dSx) A.dSx[o] = dS;
-    if ((EPI == STFT_EPI_SSQ || EPI == STFT_EPI_SSQ_TX) && is_active_exact(S.x, S.y, A.grid.gamma)) {
-      double r = phase_ratio_exact<T>(dS.x, dS.y, S.x, S.y);
-      double w = fabs((double)A.Sfs[k] - r);
-      int kk = bin_from_w_exact(w, A.grid);
-      T cc = (T)A.cst[k];
-      atomic_add_cx<T>(&A.Tx[((long long)b * nrows + kk) * A.n_hops + frame], S.x * cc, S.y * cc);
-    }
+    ssq1_emit<T, EPI>(A, b, k, frame, C(0, k), C(0, mk), A.inv_kappa);
   }
 };
 
@@ -131,7 +141,9 @@ struct StftAdjArgs {
   using Framing = StftAdjArgs;
 
   template <bool CONJ>
-  __device__ __forceinline__ cx<T> pack(T v, int l, int) const { return mkc<T>(v * A.win[l], (T)0); }
+  __device__ __forceinline__ cx<T> pack(T v, int l, int, long long) const {
+    return mkc<T>(v * A.win[l], (T)0);
+  }
 
   template <int EPI, class Bins>
   __device__ __forceinline__ void emit(int b, int k, long long frame, const Bins& C, int mk) const {
@@ -182,13 +194,14 @@ __device__ __forceinline__ void frame_tile(const Route& P, cx<T>* s, cx<T>* tw, 
     // halves the occupancy of some second-order instances.
     if constexpr (Route::SEQ == 1) {
       cx<T> z = mkc<T>((T)0, (T)0);
-      if (fr < total_frames) z = P.template pack<true>(frame_sample<T>(A, M, l, fr), l, 0);
+      if (fr < total_frames) z = P.template pack<true>(frame_sample<T>(A, M, l, fr), l, 0, fr);
       s[l * STRIDE + r] = z;
     } else {
       T v = (T)0;
       if (fr < total_frames) v = frame_sample<T>(A, M, l, fr);
 #pragma unroll
-      for (int j = 0; j < Route::SEQ; ++j) s[l * STRIDE + j * F + r] = P.template pack<true>(v, l, j);
+      for (int j = 0; j < Route::SEQ; ++j)
+        s[l * STRIDE + j * F + r] = P.template pack<true>(v, l, j, fr);
     }
   }
   __syncthreads();
@@ -233,7 +246,7 @@ stft_frames_kernel(const Route P, cx<T>* __restrict__ c, long long f0, long long
   const T v = frame_sample<T>(P.A, M, l, f0 + fl);
   cx<T>* cf = c + idx + (Route::SEQ - 1) * fl * M;        // c[SEQ fl][l]
 #pragma unroll
-  for (int j = 0; j < Route::SEQ; ++j) cf[j * M] = P.template pack<false>(v, l, j);
+  for (int j = 0; j < Route::SEQ; ++j) cf[j * M] = P.template pack<false>(v, l, j, f0 + fl);
 }
 template <typename T, class Route, int EPI>
 __global__ void __launch_bounds__(256)
@@ -466,7 +479,7 @@ struct Stft2Args {
   using Framing = Stft2Args;
 
   template <bool CONJ>
-  __device__ __forceinline__ cx<T> pack(T v, int l, int j) const {
+  __device__ __forceinline__ cx<T> pack(T v, int l, int j, long long) const {
     if (j == 0) return pack_pair<T, CONJ>(v, A.win[l], A.dwin[l], A.kappa);
     if (j == 1) return pack_pair<T, CONJ>(v, twin[l], tdwin[l], kappa2);
     return mkc<T>(v * ddwin[l], (T)0);

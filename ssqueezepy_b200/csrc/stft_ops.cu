@@ -8,6 +8,7 @@
 #include "extract_kernels.cuh"
 #include "conceft_kernels.cuh"
 #include "lmssq_kernels.cuh"
+#include "adaptive_kernels.cuh"
 #include "inverse_kernels.cuh"   // IstftArgs, istft_bwd_norm_kernel
 #include "cwt_generic.cuh"      // Gfft<T>: generic-length FFT
 #include <algorithm>
@@ -739,6 +740,116 @@ int run_lmssq_stft(const ssqb_stft_desc* d, const ssqb_reassign_desc* r, const i
   int rc = lmssq_tables(r, win_host, rb_host, d->n_fft / 2 + 1, st, &L); if (rc) return rc;
   return stft_dispatch(d, B, [&](auto t) {
     return lmssq_stft_t<decltype(t)>(d, L, x, B, Sx, Tx, tgt, st);
+  });
+}
+
+// ---- adaptive-window synchrosqueezed STFT (adaptive_kernels.cuh) ------------------------------
+// The route of both passes: the framing of d, the K candidates' windows and derivative windows
+// (bank_host [2K][n_fft], ifftshifted and scaled like d's), each candidate's own kappa, the
+// first-order grid, weights and Sfs
+template <typename T>
+static int adaptive_args(AdaptiveStftArgs<T>& P, const ssqb_stft_desc* d, const void* bank_host,
+                         int K, const ssqb_reassign_desc* r, const void* x, long long B, void* Sx,
+                         void* Tx, void* dSx, cudaStream_t st) {
+  const int M = d->n_fft, nrows = M / 2 + 1;
+  memset(&P, 0, sizeof(P));
+  StftArgs<T>& A = P.A;
+  const T* bank = (const T*)bank_host;
+  stft_args(A, d, x, B, Sx, dSx, Tx, bank, bank + (size_t)K * M);
+  std::vector<T> kap((size_t)2 * K);
+  for (int c = 0; c < K; ++c) {                // pack_kappa as a fixed-window call of g_c takes it
+    const double k = pack_kappa(bank + (size_t)c * M, bank + (size_t)(K + c) * M, M);
+    kap[(size_t)c] = (T)k; kap[(size_t)(K + c)] = (T)(1.0 / k);
+  }
+  BlobBuilder bb;
+  const size_t o_tw = bb.put(stft_roots<T>(M).data(), sizeof(cx<T>) * M);
+  const size_t o_cst = bb.put(r->cst_host, sizeof(double) * nrows);
+  const size_t o_sfs = bb.put(d->Sfs_host, sizeof(T) * nrows);
+  const size_t o_bank = bb.put(bank, sizeof(T) * 2 * (size_t)K * M);
+  const size_t o_kap = bb.put(kap.data(), sizeof(T) * 2 * K);
+  unsigned char* blob = nullptr;
+  int rc = table_blob(bb.h, st, &blob); if (rc) return rc;
+  A.tw = (const cx<T>*)(blob + o_tw); A.cst = (const double*)(blob + o_cst);
+  A.Sfs = (const T*)(blob + o_sfs);
+  P.bank = (const T*)(blob + o_bank); P.kap = (const T*)(blob + o_kap);
+  P.K = K;
+  return fill_form_grid(r, nrows, FORM_STFT, &A.grid);
+}
+
+// pass 1: (E', Q', e) of every candidate and frame into eq / ex [K][B * n_hops]
+template <typename T>
+static int adaptive_score_t(const ssqb_stft_desc* d, const void* bank_host, int K,
+                            const ssqb_reassign_desc* r, double alpha, const void* x, long long B,
+                            double2* eq, int* ex, cudaStream_t st) {
+  AdaptiveScoreArgs<T> P;
+  int rc = adaptive_args<T>(P, d, bank_host, K, r, x, B, nullptr, nullptr, nullptr, st);
+  if (rc) return rc;
+  P.eq = eq; P.ex = ex;
+  const long long M = d->n_fft, nrows = M / 2 + 1, total = (long long)B * P.A.n_hops;
+  const int logm = ilog2_exact(M);
+  if (pow2_tile_fits<AdaptiveScoreArgs<T>>(logm))
+    return dispatch_log2<1, 12>(logm, [&](auto L) {
+      using Tl = AdaptiveScoreTile<T, L>;
+      if constexpr (Tl::SMEM > kMaxBlockSmem) {
+        return set_error(SSQB_E_UNSUPP, "n_fft = 2^%d does not fit one CTA", (int)L);
+      } else {
+        auto kern = adaptive_score_pow2_kernel<T, L>;
+        SSQB_CUDA(opt_in_smem(kern, Tl::SMEM));
+        kern<<<dim3((unsigned)((total + Tl::F - 1) / Tl::F), (unsigned)K), Tile<T>::NT, Tl::SMEM,
+               st>>>(P, alpha);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      }
+    });
+  const size_t smem = (sizeof(double2) + sizeof(cx<T>) + sizeof(short)) * (size_t)nrows;
+  if (smem > kMaxBlockSmem || nrows > 32767)
+    return set_error(SSQB_E_UNSUPP, "n_fft = %d: the bins of a frame do not fit one CTA", d->n_fft);
+  SSQB_CUDA(opt_in_smem(adaptive_score_emit_kernel<T>, smem));
+  return generic_frames<T>(d->n_fft, total, K, -1,
+      [&](cx<T>* c, long long f0, long long nf) {
+        adaptive_score_frames_kernel<T><<<dim3((unsigned)((nf * M + 255) / 256), (unsigned)K), 256,
+                                          0, st>>>(P, c, f0, nf);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      },
+      [&](const cx<T>* C, long long f0, long long nf) {
+        adaptive_score_emit_kernel<T><<<dim3((unsigned)nf, (unsigned)K), 256, smem, st>>>(
+            P, C, f0, nf, alpha);
+        SSQB_LAUNCH_CHECK();
+        return 0;
+      }, st);
+}
+
+int run_adaptive_score(const ssqb_stft_desc* d, const void* bank_host, int K,
+                       const ssqb_reassign_desc* r, double alpha, const void* x, long long B,
+                       double2* eq, int* ex, cudaStream_t st) {
+  return stft_dispatch(d, B, [&](auto t) {
+    return adaptive_score_t<decltype(t)>(d, bank_host, K, r, alpha, x, B, eq, ex, st);
+  });
+}
+
+// pass 2: frame j packs with candidate sel[j] in the shared tile (or frames -> Gfft -> emit)
+template <typename T>
+static int adaptive_stft_t(const ssqb_stft_desc* d, const void* bank_host, int K,
+                           const ssqb_reassign_desc* r, const long long* sel, const void* x,
+                           long long B, void* Sx, void* Tx, void* dSx, cudaStream_t st) {
+  AdaptiveStftArgs<T> P;
+  int rc = adaptive_args<T>(P, d, bank_host, K, r, x, B, Sx, Tx, dSx, st);
+  if (rc) return rc;
+  P.sel = sel;
+  const int nrows = d->n_fft / 2 + 1;
+  SSQB_CUDA(cudaMemsetAsync(Tx, 0, (size_t)B * nrows * (size_t)P.A.n_hops * sizeof(cx<T>), st));
+  return Sx ? launch_route<T, AdaptiveStftArgs<T>, STFT_EPI_SSQ>(P, st)
+            : launch_route<T, AdaptiveStftArgs<T>, STFT_EPI_SSQ_TX>(P, st);
+}
+
+int run_adaptive_stft(const ssqb_stft_desc* d, const void* bank_host, int K,
+                      const ssqb_reassign_desc* r, const long long* sel, const void* x,
+                      long long B, void* Sx, void* Tx, void* dSx, cudaStream_t st) {
+  if (!d || !r || !x || !Tx || !sel) return set_error(SSQB_E_ARG, "null pointer");
+  int rc = adaptive_check(d, bank_host, K, r); if (rc) return rc;
+  return stft_dispatch(d, B, [&](auto t) {
+    return adaptive_stft_t<decltype(t)>(d, bank_host, K, r, sel, x, B, Sx, Tx, dSx, st);
   });
 }
 
